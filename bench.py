@@ -2,11 +2,12 @@
 """bench.py -- matched image-pairs / second on the compute-matches hot path (BASELINE.json metric).
 
     python bench.py [--gpus N --steps K --warmup W] [--impl reference] [--workload c3|c2|c2-msurf64|c4|c4-exact] [--matcher exact|cascade]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 Workload (default): BASELINE.json configs[2] = **C3**, the configuration the north_star target is quoted on:
 200 synthetic images x 20 000 SIFT-128 uint8 descriptors, exhaustive pairs (19 900), brute-force L2 2-NN +
-ratio 0.6 + (i,j) and coordinate de-duplication.  It fits one B200 (0.5 GB of descriptors + 1.4 GB of fp16
+ratio 0.6 + (i,j) and coordinate de-duplication.  It fits one H100 (0.5 GB of descriptors + 1.4 GB of fp16
 operands), so N = 1 runs the whole set.  One step = one pass over ALL 19 900 pairs.
 
 N > 1 = STRONG scaling of that one set: every rank holds the regions its shard touches, the I-sorted pair list
@@ -21,13 +22,16 @@ the step) + the F filter; c4-exact = the same images through the exact tensor-co
 value : pairs/s, descriptors already resident in HBM (r3d_match_pairs on the shard + gather).
 e2e   : pairs/s through the C ABI from pinned HOST buffers: r3d_clear_regions + r3d_upload_regions of every view
         the shard touches + r3d_match_pairs + gather, every step.
-roofline : the tcgen05 candidate kernel, algorithmic 2*N_I*N_J*D flop per pair (SURVEY.md 8d) over its
-        CUDA-event time on its own stream, against MEASURED_PEAKS.json bf16 TFLOP/s.
+roofline : the wgmma candidate kernel, algorithmic 2*N_I*N_J*D flop per pair (SURVEY.md 8d) over its
+        CUDA-event time on its own stream, against MEASURED_PEAKS.json bf16 TFLOP/s when present, else the H100 SXM
+        data-sheet peak (dense fp16 989 TFLOP/s, HBM3 3.35 TB/s).
 cpu_baseline : the oracle port on a bounded sample of the same pairs with all usable host threads (N = 1 only).
 f_filter / ba : the F AC-RANSAC leg over the step's putatives and the C5 bundle adjustment, reported alongside.
 --impl reference : the reference's CPU path (oracle port; the reference itself cannot be built here) on a
         bounded sample of the same workload per step, explicit OMP team = the usable CPUs (torchrun exports
         OMP_NUM_THREADS=1, which is ignored on purpose).
+--dump-outputs DIR : after the timed steps, the putative matches of the last resident step as DIR/*.npy (see
+        dump_outputs); the inputs are seeded, so two builds run with the same arguments can be compared file by file.
 """
 import argparse
 import json
@@ -58,11 +62,11 @@ def load_peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return json.load(open(p)), "measured"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "H100 SXM data-sheet"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
 
     def __init__(self, index):
         self.index = index
@@ -121,8 +125,8 @@ class ClockSampler:
 
 
 def effective_cpus():
-    """Host CPUs this process may actually use: the affinity mask, cut by the cgroup CPU-time quota (the GPU boxes
-    give a container ~16 CPUs of quota per GPU although 128 hardware threads are visible)."""
+    """Host CPUs this process may actually use: the affinity mask, cut by the cgroup CPU-time quota (a container may
+    see far more hardware threads than its quota lets it use)."""
     n = len(os.sched_getaffinity(0)) if hasattr(os, "sched_getaffinity") else (os.cpu_count() or 1)
     try:
         q, per = open("/sys/fs/cgroup/cpu.max").read().split()[:2]
@@ -133,25 +137,44 @@ def effective_cpus():
     return n
 
 
-def measured_traffic_per_pair(wl_key):
-    """DRAM bytes per image pair of the candidate kernel, from the committed `ncu --set full` capture of one
-    batch launch of THIS workload (profiles/*_keymetrics.csv: dram__bytes_read/write + the pairs the launch held);
-    None when no capture of this workload is committed."""
-    name = {"c3": "r02_k_l2_candidates_2sm_c3_keymetrics.csv", "c2": "r01_k_l2_candidates_2sm_keymetrics.csv"}.get(wl_key)
-    if not name:
-        return None, None
-    p = os.path.join(ROOT, "profiles", name)
-    if not os.path.exists(p):
-        return None, None
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    tot, pairs = 0.0, 128.0
-    import csv
-    for f in csv.reader(open(p)):
-        if len(f) >= 4 and f[1] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-            tot += float(f[2]) * unit.get(f[3], 1.0)
-        if len(f) >= 3 and f[1] == "pairs_in_launch":
-            pairs = float(f[2])
-    return (tot / pairs if tot else None), "profiles/" + name
+DUMP_BYTES = 64 << 20
+DUMP_SEED = 20260924
+
+
+def dump_outputs(out_dir, pairs, result, rank):
+    """The matches the timed path returned in its last step, as DIR/<name>.npy (rank 0 only; `result` is the
+    PairWiseMatches map, or with N > 1 the gather that holds every rank's map on rank 0):
+        pairs.npy        [P, 2] float64  the dumped (I, J) pairs, in the order of the input pair list
+        match_counts.npy [P]    float64  matches of each of them (0: absent from the map)
+        matches.npy      [M, 2] float32  (i, j) of every match of those pairs, pair after pair, in the map's order
+    Every pair of the list is dumped while the matches fit DUMP_BYTES; beyond that a fixed seeded sample of the pair
+    list, halved until they fit."""
+    if rank != 0:
+        return
+    if hasattr(result, "result"):
+        parts = result.result()
+        pp = np.concatenate([p[0] for p in parts], 0)
+        ofs = [p[1].astype(np.int64) for p in parts]
+        mm = [p[2] for p in parts]
+        found = {}
+        for r, (pr, _, _) in enumerate(parts):
+            for k, (I, J) in enumerate(pr):
+                found[(int(I), int(J))] = mm[r][int(ofs[r][k]):int(ofs[r][k + 1])]
+    else:
+        pp, of, allm = result.export_csr()
+        found = {(int(I), int(J)): allm[int(of[k]):int(of[k + 1])] for k, (I, J) in enumerate(pp)}
+    keys = [(int(I), int(J)) for I, J in np.asarray(pairs).reshape(-1, 2)]
+    sel = np.arange(len(keys))
+    order = np.random.default_rng(DUMP_SEED).permutation(len(keys))
+    while len(sel) > 1 and 8 * sum(len(found.get(keys[k], ())) for k in sel) > DUMP_BYTES - 24 * len(sel):
+        sel = np.sort(order[:len(sel) // 2])
+    counts = np.array([len(found.get(keys[k], ())) for k in sel], np.float64)
+    chunks = [found[keys[k]] for k in sel if keys[k] in found]
+    allm = np.concatenate(chunks) if chunks else np.zeros(0, [("i", np.uint32), ("j", np.uint32)])
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "pairs.npy"), np.array([keys[k] for k in sel], np.float64).reshape(-1, 2))
+    np.save(os.path.join(out_dir, "match_counts.npy"), counts)
+    np.save(os.path.join(out_dir, "matches.npy"), np.stack([allm["i"], allm["j"]], 1).astype(np.float32))
 
 
 def make_workload(wl):
@@ -170,7 +193,7 @@ def workload_config(wl, world):
             "parallelism": ("one GPU, all pairs" if world == 1 else
                             "ONE pair list cut into %d cost-balanced contiguous shards (sharding.my_shard), no data-path "
                             "collective, per-rank results gathered to rank 0 in pair order inside the timed region" % world),
-            "l2_policy": "inputs (descriptors + fp16 operands, %.1f GB) exceed the 126 MB L2"
+            "l2_policy": "inputs (descriptors + fp16 operands, %.1f GB) exceed the 50 MB L2"
                          % (wl["images"] * wl["feats"] * (wl["dim"] * esz + 2 * 2 * (wl["dim"] + 48)) / 1e9)}
 
 
@@ -248,6 +271,8 @@ def main():
                     help="exact = tensor-core brute force (default); cascade = OpenMVG CASCADE_HASHING_L2 (default of c4)")
     ap.add_argument("--feats", type=int, default=0, help="experiment only")
     ap.add_argument("--images", type=int, default=0, help="experiment only")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write the putative matches of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     # stdout carries exactly ONE line (the JSON): anything a library prints there (NCCL's version banner
     # at communicator creation, ...) is sent to stderr instead
@@ -355,6 +380,8 @@ def main():
     barrier()
     t_res = time.perf_counter() - t0
     n_matches, n_match_pairs = sum_over_ranks(m.total, m.num_pairs)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, pairs, m if gather is None else gather, rank)
 
     # ---------------- end-to-end leg: `e2e` ----------------
     for _ in range(2):
@@ -454,7 +481,7 @@ def main():
             torch.cuda.synchronize()
             te = time.perf_counter() - te0
             fl = 2.0 * w2["feats"] * w2["feats"] * w2["dim"] * len(pairs2)
-            peak = float(load_peaks()[0].get("bf16_tflops", 1590.0))
+            peak = float(load_peaks()[0].get("bf16_tflops", 989.0))
             extras[key] = {"workload": workload_config(w2, 1)["workload"], "pairs_per_s": 5 * len(pairs2) / te,
                            "ms_candidates": float(np.mean(c_ms)),
                            "roofline_frac": fl / (np.mean(c_ms) * 1e-3) / 1e12 / peak, "matches": mm.total}
@@ -472,8 +499,7 @@ def main():
         my_flop = 2.0 * float(np.sum(counts[my_pairs[:, 0].astype(np.int64)] * counts[my_pairs[:, 1].astype(np.int64)])) * dim
         ms_c = float(np.mean(cand_ms))
         achieved = my_flop / (ms_c * 1e-3) / 1e12
-        peak = float(peaks.get("bf16_tflops", 1590.0))
-        tpp, tsrc = measured_traffic_per_pair(args.workload)
+        peak = float(peaks.get("bf16_tflops", 989.0))
         line = {
             "metric": METRIC, "value": value, "unit": "pairs/s", "n_gpus": world, "steps": args.steps,
             "warmup": warmup, "ms_per_step": 1e3 * t_res / args.steps, "higher_is_better": True,
@@ -484,15 +510,12 @@ def main():
                     "bytes": "whole job (sum over ranks): r3d_upload_regions of the views each shard touches + packed "
                              "matches back" + (" + the gather's H2D on the senders / D2H on rank 0" if world > 1 else "")},
             "gpu_launches": int(launches_all),
-            "roofline": {"bound": "tensor", "kernel": "k_l2_candidates_2sm (tcgen05 kind::f16 cta_group::2, f16 candidates; "
+            "roofline": {"bound": "tensor", "kernel": "k_l2_candidates (wgmma m64n256k16 f16 -> f32, f16 candidates; "
                                                       "every reported distance is re-computed exactly)",
                          "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
                          "peak_source": "%s bf16_tflops (burst; kernel timed alone with CUDA events)" % peak_src,
                          "ms_per_launch": ms_c, "flop_per_launch": my_flop,
-                         "launch": "rank 0's shard of the step = %d pairs (batch launches of <= 128 pairs, summed)" % len(my_pairs),
-                         "traffic": (tpp * len(my_pairs) if tpp else None),
-                         "traffic_unit": "DRAM bytes per step of rank 0 (ncu dram__bytes_read+write of one batch launch, "
-                                         "scaled to the shard's pairs; %s)" % tsrc},
+                         "launch": "rank 0's shard of the step = %d pairs (batch launches of <= 128 pairs, summed)" % len(my_pairs)},
             "breakdown_ms": {"candidates": ms_c, "rerank": float(np.mean(rerank_ms)),
                              "exact_scan_and_pack": float(np.mean(fb_ms)), "device_total": float(np.mean(dev_ms)),
                              "host_dedup": float(np.mean(host_ms)), "of": "rank 0's shard"},
@@ -510,14 +533,14 @@ def main():
             rowb = dim * (1 if wl["u8"] else 4)
             per_step = (4.0 * stbq + 4.0 * words * stcq + q * (11.0 * rowb + 4.0 * words + 12 + 48)) / max(args.steps, 1)
             ms_k = float(np.mean(fb_ms))
-            hbm = float(peaks.get("hbm_gbs", 6650.0))
+            hbm = float(peaks.get("hbm_gbs", 3350.0))
             line["roofline"] = {"bound": "hbm", "kernel": "k_cascade_match (bucket gather + Hamming + 10 exact distances per query; "
                                                           "timed with the pack kernel that follows it)",
                                 "achieved": per_step / (ms_k * 1e-3) / 1e9, "peak": hbm, "unit": "GB/s",
                                 "frac": per_step / (ms_k * 1e-3) / 1e9 / hbm,
                                 "peak_source": "%s hbm_gbs (the tables of a pair fit the L2: the fraction can exceed what DRAM alone allows)" % peak_src,
                                 "ms_per_launch": ms_k, "bytes_per_launch": per_step,
-                                "launch": "rank 0's shard of the step = %d pairs" % len(my_pairs), "traffic": None}
+                                "launch": "rank 0's shard of the step = %d pairs" % len(my_pairs)}
             line["result"]["candidates_per_query"] = stbq / max(q, 1)
             line["result"]["distinct_candidates_per_query"] = stcq / max(q, 1)
             line["config"]["matcher"] = "cascade hashing (OpenMVG CASCADE_HASHING_L2 restated: SURVEY.md A.8), hashing of all views inside the step"
@@ -628,7 +651,7 @@ def ba_leg(args, ctx, torch, dist, rank, world, barrier, max_over_ranks):
     n_obs = int(len(arrs["obs_xy"]))
     nB = 6 * 200 + 6
     bytes_iter = 3 * (n_obs * 24 + len(arrs["points"]) * 24) + 2 * nB * nB * 8          # SURVEY.md 8d
-    peak_hbm = float(load_peaks()[0].get("hbm_gbs", 6650.0))
+    peak_hbm = float(load_peaks()[0].get("hbm_gbs", 3350.0))
     ba = {"iters_per_s": sg["iterations"] / t_loop, "e2e_iters_per_s": sg["iterations"] / tb,
           "iterations": int(sg["iterations"]), "seconds_lm_loop": t_loop, "seconds_call": tb,
           "seconds_setup": sg["seconds_setup"], "seconds_linear": sg["seconds_linear"],

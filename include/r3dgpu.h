@@ -1,5 +1,5 @@
 /*
- * r3dgpu.h -- C ABI of libr3dgpu.so: the B200 (sm_100a) replacement of Regard3D's compute-matches
+ * r3dgpu.h -- C ABI of libr3dgpu.so: the H100 (sm_90a) replacement of Regard3D's compute-matches
  * hot path and the downstream bundle-adjustment solve.
  *
  * Every entry point names the reference interface it replaces (paths relative to the Regard3D
@@ -9,7 +9,7 @@
  *
  * Conventions: plain pointers + sizes, host memory in and out, no C++/CUDA/torch types.
  * Return value: 0 = R3D_OK, negative = error (r3d_last_error() gives the text).  There is NO CPU
- * fallback: without a usable sm_100 device r3d_create() fails with R3D_ERR_NO_DEVICE.
+ * fallback: without a usable sm_90 device r3d_create() fails with R3D_ERR_NO_DEVICE.
  * Threading: a context may be used from any one thread at a time (the reference calls
  * computeMatches() on one dedicated wxThread: src/threads/R3DComputeMatchesThread.cpp:91-103).
  */
@@ -29,7 +29,7 @@ typedef enum {
   R3D_ERR_NOMEM = -3,
   R3D_ERR_IO = -4,           /* file could not be read / written */
   R3D_ERR_UNSUPPORTED = -5,  /* e.g. descriptor range outside what the fp16 operand can hold */
-  R3D_ERR_NO_DEVICE = -6     /* no sm_100 GPU: the library never falls back to the CPU */
+  R3D_ERR_NO_DEVICE = -6     /* no sm_90 GPU: the library never falls back to the CPU */
 } r3d_status;
 
 typedef enum { R3D_F32 = 0, R3D_U8 = 1 } r3d_dtype;
@@ -367,7 +367,7 @@ int r3d_compute_matches(r3d_ctx* ctx, const r3d_cm_params* params, const r3d_cm_
 /* ---- instrumentation ----------------------------------------------------------------------- */
 typedef struct {
   double ms_prep;        /* upload-time operand preparation kernels */
-  double ms_candidates;  /* tcgen05 candidate kernel(s), CUDA-event time on their stream */
+  double ms_candidates;  /* wgmma candidate kernel(s), CUDA-event time on their stream */
   double ms_rerank;      /* exact re-rank + ratio kernel(s) */
   double ms_fallback;    /* exact-scan kernel for uncertified queries + the per-pair pack / (i,j) sort kernel */
   double ms_device_total;/* first launch -> last kernel of the last r3d_match_pairs */

@@ -1,4 +1,4 @@
-"""Build libr3dgpu.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libr3dgpu.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m regard3d_b200.build [--force]
 
@@ -14,8 +14,8 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libr3dgpu.so")
 NVCC = os.environ.get("R3D_NVCC", "/usr/local/cuda/bin/nvcc")
 
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + [
     "-O3", "-lineinfo", "-std=c++17",
     "-ccbin", "g++",
     "-Xcompiler", "-fPIC,-O3,-pthread,-ffp-contract=off",
@@ -66,8 +66,8 @@ def build(force=False, verbose=False, defines=(), out_path=None, objdir_name="bu
             sys.stderr.write(out)
     if failed:
         raise RuntimeError("libr3dgpu build failed")
-    cmd = [NVCC, "-shared", "-o", out_path or OUT] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-ccbin", "g++",
-                                               "-Xcompiler", "-pthread", "-lpthread", "-ldl"]
+    cmd = [NVCC, "-shared", "-o", out_path or OUT] + objs + ARCH + ["-ccbin", "g++", "-Xcompiler", "-pthread", "-lpthread",
+                                                                    "-ldl"]
     subprocess.check_call(cmd)
     return out_path or OUT
 

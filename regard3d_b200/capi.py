@@ -1,7 +1,7 @@
 """ctypes binding of libr3dgpu.so (include/r3dgpu.h).
 
 Fails loudly: importing works anywhere (the CPU-only tests check the exported symbols), but
-`Context()` raises R3DError when no sm_100 device is present -- there is no CPU fallback.
+`Context()` raises R3DError when no sm_90 device is present -- there is no CPU fallback.
 """
 import ctypes as C
 import os

@@ -91,7 +91,7 @@ static void free_worker(DeviceWorker& w) {
   for (auto& kv : w.pool_sizes) cudaFree(kv.first);
   w.pool_sizes.clear();
   w.pool_free_blocks.clear();
-  void* ptrs[] = {w.d_pairs, w.d_items, w.d_keys, w.d_fb, w.d_nn, w.d_tmapQ, w.d_tmapD, w.d_tmapDh,
+  void* ptrs[] = {w.d_pairs, w.d_items, w.d_keys, w.d_fb, w.d_nn, w.d_tmapQ, w.d_tmapD,
                   w.d_cnt, w.d_slot, w.d_list, w.d_parts, w.d_list2, w.d_mdense, w.d_scan};
   for (void* p : ptrs)
     if (p) cudaFree(p);
@@ -112,16 +112,16 @@ static void free_worker(DeviceWorker& w) {
 }
 
 // Encode the two TMA descriptors of a view: 2-D fp16 [n_pad][kp], box = 64 columns x 128 rows,
-// 128-byte swizzle (the canonical K-major SWIZZLE_128B UMMA operand layout).
+// 128-byte swizzle (the K-major SWIZZLE_128B operand layout of wgmma).
 static int encode_view_maps(r3d_ctx* ctx, DeviceWorker& w, ViewDev& v, uint32_t slot) {
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) return fail(ctx, R3D_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
-  CUtensorMap maps[3];
-  void* bases[3] = {(void*)v.d_opQ, (void*)v.d_opD, (void*)v.d_opD};
-  for (int m = 0; m < 3; ++m) {
+  CUtensorMap maps[2];
+  void* bases[2] = {(void*)v.d_opQ, (void*)v.d_opD};
+  for (int m = 0; m < 2; ++m) {
     cuuint64_t gdim[2] = {(cuuint64_t)v.kp, (cuuint64_t)(v.tc_ok ? v.n_pad : (uint32_t)kRowPad)};
     cuuint64_t gstride[1] = {(cuuint64_t)v.kp * sizeof(__half)};
-    cuuint32_t box[2] = {(cuuint32_t)kKBlock, (cuuint32_t)(m == 2 ? kTileRows / 2 : kTileRows)};
+    cuuint32_t box[2] = {(cuuint32_t)kKBlock, (cuuint32_t)kTileRows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(&maps[m], CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, bases[m], gdim, gstride, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -130,7 +130,6 @@ static int encode_view_maps(r3d_ctx* ctx, DeviceWorker& w, ViewDev& v, uint32_t 
   }
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(w.d_tmapQ + slot, &maps[0], sizeof(CUtensorMap), cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(w.d_tmapD + slot, &maps[1], sizeof(CUtensorMap), cudaMemcpyHostToDevice, w.stream));
-  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(w.d_tmapDh + slot, &maps[2], sizeof(CUtensorMap), cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));  // maps[] is a stack temporary
   return R3D_OK;
 }
@@ -139,21 +138,17 @@ static int ensure_tmap_capacity(r3d_ctx* ctx, DeviceWorker& w, uint32_t need) {
   if (need <= w.tmap_cap) return R3D_OK;
   uint32_t cap = w.tmap_cap ? w.tmap_cap : 64;
   while (cap < need) cap *= 2;
-  CUtensorMap *nq = nullptr, *nd = nullptr, *nh = nullptr;
+  CUtensorMap *nq = nullptr, *nd = nullptr;
   R3D_CUDA_TRY(ctx, cudaMalloc(&nq, cap * sizeof(CUtensorMap)));
   R3D_CUDA_TRY(ctx, cudaMalloc(&nd, cap * sizeof(CUtensorMap)));
-  R3D_CUDA_TRY(ctx, cudaMalloc(&nh, cap * sizeof(CUtensorMap)));
   if (w.tmap_cap) {
     R3D_CUDA_TRY(ctx, cudaMemcpy(nq, w.d_tmapQ, w.tmap_cap * sizeof(CUtensorMap), cudaMemcpyDeviceToDevice));
     R3D_CUDA_TRY(ctx, cudaMemcpy(nd, w.d_tmapD, w.tmap_cap * sizeof(CUtensorMap), cudaMemcpyDeviceToDevice));
-    R3D_CUDA_TRY(ctx, cudaMemcpy(nh, w.d_tmapDh, w.tmap_cap * sizeof(CUtensorMap), cudaMemcpyDeviceToDevice));
     cudaFree(w.d_tmapQ);
     cudaFree(w.d_tmapD);
-    cudaFree(w.d_tmapDh);
   }
   w.d_tmapQ = nq;
   w.d_tmapD = nd;
-  w.d_tmapDh = nh;
   w.tmap_cap = cap;
   return R3D_OK;
 }
@@ -253,11 +248,11 @@ int r3d_create(const int* device_ids, int n_devices, r3d_ctx** out) {
     }
     cudaDeviceProp prop;
     cudaGetDeviceProperties(&prop, id);
-    if (prop.major != 10) {
+    if (prop.major != 9 || prop.minor != 0) {
       delete ctx;
       return fail(nullptr, R3D_ERR_NO_DEVICE,
                   "r3d_create: device " + std::to_string(id) + " is sm_" + std::to_string(prop.major) +
-                      std::to_string(prop.minor) + "; this library is built for sm_100a only");
+                      std::to_string(prop.minor) + "; this library is built for sm_90a only");
     }
     DeviceWorker w;
     w.device = id;

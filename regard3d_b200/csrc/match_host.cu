@@ -239,7 +239,7 @@ static int match_on_worker(r3d_ctx* ctx, DeviceWorker& w, const uint32_t* pairs,
     auto hitems = std::make_shared<std::vector<WorkItem>>();
     hitems->reserve(2 * n_items + nb);
     for (uint32_t k = 0; k < nb; ++k)
-      if ((*hp)[k].use_tc)  // CTA-pair kernel: 128-query blocks; n_pad is a multiple of 256 -> always an even count per pair
+      if ((*hp)[k].use_tc)  // 128-query blocks
         for (uint32_t qb = 0; qb < (*hp)[k].nJ_pad / kTileRows; ++qb) hitems->push_back(WorkItem{k, qb});
     const bool any_tc = !hitems->empty();
     if (cascade)  // the item array carries (table row of I, table row of J) per pair instead of work items
@@ -291,8 +291,8 @@ static int match_on_worker(r3d_ctx* ctx, DeviceWorker& w, const uint32_t* pairs,
 
     R3D_CUDA_TRY(ctx, cudaEventRecord(o.ev[0], w.stream));
     if (any_tc) {
-      rc = launch_l2_candidates_2sm(ctx, w, (const PairDesc*)w.d_pairs, (const WorkItem*)w.d_items, (uint32_t)hitems->size(),
-                                    (uint32_t*)w.d_keys, kp, operand_ksteps((int)dim));
+      rc = launch_l2_candidates(ctx, w, (const PairDesc*)w.d_pairs, (const WorkItem*)w.d_items, (uint32_t)hitems->size(),
+                                (uint32_t*)w.d_keys, kp, operand_ksteps((int)dim));
       if (rc) return rc;
       launches += 1;
     }

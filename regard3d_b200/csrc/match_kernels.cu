@@ -1,4 +1,4 @@
-// match_kernels.cu -- CUDA-core kernels of the putative-matching path (sm_100a):
+// match_kernels.cu -- CUDA-core kernels of the putative-matching path (sm_90a):
 //   k_view_stats / k_view_prepare : build the fp16 tensor-core operands of a view (+ error constants)
 //   k_rerank                      : exact re-rank of the candidate chunks, certification, ratio test
 //   k_exact_scan                  : exact brute-force 2-NN for listed queries (uncertified / forced)

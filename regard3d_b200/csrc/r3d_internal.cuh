@@ -1,4 +1,4 @@
-// r3d_internal.cuh -- internal declarations of libr3dgpu (B200 / sm_100a only).
+// r3d_internal.cuh -- internal declarations of libr3dgpu (H100 / sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -18,16 +18,16 @@
 #include "r3d_matches.h"
 
 // ------------------------------------------------------------------------------------------------
-// Geometry of the tensor-core candidate kernel (k_l2_candidates_2sm.cu) and the operand layout.
+// Geometry of the tensor-core candidate kernel (k_l2_candidates.cu) and the operand layout.
 // ------------------------------------------------------------------------------------------------
 namespace r3d {
 
-constexpr int kTileRows = 128;      // rows of one TMA box / one UMMA M or N extent
+constexpr int kTileRows = 128;      // rows of one TMA box / one query block
 constexpr int kKBlock = 64;         // fp16 elements per 128-byte swizzle row
 constexpr int kQB = 2;              // query blocks (of 128 rows) resident per CTA
 constexpr int kSuperRows = kTileRows * kQB;  // 256 query rows per work item
 constexpr int kRowPad = 256;        // every view is padded to a multiple of this many rows
-constexpr int kBiasCols = 16;       // one UMMA K-step holding the norm terms
+constexpr int kBiasCols = 16;       // one MMA K-step holding the norm terms
 #ifndef R3D_CHUNK
 #define R3D_CHUNK 8
 #endif
@@ -116,7 +116,6 @@ struct DeviceWorker {
   std::map<uint32_t, uint32_t> view_slot;
   CUtensorMap* d_tmapQ = nullptr;
   CUtensorMap* d_tmapD = nullptr;
-  CUtensorMap* d_tmapDh = nullptr;  // database role, 64-row boxes (2-CTA multicast halves)
   uint32_t tmap_cap = 0;
   // per-context scale exponent of the norm split (S0 = 2^e0, S1 = 2^(e0-11))
   int e0 = -3;
@@ -218,10 +217,9 @@ inline void parallel_for(int n_threads, size_t n, F&& f) {
 // operand preparation
 int launch_view_stats(r3d_ctx* ctx, DeviceWorker& w, ViewDev& v);
 int launch_view_prepare(r3d_ctx* ctx, DeviceWorker& w, ViewDev& v, int e0);
-// tensor-core candidate kernel: persistent CTA pairs (tcgen05 cta_group::2); work items are 128-query blocks, two
-// consecutive items share a pair
-int launch_l2_candidates_2sm(r3d_ctx* ctx, DeviceWorker& w, const PairDesc* d_pairs, const WorkItem* d_items,
-                             uint32_t n_items, uint32_t* d_keys, int kp_cols, int ksteps);
+// tensor-core candidate kernel: persistent CTAs (TMA + wgmma); work items are 128-query blocks
+int launch_l2_candidates(r3d_ctx* ctx, DeviceWorker& w, const PairDesc* d_pairs, const WorkItem* d_items,
+                         uint32_t n_items, uint32_t* d_keys, int kp_cols, int ksteps);
 // exact re-rank + ratio
 int launch_rerank_list(r3d_ctx* ctx, DeviceWorker& w, const PairDesc* d_pairs, const uint32_t* d_keys, const void* d_parts,
                        const uint2* d_list, const uint32_t* d_list_count, uint32_t max_list, uint32_t dim, int dtype,

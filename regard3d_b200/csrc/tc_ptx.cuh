@@ -1,5 +1,5 @@
-// tc_ptx.cuh -- inline-PTX wrappers for the sm_100a tensor-core path (mbarrier, TMA, tcgen05, clusters)
-// and the candidate-key epilogue shared by the k_l2_candidates kernels.
+// tc_ptx.cuh -- inline-PTX wrappers for the sm_90a tensor-core path (mbarrier, TMA, wgmma)
+// and the candidate-key update of the k_l2_candidates kernel.
 #pragma once
 #include "r3d_internal.cuh"
 
@@ -35,81 +35,10 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 __device__ __forceinline__ void fence_barrier_init() {
   asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-__device__ __forceinline__ void fence_proxy_async() {
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
       ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_mc(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar,
-                                               uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%2, %3}], [%4], %5;"
-      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar), "h"(cta_mask) : "memory");
-}
-__device__ __forceinline__ void tc_commit_mc(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(cta_mask) : "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t cluster_nctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
-  asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                           uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
-}
-// tcgen05.wait::ld that also names the destination registers, so no use of them can be scheduled
-// above the wait by the compiler.
-__device__ __forceinline__ void tc_wait_ld(uint32_t (&v)[32]) {
-  asm volatile("tcgen05.wait::ld.sync.aligned;"
-               : "+r"(v[0]), "+r"(v[1]), "+r"(v[2]), "+r"(v[3]), "+r"(v[4]), "+r"(v[5]), "+r"(v[6]), "+r"(v[7]),
-                 "+r"(v[8]), "+r"(v[9]), "+r"(v[10]), "+r"(v[11]), "+r"(v[12]), "+r"(v[13]), "+r"(v[14]), "+r"(v[15]),
-                 "+r"(v[16]), "+r"(v[17]), "+r"(v[18]), "+r"(v[19]), "+r"(v[20]), "+r"(v[21]), "+r"(v[22]), "+r"(v[23]),
-                 "+r"(v[24]), "+r"(v[25]), "+r"(v[26]), "+r"(v[27]), "+r"(v[28]), "+r"(v[29]), "+r"(v[30]), "+r"(v[31])
-               :: "memory");
-}
-
-__device__ __forceinline__ float fmin3(float a, float b, float c) {
-  float r;
-  asm("min.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-  return r;
 }
 
 // one lane of a converged warp (all 32 lanes must execute this)
@@ -124,30 +53,70 @@ __device__ __forceinline__ bool elect_one() {
   return pred != 0;
 }
 
-// K-major, 128-byte swizzle shared-memory matrix descriptor (SM100 "version 1"):
-//   start address >> 4 | LBO (ignored for swizzled K-major) | SBO = 1024 B (8 rows x 128 B) |
-//   version = 1 | layout type = SWIZZLE_128B (2)
-constexpr uint32_t kDescHi = (uint32_t)(1024 >> 4) | (1u << 14) | (2u << 29);  // SBO | version | SWIZZLE_128B
+// register budget of a warpgroup (all 128 threads of the warpgroup execute it)
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+
+// K-major, 128-byte swizzle shared-memory matrix descriptor of wgmma:
+//   start address >> 4 | LBO (unused for swizzled K-major: 1) | SBO = 1024 B (8 rows x 128 B) | SWIZZLE_128B (1 << 62)
+// The operand tiles are the TMA boxes (128-byte rows, SWIZZLE_128B, 1024-byte aligned); one K-step of 16 fp16
+// columns advances the start address by 32 bytes (2 in the >> 4 encoding).
+constexpr uint32_t kDescHi = (uint32_t)(1024 >> 4) | (1u << 30);  // SBO | layout type 1 (bits 62-63)
 __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr) { return ((saddr >> 4) & 0x3fffu) | (1u << 16); }
 __device__ __forceinline__ uint64_t make_desc(uint32_t lo) { return ((uint64_t)kDescHi << 32) | (uint64_t)lo; }
-// kind::f16 instruction descriptor: D = f32, A = B = f16, both K-major, N = 128, M = 128.
-constexpr uint32_t kInstrDesc = (1u << 4) | ((uint32_t)(kTileRows >> 3) << 17) | ((uint32_t)(kTileRows >> 4) << 24);
 
-// minimum of kChunk accumulator columns, packed with the chunk id, inserted into the sorted key set
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kPending>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kPending) : "memory"); }
+// ties the accumulator registers to this point: no read of them is scheduled above a preceding wgmma_wait
+__device__ __forceinline__ void wgmma_fence_operand(float (&d)[128]) {
+#pragma unroll
+  for (int i = 0; i < 128; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// D (64 x 256, f32, registers) (+)= A (64 x 16, f16, shared) x B (256 x 16, f16, shared)^T; both operands K-major.
+// scale_d = 0 overwrites D (first K-step of a tile).
+__device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+      "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, "
+      "%80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, "
+      "%96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, "
+      "%112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+      "}, %128, %129, p, 1, 1, 0, 0;\n\t"
+      "}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]),
+        "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]),
+        "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]),
+        "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]),
+        "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]),
+        "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]),
+        "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]),
+        "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]),
+        "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+}
+
+// A chunk minimum, packed with its chunk id, inserted into the sorted key set of its query row.
 template <bool kVote = false>
-__device__ __forceinline__ void chunk_update(const uint32_t* v, uint32_t chunk_id, uint32_t keep_mask,
-                                             float (&key)[kNumKeys]) {
-  static_assert(kChunk == 8 || kChunk == 16, "chunk width");
-  float m = fmin3(__uint_as_float(v[0]), __uint_as_float(v[1]), __uint_as_float(v[2]));
-  m = fmin3(m, __uint_as_float(v[3]), __uint_as_float(v[4]));
-  m = fmin3(m, __uint_as_float(v[5]), __uint_as_float(v[6]));
-  if (kChunk == 16) {
-    m = fmin3(m, __uint_as_float(v[7]), __uint_as_float(v[8]));
-    m = fmin3(m, __uint_as_float(v[9]), __uint_as_float(v[10]));
-    m = fmin3(m, __uint_as_float(v[11]), __uint_as_float(v[12]));
-    m = fmin3(m, __uint_as_float(v[13]), __uint_as_float(v[14]));
-  }
-  m = fminf(m, __uint_as_float(v[kChunk - 1]));
+__device__ __forceinline__ void key_insert(float m, uint32_t chunk_id, uint32_t keep_mask, float (&key)[kNumKeys]) {
   float x = __uint_as_float((__float_as_uint(m) & keep_mask) | chunk_id);
   // A key that is not below the current largest kept key leaves the set unchanged (the network would carry it
   // through every level).  After t chunks a lane inserts with probability ~ kNumKeys / t, so most chunks need no
@@ -160,35 +129,6 @@ __device__ __forceinline__ void chunk_update(const uint32_t* v, uint32_t chunk_i
     x = hi;
   }
   key[kNumKeys - 1] = fminf(key[kNumKeys - 1], x);
-}
-
-
-// ---- cluster-remote mbarrier arrive (CTA pair protocols) ----------------------------------------
-__device__ __forceinline__ uint32_t mapa_shared(uint32_t local_addr, uint32_t cta_rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(cta_rank));
-  return r;
-}
-// RELAXED on purpose: a release at cluster scope compiles to MEMBAR.ALL.GPU + ERRBAR + CGAERRBAR per
-// arrive (measured: +65 % kernel time).  The hand-shakes that use it publish no generic-proxy writes:
-// "TMEM stage drained" follows tcgen05.wait::ld + tcgen05.fence::before_thread_sync, and "operands
-// landed" forwards an mbarrier completion of TMA (async-proxy) writes that the tensor core reads.
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// ---- cta_group::2 variants -----------------------------------------------------------------------
-__device__ __forceinline__ void tc2_mma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tc2_commit_mc(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(cta_mask) : "memory");
 }
 
 }  // namespace tcx

@@ -6,6 +6,7 @@
   liop_ref_v1.npz        patches (float32 41x41, seeded: smooth / noisy / quantised-with-ties / flat / steps) and the
                          descriptors THE REFERENCE ITSELF computes for them: oracle/_ref/libvlliop_ref.so, built by
                          oracle/Makefile from /root/reference/src/thirdparty/liop/vl_liop.c (r3d_vl_liopdesc_process).
+  liop_ref_mixed_v1.npz  the reference's descriptors of mixed_patches() (noise, quantised with ties, row sums).
   liop_patch_cv2_v1.npz  a seeded image, keypoints, and the 41x41 patches cv2 (version recorded) produces with the
                          reference's call sequence (src/Regard3DFeatures.cpp:766-806): warpAffine(INTER_LINEAR |
                          WARP_INVERSE_MAP) then GaussianBlur(sigma = 1.2); warped-only patches are stored too.
@@ -44,6 +45,19 @@ def make_patches(seed=20260924):
     return np.stack(out).astype(np.float32)
 
 
+def mixed_patches(seed=11):
+    rng = np.random.default_rng(seed)
+    patches = []
+    for k in range(120):
+        p = rng.random((41, 41)).astype(np.float32)
+        if k % 3 == 1:
+            p = np.floor(p * (2 + k % 7)) / (2 + k % 7)        # exact ties: the order is the quick sort's own
+        if k % 3 == 2:
+            p = np.cumsum(p, 1) / 41
+        patches.append(p.astype(np.float32))
+    return np.stack(patches)
+
+
 def main():
     import cv2
     assert po.liop_ref_available(), "needs /root/reference (oracle/_ref)"
@@ -51,6 +65,8 @@ def main():
     desc = po.liop_ref_process(patches)
     np.savez_compressed(os.path.join(HERE, "liop_ref_v1.npz"), patches=patches, desc=desc,
                         source="r3d_vl_liopdesc_process of /root/reference/src/thirdparty/liop/vl_liop.c (oracle/_ref)")
+    np.savez_compressed(os.path.join(HERE, "liop_ref_mixed_v1.npz"), desc=po.liop_ref_process(mixed_patches()),
+                        source="r3d_vl_liopdesc_process of src/thirdparty/liop/vl_liop.c (oracle/_ref)")
     # ---- OpenCV patch extraction ----
     rng = np.random.default_rng(20260925)
     h, w = 240, 320
@@ -68,10 +84,11 @@ def main():
         p = cv2.warpAffine(img, M, (41, 41), flags=cv2.INTER_LINEAR | cv2.WARP_INVERSE_MAP)
         warped.append(p.copy())
         blurred.append(cv2.GaussianBlur(p, (0, 0), 1.2))
-    np.savez_compressed(os.path.join(HERE, "liop_patch_cv2_v1.npz"), img=img, kps=kps, factor=factor,
-                        warped=np.stack(warped), blurred=np.stack(blurred), cv2_version=cv2.__version__,
+    keep = 40                                            # the first keypoints only: the file stays below 1 MB
+    np.savez_compressed(os.path.join(HERE, "liop_patch_cv2_v1.npz"), img=img, kps=kps[:keep], factor=factor,
+                        warped=np.stack(warped[:keep]), blurred=np.stack(blurred[:keep]), cv2_version=cv2.__version__,
                         gauss_kernel=cv2.getGaussianKernel(11, 1.2, cv2.CV_32F).ravel())
-    print("wrote liop_ref_v1.npz (%d patches) and liop_patch_cv2_v1.npz (%d keypoints), cv2 %s" % (len(patches), n, cv2.__version__))
+    print("wrote liop_ref_v1.npz (%d patches) and liop_patch_cv2_v1.npz (%d keypoints), cv2 %s" % (len(patches), keep, cv2.__version__))
 
 
 if __name__ == "__main__":

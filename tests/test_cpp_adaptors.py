@@ -1,6 +1,6 @@
 """The header-only openMVG::matching::ArrayMatcher adaptor (regard3d_b200/csrc/ArrayMatcher_b200.h) compiles against a
 stand-in of the two OpenMVG types it is instantiated with, links with libr3dgpu.so, and -- on a machine without a
-B200 -- fails loudly (Build returns false, the error text says there is no CPU fallback)."""
+H100 -- fails loudly (Build returns false, the error text says there is no CPU fallback)."""
 import os
 import subprocess
 import textwrap
