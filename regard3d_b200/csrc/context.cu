@@ -77,6 +77,7 @@ static void free_view(DeviceWorker& w, ViewDev& v) {
   pool_release(w, v.d_desc);
   pool_release(w, v.d_opQ);
   pool_release(w, v.d_opD);
+  pool_release(w, v.d_norm);
   pool_release(w, v.d_xy);
   pool_release(w, v.d_stats);
   if (v.d_cascade) pool_release(w, v.d_cascade);
@@ -112,13 +113,26 @@ static void free_worker(DeviceWorker& w) {
 }
 
 // Encode the two TMA descriptors of a view: 2-D fp16 [n_pad][kp], box = 64 columns x 128 rows,
-// 128-byte swizzle (the K-major SWIZZLE_128B operand layout of wgmma).
+// 128-byte swizzle (the K-major SWIZZLE_128B operand layout of wgmma).  Integer path: one 2-D uint8 map over the
+// descriptors themselves ([n][dim], box = 128 columns x 128 rows; TMA zero-fills rows >= n and columns >= dim)
+// serves both roles.
 static int encode_view_maps(r3d_ctx* ctx, DeviceWorker& w, ViewDev& v, uint32_t slot) {
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) return fail(ctx, R3D_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   CUtensorMap maps[2];
   void* bases[2] = {(void*)v.d_opQ, (void*)v.d_opD};
-  for (int m = 0; m < 2; ++m) {
+  if (v.int_ops) {
+    cuuint64_t gdim[2] = {(cuuint64_t)v.dim, (cuuint64_t)std::max<uint32_t>(v.n, 1)};
+    cuuint64_t gstride[1] = {(cuuint64_t)v.dim};
+    cuuint32_t box[2] = {128, (cuuint32_t)kTileRows};
+    cuuint32_t estr[2] = {1, 1};
+    CUresult r = enc(&maps[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, v.d_desc, gdim, gstride, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(ctx, R3D_ERR_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
+    maps[1] = maps[0];
+  }
+  for (int m = 0; m < 2 && !v.int_ops; ++m) {
     cuuint64_t gdim[2] = {(cuuint64_t)v.kp, (cuuint64_t)(v.tc_ok ? v.n_pad : (uint32_t)kRowPad)};
     cuuint64_t gstride[1] = {(cuuint64_t)v.kp * sizeof(__half)};
     cuuint32_t box[2] = {(cuuint32_t)kKBlock, (cuuint32_t)kTileRows};
@@ -176,6 +190,10 @@ int prepare_views(r3d_ctx* ctx, DeviceWorker& w) {
     v->max_hnorm = std::sqrt(stats[4 * i + 1]) * (1.f + 1e-6f);
     v->max_dnorm = std::sqrt(stats[4 * i + 2]) * (1.f + 1e-6f);
     v->max_abs = stats[4 * i + 3];
+    if (v->int_ops) {  // the stats pass wrote its exact norms: nothing else to prepare, no part in e0
+      v->prepared = true;
+      continue;
+    }
     // a view the fp16 operands cannot represent (|a_k| > 32000, or ||a||^2 >= 2^28 for the two-piece norm split)
     // keeps its exact descriptors only: its pairs take the exact scan (slower, same results)
     if (!v->tc_ok || !(v->max_abs <= 32000.f) || !(stats[4 * i + 0] < 2.6e8f)) {
@@ -186,7 +204,7 @@ int prepare_views(r3d_ctx* ctx, DeviceWorker& w) {
     max_n2 = std::fmax(max_n2, stats[4 * i + 0]);
   }
   for (auto& kv : w.views)
-    if (kv.second.prepared && kv.second.tc_ok) max_n2 = std::fmax(max_n2, kv.second.max_norm * kv.second.max_norm);
+    if (kv.second.prepared && kv.second.tc_ok && !kv.second.int_ops) max_n2 = std::fmax(max_n2, kv.second.max_norm * kv.second.max_norm);
   // Norm split scale: ||a||^2 ~= p0*2^e0 + p1*2^(e0-11) with p0 <= 2^13 and 2^(e0-11) a normal fp16.
   int e0 = -3;
   if (max_n2 > 0.f) {
@@ -201,7 +219,7 @@ int prepare_views(r3d_ctx* ctx, DeviceWorker& w) {
   w.e0_fixed = true;
   for (auto& kv : w.views) {
     ViewDev& v = kv.second;
-    if (!v.tc_ok) continue;
+    if (!v.tc_ok || v.int_ops) continue;
     if (v.prepared && !redo_all) continue;
     int rc = launch_view_prepare(ctx, w, v, e0);
     if (rc) return rc;
@@ -309,16 +327,21 @@ int r3d_upload_regions(r3d_ctx* ctx, uint32_t view_id, const void* desc, uint32_
     ViewDev v;
     v.n = n; v.dim = dim; v.dtype = (uint32_t)dtype;
     v.n_pad = (uint32_t)pad_up((int)(n ? n : 1), kRowPad);
-    v.tc_ok = dim <= 240;  // Kp <= 256 columns; wider descriptors are matched by the exact scan only
-    v.kp = (uint32_t)operand_cols((int)(dim && v.tc_ok ? dim : 16));
+    v.int_ops = int_operand(dtype, dim);
+    v.tc_ok = v.int_ops || dim <= 240;  // fp16: Kp <= 256 columns; wider descriptors are matched by the exact scan only
+    v.kp = v.int_ops ? 0u : (uint32_t)operand_cols((int)(dim && v.tc_ok ? dim : 16));
     const size_t rb = dtype == R3D_F32 ? (size_t)dim * 4 : (size_t)dim;
-    v.d_desc = pool_alloc(w, std::max<size_t>(rb * n, 16));
-    const size_t op_rows = v.tc_ok ? v.n_pad : (uint32_t)kRowPad;  // a token block keeps the tensor maps valid
-    v.d_opQ = (__half*)pool_alloc(w, op_rows * v.kp * sizeof(__half));
-    v.d_opD = (__half*)pool_alloc(w, op_rows * v.kp * sizeof(__half));
+    v.d_desc = pool_alloc(w, std::max<size_t>(rb * std::max<uint32_t>(n, 1), 16));  // >= one row: the u8 map's extent
+    if (v.int_ops) {
+      v.d_norm = (int32_t*)pool_alloc(w, (size_t)v.n_pad * sizeof(int32_t));
+    } else {
+      const size_t op_rows = v.tc_ok ? v.n_pad : (uint32_t)kRowPad;  // a token block keeps the tensor maps valid
+      v.d_opQ = (__half*)pool_alloc(w, op_rows * v.kp * sizeof(__half));
+      v.d_opD = (__half*)pool_alloc(w, op_rows * v.kp * sizeof(__half));
+    }
     v.d_stats = (float*)pool_alloc(w, 4 * sizeof(float));
     if (xy && n) v.d_xy = (float2*)pool_alloc(w, (size_t)n * sizeof(float2));
-    if (!v.d_desc || !v.d_opQ || !v.d_opD || !v.d_stats || (xy && n && !v.d_xy)) {
+    if (!v.d_desc || (v.int_ops ? !v.d_norm : (!v.d_opQ || !v.d_opD)) || !v.d_stats || (xy && n && !v.d_xy)) {
       free_view(w, v);
       return fail(ctx, R3D_ERR_NOMEM, "r3d_upload_regions: device allocation failed");
     }

@@ -1,16 +1,22 @@
 // k_l2_candidates.cu -- the tensor-core candidate kernel (sm_90a: TMA, mbarrier, wgmma).
 //
-// Work item = (pair, 128-query block of view J).  For every query row the kernel evaluates the fp16 distance
-// surrogate opQ(J) . opD(I) against all database rows of view I and keeps the kNumKeys smallest chunk minima
-// (kChunk consecutive database rows each), packed with the chunk id, in keys_out.
+// Work item = (pair, 128-query block of view J).  For every query row the kernel evaluates a squared distance
+// against all database rows of view I and keeps the kNumKeys smallest chunk minima (kChunk consecutive database rows
+// each), packed with the chunk id, in keys_out.  Two operand kinds, one kernel template:
+//   fp16 (kU8 = false)  the distance surrogate opQ(J) . opD(I) of the fp16 operands (k_view_prepare), f32 accumulation
+//   u8   (kU8 = true)   uint8 descriptors read in place (int_operand()): ||a||^2 - 2 q.a from u8 x u8 -> s32 MMAs plus
+//                       the exact norms, so the keys are exact up to the chunk-id packing
 //
 // Persistent CTAs (one per SM, 227 KB of shared memory), three warpgroups:
-//   warpgroup 0      one TMA producer warp: the item's query block (nkb boxes of 128 rows x 64 columns, double
-//                    buffered across items) and a ring of database stages (one 64-column K-block of a 256-row tile)
-//   warpgroups 1, 2  consumers of query rows 0-63 / 64-127: per 256-row tile, m64n256k16 wgmma into 128 f32
-//                    registers per thread, then the chunk minima and the key insertion in registers.
-// Both consumers read every database stage.  The tensor core runs one consumer's tile while the other reduces its
-// accumulator, so the epilogue overlaps the MMAs without a second accumulator.
+//   warpgroup 0      one TMA producer warp: the item's query block (nkb boxes of 128 rows x 128 bytes, double
+//                    buffered across items) and a ring of database stages (one 128-byte K-block of a 256-row tile;
+//                    u8: plus the tile's 256 database norms)
+//   warpgroups 1, 2  consumers of query rows 0-63 / 64-127: the MMAs, then the chunk minima and the key insertion in
+//                    registers.
+//     fp16: per 256-row tile, m64n256k16 into 128 f32 registers, then the epilogue.
+//     u8:   per 128-row half tile, m64n128k32 into one of two 64-register s32 accumulators; the epilogue of half h
+//           runs while the MMAs of half h + 1 are in the tensor pipe (at the integer rate the MMAs of a half take
+//           about as long as its epilogue).
 // Barriers: full[s] (TMA bytes landed), empty[s] (the 8 consumer warps are done with the stage), qfull / qempty the
 // same for the query buffers.
 #include "r3d_internal.cuh"
@@ -25,18 +31,23 @@ namespace {
 constexpr int kMaxStages = 8;
 constexpr uint32_t kTileN = 256;                  // database rows per tile (the wgmma N extent)
 constexpr uint32_t kStageBytes = 2 * kBoxBytes;   // one K-block of a 256-row tile: two 128-row TMA boxes
+constexpr uint32_t kNormBytes = kTileN * 4;       // u8: the int32 norms of a tile's database rows
 constexpr uint32_t kConsumerWarps = 8;
 constexpr uint32_t kThreads = 384;
 constexpr size_t kSmemOptIn = 232448;             // 227 KB: the largest dynamic shared memory of one block on sm_90
 static_assert(kChunk == 8, "the epilogue reduces one 8-column block of the wgmma accumulator per chunk");
 
+__device__ __forceinline__ float vmin(float a, float b) { return fminf(a, b); }
+__device__ __forceinline__ int32_t vmin(int32_t a, int32_t b) { return min(a, b); }
+
 // Minima of four consecutive chunks of one accumulator row, spread over the 4 lanes of a quad (2 columns each),
 // reduced and scattered so that lane q of the quad ends with the minimum of chunk q: 3 shuffles for 4 chunks.
-__device__ __forceinline__ float quad_min4(float p0, float p1, float p2, float p3, uint32_t q) {
+template <typename T>
+__device__ __forceinline__ T quad_min4(T p0, T p1, T p2, T p3, uint32_t q) {
   const bool b1 = (q & 2u) != 0, b0 = (q & 1u) != 0;
-  const float k0 = fminf(b1 ? p2 : p0, __shfl_xor_sync(0xffffffffu, b1 ? p0 : p2, 2));
-  const float k1 = fminf(b1 ? p3 : p1, __shfl_xor_sync(0xffffffffu, b1 ? p1 : p3, 2));
-  return fminf(b0 ? k1 : k0, __shfl_xor_sync(0xffffffffu, b0 ? k0 : k1, 1));
+  const T k0 = vmin(b1 ? p2 : p0, __shfl_xor_sync(0xffffffffu, b1 ? p0 : p2, 2));
+  const T k1 = vmin(b1 ? p3 : p1, __shfl_xor_sync(0xffffffffu, b1 ? p1 : p3, 2));
+  return vmin(b0 ? k1 : k0, __shfl_xor_sync(0xffffffffu, b0 ? k0 : k1, 1));
 }
 
 // the kNumKeys smallest keys of this lane's set and the set of lane ^ d (the keys of different chunks differ)
@@ -59,10 +70,12 @@ __device__ __forceinline__ void merge_keys(float (&key)[kNumKeys], int d) {
 
 }  // namespace
 
+template <bool kU8>
 __global__ void __launch_bounds__(kThreads, 1)
 k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __restrict__ tmapD,
                 const PairDesc* __restrict__ pairs, const WorkItem* __restrict__ items, uint32_t n_items,
                 uint32_t* __restrict__ keys_out, uint32_t nkb, uint32_t ksteps, uint32_t n_stages, uint32_t n_qbuf) {
+  constexpr uint32_t kBoxCols = kU8 ? 128u : (uint32_t)kKBlock;  // elements in a 128-byte box row
   extern __shared__ unsigned char smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
   // n_qbuf (1 or 2) x nkb boxes: the item's 128 query rows.  With two buffers the next item's query block is loaded
@@ -70,7 +83,8 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
   const uint32_t q_base = base;
   const uint32_t q_bytes = nkb * kBoxBytes;
   const uint32_t d_base = q_base + n_qbuf * q_bytes;            // n_stages stages
-  const uint32_t bar_full = d_base + n_stages * kStageBytes;    // [kMaxStages]
+  const uint32_t n_base = d_base + n_stages * kStageBytes;      // u8: n_stages x kNormBytes
+  const uint32_t bar_full = n_base + (kU8 ? n_stages * kNormBytes : 0u);  // [kMaxStages]
   const uint32_t bar_empty = bar_full + 8 * kMaxStages;         // [kMaxStages]
   const uint32_t bar_qfull = bar_empty + 8 * kMaxStages;        // [2]
   const uint32_t bar_qempty = bar_qfull + 16;                   // [2]
@@ -109,7 +123,7 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       if (elect_one()) {
         mbar_arrive_expect_tx(bar_qfull + 8 * qb, nkb * kBoxBytes);
         for (uint32_t kb = 0; kb < nkb; ++kb)
-          tma_load_2d(q_base + qb * q_bytes + kb * kBoxBytes, mq, (int)(kb * kKBlock), (int)(wi.sb * kTileRows),
+          tma_load_2d(q_base + qb * q_bytes + kb * kBoxBytes, mq, (int)(kb * kBoxCols), (int)(wi.sb * kTileRows),
                       bar_qfull + 8 * qb);
       }
       __syncwarp();
@@ -118,9 +132,11 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
           mbar_wait(bar_empty + 8 * stage, phase ^ 1u);
           if (elect_one()) {
             const uint32_t dst = d_base + stage * kStageBytes;
-            mbar_arrive_expect_tx(bar_full + 8 * stage, kStageBytes);
-            tma_load_2d(dst, md, (int)(kb * kKBlock), (int)(t * kTileN), bar_full + 8 * stage);
-            tma_load_2d(dst + kBoxBytes, md, (int)(kb * kKBlock), (int)(t * kTileN + kTileRows), bar_full + 8 * stage);
+            const bool norms = kU8 && kb == 0;  // the tile's norms travel with its first K-block
+            mbar_arrive_expect_tx(bar_full + 8 * stage, kStageBytes + (norms ? kNormBytes : 0u));
+            tma_load_2d(dst, md, (int)(kb * kBoxCols), (int)(t * kTileN), bar_full + 8 * stage);
+            tma_load_2d(dst + kBoxBytes, md, (int)(kb * kBoxCols), (int)(t * kTileN + kTileRows), bar_full + 8 * stage);
+            if (norms) bulk_load(n_base + stage * kNormBytes, pd.normI + t * kTileN, kNormBytes, bar_full + 8 * stage);
           }
           __syncwarp();
           if (++stage == n_stages) { stage = 0; phase ^= 1u; }
@@ -136,7 +152,6 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
   const uint32_t q = lane & 3u;                                  // lane inside the quad
   const uint32_t row0 = cw * 64u + (warp & 3u) * 16u + (lane >> 2);  // accumulator rows row0 and row0 + 8
   uint32_t stage = 0, phase = 0, qi = 0;
-  float acc[128];
   for (uint32_t it = blockIdx.x; it < n_items; it += gridDim.x, ++qi) {
     const WorkItem wi = items[it];
     const PairDesc pd = pairs[wi.pair];
@@ -148,44 +163,142 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
 #pragma unroll
     for (int i = 0; i < kNumKeys; ++i) key0[i] = key1[i] = __uint_as_float(kKeySentinel);
     const uint32_t a_base = q_base + qb * q_bytes + cw * (kBoxBytes / 2);  // 64 rows x 128 B into each query box
-    mbar_wait(bar_qfull + 8 * qb, qf);
-    for (uint32_t t = 0; t < ntiles; ++t) {
-      uint32_t ks_left = ksteps, prev = 0;
-      for (uint32_t kb = 0; kb < nkb; ++kb) {
-        mbar_wait(bar_full + 8 * stage, phase);
+    if constexpr (kU8) {
+      // ||q||^2 of the two rows (kPadNorm beyond nJ: those rows' keys are never read)
+      const int32_t qn0 = __ldg(pd.normJ + wi.sb * kTileRows + row0);
+      const int32_t qn1 = __ldg(pd.normJ + wi.sb * kTileRows + row0 + 8u);
+      int32_t acc0[64], acc1[64];
+      // MMAs of half h (database rows h * 128 .. + 127) of the tile whose K-blocks start at stage s0
+      auto issue = [&](int32_t (&acc)[64], uint32_t h, uint32_t s0) {
         wgmma_fence();
-        const uint32_t a_lo = desc_lo(a_base + kb * kBoxBytes);
-        const uint32_t b_lo = desc_lo(d_base + stage * kStageBytes);
-        const uint32_t ks_here = ks_left < 4u ? ks_left : 4u;
+        uint32_t s = s0, ks_left = ksteps;
+        for (uint32_t kb = 0; kb < nkb; ++kb) {
+          const uint32_t a_lo = desc_lo(a_base + kb * kBoxBytes);
+          const uint32_t b_lo = desc_lo(d_base + s * kStageBytes + h * kBoxBytes);
+          const uint32_t ks_here = ks_left < 4u ? ks_left : 4u;
 #pragma unroll
-        for (uint32_t k = 0; k < 4; ++k) {
-          if (k < ks_here) wgmma_m64n256k16(acc, make_desc(a_lo + 2 * k), make_desc(b_lo + 2 * k), (kb | k) != 0u ? 1u : 0u);
+          for (uint32_t k = 0; k < 4; ++k) {
+            if (k < ks_here) wgmma_m64n128k32_u8(acc, make_desc(a_lo + 2 * k), make_desc(b_lo + 2 * k), (kb | k) != 0u ? 1u : 0u);
+          }
+          ks_left -= ks_here;
+          if (++s == n_stages) s = 0;
         }
         wgmma_commit();
-        if (kb > 0) {  // the previous K-block's MMAs have read their stage
-          wgmma_wait<1>();
-          if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+      };
+      // accumulator column 8 j + 2 q + {0, 1} of rows row0 / row0 + 8 is acc[4 j + {0, 1}] / acc[4 j + {2, 3}];
+      // column c of half h of tile t is database row t * 256 + h * 128 + c, i.e. chunk t * 32 + h * 16 + c / 8.
+      // ||q - a||^2 = ||q||^2 + (||a||^2 - 2 q.a): the chunk minima are taken over the bracket, exactly in s32.
+      // All 8 packed keys of the half are formed first (independent chains the scheduler can interleave), then one
+      // vote skips the insertions unless a lane of the warp holds a key below its current largest: the same keys as
+      // an insertion per candidate, without 8 vote-and-branch points in the dependency chain.
+      auto reduce = [&](const int32_t (&acc)[64], uint32_t t, uint32_t h, uint32_t s0) {
+        const int32_t* nrm = (const int32_t*)(smem_raw + (n_base + s0 * kNormBytes - smem_u32(smem_raw))) + h * 128u;
+        const uint32_t chunk0 = t * (kTileN / kChunk) + h * (kTileN / 2 / kChunk);
+        float x0[4], x1[4];
+        bool any = false;
+#pragma unroll
+        for (uint32_t g = 0; g < 4; ++g) {
+          int32_t p0[4], p1[4];
+#pragma unroll
+          for (uint32_t jj = 0; jj < 4; ++jj) {
+            const uint32_t j = 4 * g + jj;
+            const int2 na = *(const int2*)(nrm + 8 * j + 2 * q);
+            const int32_t* a = acc + 4 * j;
+            p0[jj] = min(na.x - 2 * a[0], na.y - 2 * a[1]);
+            p1[jj] = min(na.x - 2 * a[2], na.y - 2 * a[3]);
+          }
+          const uint32_t cid = chunk0 + 4 * g + q;
+          // exact: real distances are < 2^24
+          const float m0 = (float)(quad_min4(p0[0], p0[1], p0[2], p0[3], q) + qn0);
+          const float m1 = (float)(quad_min4(p1[0], p1[1], p1[2], p1[3], q) + qn1);
+          x0[g] = __uint_as_float((__float_as_uint(m0) & keep_mask) | cid);
+          x1[g] = __uint_as_float((__float_as_uint(m1) & keep_mask) | cid);
+          any |= (x0[g] < key0[kNumKeys - 1]) | (x1[g] < key1[kNumKeys - 1]);
         }
-        prev = stage;
-        ks_left -= ks_here;
-        if (++stage == n_stages) { stage = 0; phase ^= 1u; }
+        if (__any_sync(0xffffffffu, any)) {
+#pragma unroll
+          for (uint32_t g = 0; g < 4; ++g) {
+            key_insert_packed(x0[g], key0);
+            key_insert_packed(x1[g], key1);
+          }
+        }
+      };
+      // the epilogue has read the tile's norms and the MMAs its operands: hand its stages back to the producer
+      auto release = [&](uint32_t s0) {
+        __syncwarp();
+        if (lane == 0)
+          for (uint32_t kb = 0, s = s0; kb < nkb; ++kb) {
+            mbar_arrive(bar_empty + 8 * s);
+            if (++s == n_stages) s = 0;
+          }
+      };
+      mbar_wait(bar_qfull + 8 * qb, qf);
+      uint32_t s_prev = 0;
+      for (uint32_t t = 0; t < ntiles; ++t) {
+        const uint32_t s_t = stage;
+        for (uint32_t kb = 0; kb < nkb; ++kb) {
+          mbar_wait(bar_full + 8 * stage, phase);
+          if (++stage == n_stages) { stage = 0; phase ^= 1u; }
+        }
+        issue(acc0, 0, s_t);
+        if (t > 0) {  // half 1 of the previous tile is done: reduce it while half 0 of this tile runs
+          wgmma_wait<1>();
+          wgmma_fence_operand(acc1);
+          reduce(acc1, t - 1, 1, s_prev);
+          release(s_prev);
+        }
+        issue(acc1, 1, s_t);
+        wgmma_wait<1>();
+        wgmma_fence_operand(acc0);
+        reduce(acc0, t, 0, s_t);
+        s_prev = s_t;
       }
       wgmma_wait<0>();
-      wgmma_fence_operand(acc);
-      if (lane == 0) {
-        mbar_arrive(bar_empty + 8 * prev);
-        if (t + 1 == ntiles) mbar_arrive(bar_qempty + 8 * qb);  // every MMA of the item has read the query block
-      }
-      // accumulator column 8 j + 2 q + {0, 1} of rows row0 / row0 + 8 is acc[4 j + {0, 1}] / acc[4 j + {2, 3}];
-      // column c of the tile is database row t * 256 + c, i.e. chunk t * 32 + c / 8
-      const uint32_t chunk0 = t * (kTileN / kChunk);
+      wgmma_fence_operand(acc1);
+      if (lane == 0) mbar_arrive(bar_qempty + 8 * qb);  // every MMA of the item has read the query block
+      reduce(acc1, ntiles - 1, 1, s_prev);
+      release(s_prev);
+    } else {
+      float acc[128];
+      mbar_wait(bar_qfull + 8 * qb, qf);
+      for (uint32_t t = 0; t < ntiles; ++t) {
+        uint32_t ks_left = ksteps, prev = 0;
+        for (uint32_t kb = 0; kb < nkb; ++kb) {
+          mbar_wait(bar_full + 8 * stage, phase);
+          wgmma_fence();
+          const uint32_t a_lo = desc_lo(a_base + kb * kBoxBytes);
+          const uint32_t b_lo = desc_lo(d_base + stage * kStageBytes);
+          const uint32_t ks_here = ks_left < 4u ? ks_left : 4u;
 #pragma unroll
-      for (uint32_t g = 0; g < 8; ++g) {
-        const float* a = acc + 16 * g;
-        const float m0 = quad_min4(fminf(a[0], a[1]), fminf(a[4], a[5]), fminf(a[8], a[9]), fminf(a[12], a[13]), q);
-        const float m1 = quad_min4(fminf(a[2], a[3]), fminf(a[6], a[7]), fminf(a[10], a[11]), fminf(a[14], a[15]), q);
-        key_insert<true>(m0, chunk0 + 4 * g + q, keep_mask, key0);
-        key_insert<true>(m1, chunk0 + 4 * g + q, keep_mask, key1);
+          for (uint32_t k = 0; k < 4; ++k) {
+            if (k < ks_here) wgmma_m64n256k16(acc, make_desc(a_lo + 2 * k), make_desc(b_lo + 2 * k), (kb | k) != 0u ? 1u : 0u);
+          }
+          wgmma_commit();
+          if (kb > 0) {  // the previous K-block's MMAs have read their stage
+            wgmma_wait<1>();
+            if (lane == 0) mbar_arrive(bar_empty + 8 * prev);
+          }
+          prev = stage;
+          ks_left -= ks_here;
+          if (++stage == n_stages) { stage = 0; phase ^= 1u; }
+        }
+        wgmma_wait<0>();
+        wgmma_fence_operand(acc);
+        if (lane == 0) {
+          mbar_arrive(bar_empty + 8 * prev);
+          if (t + 1 == ntiles) mbar_arrive(bar_qempty + 8 * qb);  // every MMA of the item has read the query block
+        }
+        // accumulator column 8 j + 2 q + {0, 1} of rows row0 / row0 + 8 is acc[4 j + {0, 1}] / acc[4 j + {2, 3}];
+        // column c of the tile is database row t * 256 + c, i.e. chunk t * 32 + c / 8
+        const uint32_t chunk0 = t * (kTileN / kChunk);
+#pragma unroll
+        for (uint32_t g = 0; g < 8; ++g) {
+          const float* a = acc + 16 * g;
+          const float m0 = quad_min4(fminf(a[0], a[1]), fminf(a[4], a[5]), fminf(a[8], a[9]), fminf(a[12], a[13]), q);
+          const float m1 = quad_min4(fminf(a[2], a[3]), fminf(a[6], a[7]), fminf(a[10], a[11]), fminf(a[14], a[15]), q);
+          key_insert<true>(m0, chunk0 + 4 * g + q, keep_mask, key0);
+          key_insert<true>(m1, chunk0 + 4 * g + q, keep_mask, key1);
+        }
       }
     }
     // the four lanes of a quad hold the keys of disjoint chunk sets of the same two rows
@@ -210,25 +323,32 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
   }
 }
 
-static int ring_stages(int nkb, int n_qbuf) {
+static int ring_stages(int nkb, int n_qbuf, uint32_t stage_bytes) {
   const size_t fixed = 1024 + 8 * (2 * kMaxStages + 4) + (size_t)n_qbuf * nkb * kBoxBytes;
-  const int stages = (int)((kSmemOptIn - fixed) / kStageBytes);
+  const int stages = (int)((kSmemOptIn - fixed) / stage_bytes);
   return stages > kMaxStages ? kMaxStages : stages;
 }
 
 int launch_l2_candidates(r3d_ctx* ctx, DeviceWorker& w, const PairDesc* d_pairs, const WorkItem* d_items,
-                         uint32_t n_items, uint32_t* d_keys, int kp_cols, int ksteps) {
+                         uint32_t n_items, uint32_t* d_keys, int dtype, uint32_t dim) {
   if (n_items == 0) return R3D_OK;
-  const int nkb = (kp_cols + kKBlock - 1) / kKBlock;
+  const bool u8 = int_operand(dtype, dim);
+  // u8: 128 columns per K-block, k32 steps; fp16: Kp = operand_cols(dim) columns, 64 per K-block, k16 steps
+  const int nkb = u8 ? ((int)dim + 127) / 128 : (operand_cols((int)dim) + kKBlock - 1) / kKBlock;
+  const int ksteps = u8 ? ((int)dim + 31) / 32 : operand_ksteps((int)dim);
   if (nkb > kMaxKBlocks) return fail(ctx, R3D_ERR_UNSUPPORTED, "descriptor dimension too large for the tensor-core path");
-  const int n_qbuf = ring_stages(nkb, 2) >= 3 ? 2 : 1;  // very wide descriptors: keep the ring deep enough instead
-  const int stages = ring_stages(nkb, n_qbuf);
-  const size_t smem = 1024 + (size_t)n_qbuf * nkb * kBoxBytes + (size_t)stages * kStageBytes + 8 * (2 * kMaxStages + 4);
-  R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(k_l2_candidates, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  const uint32_t stage_bytes = kStageBytes + (u8 ? kNormBytes : 0u);
+  // u8 consumers hold one tile's stages while they wait for the next tile's: the ring needs two tiles
+  const int min_stages = u8 ? 2 * nkb : 3;
+  const int n_qbuf = ring_stages(nkb, 2, stage_bytes) >= min_stages ? 2 : 1;  // very wide descriptors: keep the ring deep enough instead
+  const int stages = ring_stages(nkb, n_qbuf, stage_bytes);
+  const size_t smem = 1024 + (size_t)n_qbuf * nkb * kBoxBytes + (size_t)stages * stage_bytes + 8 * (2 * kMaxStages + 4);
+  auto kern = u8 ? k_l2_candidates<true> : k_l2_candidates<false>;
+  R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const uint32_t grid = n_items < (uint32_t)w.sm_count ? n_items : (uint32_t)w.sm_count;
-  k_l2_candidates<<<grid, kThreads, smem, w.stream>>>((const CUtensorMap*)w.d_tmapQ, (const CUtensorMap*)w.d_tmapD,
-                                                      d_pairs, d_items, n_items, d_keys, (uint32_t)nkb, (uint32_t)ksteps,
-                                                      (uint32_t)stages, (uint32_t)n_qbuf);
+  kern<<<grid, kThreads, smem, w.stream>>>((const CUtensorMap*)w.d_tmapQ, (const CUtensorMap*)w.d_tmapD, d_pairs, d_items,
+                                           n_items, d_keys, (uint32_t)nkb, (uint32_t)ksteps, (uint32_t)stages,
+                                           (uint32_t)n_qbuf);
   R3D_CUDA_TRY(ctx, cudaGetLastError());
   return R3D_OK;
 }

@@ -36,6 +36,7 @@ double now_ms() {
 }
 
 float pair_eps(const ViewDev& vi, const ViewDev& vj) {
+  if (vi.int_ops && vj.int_ops) return 0.f;  // integer path: exact keys (the chunk-id packing is covered by pack_rel)
   const double nI = vi.max_norm, nJ = vj.max_norm;
   double e = 2.0 * ((double)vi.max_dnorm * nJ + (double)vi.max_hnorm * (double)vj.max_dnorm);
   e += std::ldexp(nI * nI + nJ * nJ, -21);         // two-piece fp16 split of the squared norms
@@ -152,6 +153,7 @@ static int match_on_worker(r3d_ctx* ctx, DeviceWorker& w, const uint32_t* pairs,
     pd.I = I; pd.J = J; pd.nI = vi.n; pd.nJ = vj.n; pd.nI_pad = vi.n_pad; pd.nJ_pad = vj.n_pad;
     pd.slotI = w.view_slot[I]; pd.slotJ = w.view_slot[J];
     pd.descI = vi.d_desc; pd.descJ = vj.d_desc;
+    pd.normI = vi.d_norm; pd.normJ = vj.d_norm;
     pd.use_tc = (!cascade && (flags & R3D_MATCH_EXACT_SCAN) == 0 && vi.tc_ok && vj.tc_ok && vi.n_pad <= kMaxDbRowsTC && vi.kp <= kMaxKBlocks * kKBlock) ? 1u : 0u;
     pd.eps_abs = pair_eps(vi, vj);
     {
@@ -162,7 +164,6 @@ static int match_on_worker(r3d_ctx* ctx, DeviceWorker& w, const uint32_t* pairs,
     all.push_back(bp);
   }
   if (all.empty()) return R3D_OK;
-  const int kp = operand_cols((int)dim);
   if (want_matches && (flags & R3D_MATCH_NO_COORD_DEDUP) == 0) {
     // per-view tables of the descent-free coordinate de-duplication (match_post.cpp), built once per upload
     std::vector<ViewDev*> need;
@@ -292,7 +293,7 @@ static int match_on_worker(r3d_ctx* ctx, DeviceWorker& w, const uint32_t* pairs,
     R3D_CUDA_TRY(ctx, cudaEventRecord(o.ev[0], w.stream));
     if (any_tc) {
       rc = launch_l2_candidates(ctx, w, (const PairDesc*)w.d_pairs, (const WorkItem*)w.d_items, (uint32_t)hitems->size(),
-                                (uint32_t*)w.d_keys, kp, operand_ksteps((int)dim));
+                                (uint32_t*)w.d_keys, dtype, dim);
       if (rc) return rc;
       launches += 1;
     }

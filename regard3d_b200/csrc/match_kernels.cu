@@ -1,5 +1,6 @@
 // match_kernels.cu -- CUDA-core kernels of the putative-matching path (sm_90a):
-//   k_view_stats / k_view_prepare : build the fp16 tensor-core operands of a view (+ error constants)
+//   k_view_stats / k_view_prepare : build the fp16 tensor-core operands of a view (+ error constants; the exact
+//                                   norms of the integer path)
 //   k_rerank                      : exact re-rank of the candidate chunks, certification, ratio test
 //   k_exact_scan                  : exact brute-force 2-NN for listed queries (uncertified / forced)
 //
@@ -195,10 +196,15 @@ __device__ __forceinline__ float warp_max(float v) {
 }
 
 // stats[0] = max ||a||^2, [1] = max ||fp16(a)||^2, [2] = max ||a - fp16(a)||^2, [3] = max |a_k|
-__global__ void k_view_stats(const void* __restrict__ desc, int dtype, uint32_t n, uint32_t dim, float* stats) {
+// norms (integer path only, rows [0, n_pad)): the exact ||a||^2, kPadNorm on padding rows
+__global__ void k_view_stats(const void* __restrict__ desc, int dtype, uint32_t n, uint32_t n_pad, uint32_t dim,
+                             float* stats, int32_t* __restrict__ norms) {
   const uint32_t lane = threadIdx.x & 31u;
   const uint32_t row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-  if (row >= n) return;
+  if (row >= n) {
+    if (norms && row < n_pad && lane == 0) norms[row] = kPadNorm;
+    return;
+  }
   double n2 = 0, h2 = 0, d2 = 0;
   float ma = 0.f;
   for (uint32_t k = lane; k < dim; k += 32) {
@@ -212,6 +218,7 @@ __global__ void k_view_stats(const void* __restrict__ desc, int dtype, uint32_t 
   }
   n2 = warp_sum(n2); h2 = warp_sum(h2); d2 = warp_sum(d2); ma = warp_max(ma);
   if (lane == 0) {
+    if (norms) norms[row] = (int32_t)n2;  // a sum of integer squares below 2^53: exact
     // non-negative floats order like their bit patterns; round UP so the maxima stay upper bounds
     atomicMax((unsigned int*)&stats[0], __float_as_uint(__double2float_ru(n2)));
     atomicMax((unsigned int*)&stats[1], __float_as_uint(__double2float_ru(h2)));
@@ -282,9 +289,11 @@ __global__ void k_view_prepare(const void* __restrict__ desc, int dtype, uint32_
 // ------------------------------------------------------------------------------------------------
 int launch_view_stats(r3d_ctx* ctx, DeviceWorker& w, ViewDev& v) {
   R3D_CUDA_TRY(ctx, cudaMemsetAsync(v.d_stats, 0, 4 * sizeof(float), w.stream));
-  if (v.n == 0) return R3D_OK;
+  const uint32_t rows = v.int_ops ? v.n_pad : v.n;
+  if (rows == 0) return R3D_OK;
   const int wpb = 8;
-  k_view_stats<<<(v.n + wpb - 1) / wpb, wpb * 32, 0, w.stream>>>(v.d_desc, (int)v.dtype, v.n, v.dim, v.d_stats);
+  k_view_stats<<<(rows + wpb - 1) / wpb, wpb * 32, 0, w.stream>>>(v.d_desc, (int)v.dtype, v.n, v.n_pad, v.dim, v.d_stats,
+                                                                  v.d_norm);
   R3D_CUDA_TRY(ctx, cudaGetLastError());
   return R3D_OK;
 }

@@ -42,12 +42,19 @@ inline int pad_up(int x, int m) { return (x + m - 1) / m * m; }
 int operand_col_align();  // 16, or 64 (R3D_KP_ALIGN) to make operand rows 128-byte aligned
 inline int operand_ksteps(int dim) { return (pad_up(dim, 16) + kBiasCols) / 16; }
 inline int operand_cols(int dim) { return pad_up(pad_up(dim, 16) + kBiasCols, operand_col_align()); }  // Kp
+// uint8 descriptors whose rows are whole 16-byte TMA strides take the integer tensor-core path: the candidate kernel
+// reads d_desc directly and computes exact squared distances (u8 x u8 -> s32 wgmma), no fp16 operands
+inline bool int_operand(int dtype, uint32_t dim) { return dtype == R3D_U8 && dim > 0 && dim % 16 == 0 && dim <= 256; }
+constexpr int32_t kPadNorm = 1 << 28;  // ||a||^2 of a padding row of the integer path: above every real distance
+                                       // (< 2^24 for dim <= 256), and no epilogue sum reaches 2^31
 
 struct ViewDev {
   uint32_t n = 0, dim = 0, dtype = 0, n_pad = 0, kp = 0;
   void* d_desc = nullptr;    // original descriptors [n][dim] (f32 or u8): exact re-rank operand
   __half* d_opQ = nullptr;   // query-role operand    [n_pad][kp]: -2*b | S0 S1 q0 q1 0...
   __half* d_opD = nullptr;   // database-role operand [n_pad][kp]:    a  | p0 p1 S0 S1 0...
+  int32_t* d_norm = nullptr; // integer path: exact ||a||^2 [n_pad], kPadNorm on padding rows
+  bool int_ops = false;      // int_operand(dtype, dim): no d_opQ / d_opD, kp = 0
   float2* d_xy = nullptr;    // positions [n]
   std::vector<float> h_xy;   // host copy (coordinate de-duplication, RANSAC set-up)
   std::vector<uint32_t> h_yrank;   // build_view_ranks(): tables of the descent-free coordinate de-duplication
@@ -91,8 +98,10 @@ struct PairDesc {            // one entry per pair of a batch (device + host)
   uint32_t chunk_bits;       // low mantissa bits of a key that hold the chunk id (<= kChunkBits)
   const void* descI;         // original descriptors of I / J (device)
   const void* descJ;
+  const int32_t* normI;      // integer path: exact squared norms of I / J (ViewDev::d_norm), else null
+  const int32_t* normJ;
 };
-static_assert(sizeof(PairDesc) == 64, "PairDesc layout");
+static_assert(sizeof(PairDesc) == 80, "PairDesc layout");
 
 struct WorkItem { uint32_t pair; uint32_t sb; };  // sb: super-block (256 query rows) index
 
@@ -217,9 +226,10 @@ inline void parallel_for(int n_threads, size_t n, F&& f) {
 // operand preparation
 int launch_view_stats(r3d_ctx* ctx, DeviceWorker& w, ViewDev& v);
 int launch_view_prepare(r3d_ctx* ctx, DeviceWorker& w, ViewDev& v, int e0);
-// tensor-core candidate kernel: persistent CTAs (TMA + wgmma); work items are 128-query blocks
+// tensor-core candidate kernel: persistent CTAs (TMA + wgmma); work items are 128-query blocks.  The operand kind
+// (fp16 operands or the integer path) follows from dtype and dim, which every pair of a call shares.
 int launch_l2_candidates(r3d_ctx* ctx, DeviceWorker& w, const PairDesc* d_pairs, const WorkItem* d_items,
-                         uint32_t n_items, uint32_t* d_keys, int kp_cols, int ksteps);
+                         uint32_t n_items, uint32_t* d_keys, int dtype, uint32_t dim);
 // exact re-rank + ratio
 int launch_rerank_list(r3d_ctx* ctx, DeviceWorker& w, const PairDesc* d_pairs, const uint32_t* d_keys, const void* d_parts,
                        const uint2* d_list, const uint32_t* d_list_count, uint32_t max_list, uint32_t dim, int dtype,

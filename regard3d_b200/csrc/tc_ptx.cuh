@@ -6,7 +6,7 @@
 namespace r3d {
 namespace tcx {
 
-constexpr uint32_t kBoxBytes = kTileRows * kKBlock * 2;  // one 128-row x 64-column fp16 TMA box: 16384
+constexpr uint32_t kBoxBytes = kTileRows * kKBlock * 2;  // one 128-row x 128-byte TMA box (64 fp16 / 128 u8 columns)
 constexpr uint32_t kKeySentinel = 0x7f7fffffu;            // FLT_MAX
 
 // ---- PTX wrappers ------------------------------------------------------------------------------
@@ -39,6 +39,11 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
   asm volatile(
       "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
       ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(bar) : "memory");
+}
+// contiguous global -> shared copy (bytes and both addresses multiples of 16), completing on an mbarrier
+__device__ __forceinline__ void bulk_load(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
 // one lane of a converged warp (all 32 lanes must execute this)
@@ -114,21 +119,57 @@ __device__ __forceinline__ void wgmma_m64n256k16(float (&d)[128], uint64_t a_des
       : "l"(a_desc), "l"(b_desc), "r"(scale_d));
 }
 
-// A chunk minimum, packed with its chunk id, inserted into the sorted key set of its query row.
-template <bool kVote = false>
-__device__ __forceinline__ void key_insert(float m, uint32_t chunk_id, uint32_t keep_mask, float (&key)[kNumKeys]) {
-  float x = __uint_as_float((__float_as_uint(m) & keep_mask) | chunk_id);
-  // A key that is not below the current largest kept key leaves the set unchanged (the network would carry it
-  // through every level).  After t chunks a lane inserts with probability ~ kNumKeys / t, so most chunks need no
-  // insertion in ANY lane of the warp: one vote skips the 11-instruction network (warp-uniform branch).
-  if (kVote && !__any_sync(0xffffffffu, x < key[kNumKeys - 1])) return;
+__device__ __forceinline__ void wgmma_fence_operand(int32_t (&d)[64]) {
 #pragma unroll
-  for (int i = 0; i < kNumKeys - 1; ++i) {  // sorted insertion network: 2 FMNMX per level
+  for (int i = 0; i < 64; ++i) asm volatile("" : "+r"(d[i])::"memory");
+}
+
+// D (64 x 128, s32, registers) (+)= A (64 x 32, u8, shared) x B (128 x 32, u8, shared)^T; both operands K-major.
+// Exact integer products.  One K-step of 32 u8 columns is 32 bytes, the same descriptor advance as an fp16 k16 step,
+// and the accumulator fragment has the layout of the f32 one.
+__device__ __forceinline__ void wgmma_m64n128k32_u8(int32_t (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t"
+      ".reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.s32.u8.u8 {"
+      "%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+      "}, %64, %65, p;\n\t"
+      "}"
+      : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+        "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+        "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+        "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+        "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+        "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+        "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+        "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(scale_d));
+}
+
+// A chunk minimum, packed with its chunk id, inserted into the sorted key set of its query row.
+// A packed key inserted into the sorted key set of its query row (sorted insertion network: 2 FMNMX per level).
+__device__ __forceinline__ void key_insert_packed(float x, float (&key)[kNumKeys]) {
+#pragma unroll
+  for (int i = 0; i < kNumKeys - 1; ++i) {
     const float hi = fmaxf(key[i], x);
     key[i] = fminf(key[i], x);
     x = hi;
   }
   key[kNumKeys - 1] = fminf(key[kNumKeys - 1], x);
+}
+
+template <bool kVote = false>
+__device__ __forceinline__ void key_insert(float m, uint32_t chunk_id, uint32_t keep_mask, float (&key)[kNumKeys]) {
+  const float x = __uint_as_float((__float_as_uint(m) & keep_mask) | chunk_id);
+  // A key that is not below the current largest kept key leaves the set unchanged (the network would carry it
+  // through every level).  After t chunks a lane inserts with probability ~ kNumKeys / t, so most chunks need no
+  // insertion in ANY lane of the warp: one vote skips the 11-instruction network (warp-uniform branch).
+  if (kVote && !__any_sync(0xffffffffu, x < key[kNumKeys - 1])) return;
+  key_insert_packed(x, key);
 }
 
 }  // namespace tcx
