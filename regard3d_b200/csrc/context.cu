@@ -113,24 +113,38 @@ static void free_worker(DeviceWorker& w) {
 }
 
 // Encode the two TMA descriptors of a view: 2-D fp16 [n_pad][kp], box = 64 columns x 128 rows,
-// 128-byte swizzle (the K-major SWIZZLE_128B operand layout of wgmma).  Integer path: one 2-D uint8 map over the
-// descriptors themselves ([n][dim], box = 128 columns x 128 rows; TMA zero-fills rows >= n and columns >= dim)
-// serves both roles.
+// 128-byte swizzle (the K-major SWIZZLE_128B operand layout of wgmma).  Integer path: two uint8 maps over the
+// descriptors themselves, both with 128-column boxes (TMA zero-fills columns >= dim):
+//   query role     2-D [n][dim], box 128 rows in natural order (rows >= n zero-filled)
+//   database role  5-D (column, e, q, jj, g) with strides (1, D, 8 D, 2 D, 32 D) bytes, box {128, 2, 4, 4, 4}: database
+//                  row 32 g + 8 q + 2 jj + e lands in shared-memory row 32 g + 8 jj + 2 q + e, a 4 x 4 transpose of
+//                  row pairs inside every 32-row group, so that the accumulator columns of one lane of a wgmma quad
+//                  are 8 consecutive database rows (k_l2_candidates.cu).  The map covers ceil(n / 32) whole groups:
+//                  d_desc is padded to that many rows with zeros (r3d_upload_regions), later groups are zero-filled.
 static int encode_view_maps(r3d_ctx* ctx, DeviceWorker& w, ViewDev& v, uint32_t slot) {
   PFN_encodeTiled enc = get_encode_tiled();
   if (!enc) return fail(ctx, R3D_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   CUtensorMap maps[2];
   void* bases[2] = {(void*)v.d_opQ, (void*)v.d_opD};
   if (v.int_ops) {
-    cuuint64_t gdim[2] = {(cuuint64_t)v.dim, (cuuint64_t)std::max<uint32_t>(v.n, 1)};
-    cuuint64_t gstride[1] = {(cuuint64_t)v.dim};
+    const cuuint64_t D = v.dim;
+    cuuint64_t gdim[2] = {D, (cuuint64_t)std::max<uint32_t>(v.n, 1)};
+    cuuint64_t gstride[1] = {D};
     cuuint32_t box[2] = {128, (cuuint32_t)kTileRows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = enc(&maps[0], CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, v.d_desc, gdim, gstride, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(ctx, R3D_ERR_CUDA, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
-    maps[1] = maps[0];
+    cuuint64_t gdim5[5] = {D, 2, 4, 4, (cuuint64_t)(int_desc_rows(v.n) / kGroupRows)};
+    cuuint64_t gstride5[4] = {D, 8 * D, 2 * D, kGroupRows * D};
+    cuuint32_t box5[5] = {128, 2, 4, 4, kTileRows / kGroupRows};
+    cuuint32_t estr5[5] = {1, 1, 1, 1, 1};
+    r = enc(&maps[1], CU_TENSOR_MAP_DATA_TYPE_UINT8, 5, v.d_desc, gdim5, gstride5, box5, estr5,
+            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+            CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS)
+      return fail(ctx, R3D_ERR_CUDA, "cuTensorMapEncodeTiled failed for the permuted database map: " + std::to_string((int)r));
   }
   for (int m = 0; m < 2 && !v.int_ops; ++m) {
     cuuint64_t gdim[2] = {(cuuint64_t)v.kp, (cuuint64_t)(v.tc_ok ? v.n_pad : (uint32_t)kRowPad)};
@@ -331,7 +345,9 @@ int r3d_upload_regions(r3d_ctx* ctx, uint32_t view_id, const void* desc, uint32_
     v.tc_ok = v.int_ops || dim <= 240;  // fp16: Kp <= 256 columns; wider descriptors are matched by the exact scan only
     v.kp = v.int_ops ? 0u : (uint32_t)operand_cols((int)(dim && v.tc_ok ? dim : 16));
     const size_t rb = dtype == R3D_F32 ? (size_t)dim * 4 : (size_t)dim;
-    v.d_desc = pool_alloc(w, std::max<size_t>(rb * std::max<uint32_t>(n, 1), 16));  // >= one row: the u8 map's extent
+    // >= one row: the extent of the u8 maps; integer path: whole 32-row groups of the permuted database map
+    const uint32_t desc_rows = v.int_ops ? int_desc_rows(n) : std::max<uint32_t>(n, 1);
+    v.d_desc = pool_alloc(w, std::max<size_t>(rb * desc_rows, 16));
     if (v.int_ops) {
       v.d_norm = (int32_t*)pool_alloc(w, (size_t)v.n_pad * sizeof(int32_t));
     } else {
@@ -351,6 +367,8 @@ int r3d_upload_regions(r3d_ctx* ctx, uint32_t view_id, const void* desc, uint32_
       ~ViewGuard() { if (armed) { cudaStreamSynchronize(w.stream); free_view(w, v); } }
     } guard{w, v};
     if (n) R3D_CUDA_TRY(ctx, cudaMemcpyAsync(v.d_desc, desc, rb * n, cudaMemcpyHostToDevice, w.stream));
+    if (v.int_ops && desc_rows > n)  // the database map reads these rows: zeros, so that padding keys are kPadNorm + ||q||^2
+      R3D_CUDA_TRY(ctx, cudaMemsetAsync((char*)v.d_desc + rb * n, 0, rb * (desc_rows - n), w.stream));
     if (xy && n) {
       R3D_CUDA_TRY(ctx, cudaMemcpyAsync(v.d_xy, xy, (size_t)n * sizeof(float2), cudaMemcpyHostToDevice, w.stream));
       v.h_xy.assign(xy, xy + 2 * (size_t)n);

@@ -15,8 +15,9 @@
 //                    registers.
 //     fp16: per 256-row tile, m64n256k16 into 128 f32 registers, then the epilogue.
 //     u8:   per 128-row half tile, m64n128k32 into one of two 64-register s32 accumulators; the epilogue of half h
-//           runs while the MMAs of half h + 1 are in the tensor pipe (at the integer rate the MMAs of a half take
-//           about as long as its epilogue).
+//           runs while the MMAs of half h + 1 are in the tensor pipe.  The database map loads every 32-row group
+//           with its row pairs transposed (context.cu), so each lane of a quad holds whole chunks: the chunk minima
+//           take no shuffle, and only the keys below their set's largest are inserted, in warp-uniform rounds.
 // Barriers: full[s] (TMA bytes landed), empty[s] (the 8 consumer warps are done with the stage), qfull / qempty the
 // same for the query buffers.
 #include "r3d_internal.cuh"
@@ -37,17 +38,18 @@ constexpr uint32_t kThreads = 384;
 constexpr size_t kSmemOptIn = 232448;             // 227 KB: the largest dynamic shared memory of one block on sm_90
 static_assert(kChunk == 8, "the epilogue reduces one 8-column block of the wgmma accumulator per chunk");
 
-__device__ __forceinline__ float vmin(float a, float b) { return fminf(a, b); }
-__device__ __forceinline__ int32_t vmin(int32_t a, int32_t b) { return min(a, b); }
-
-// Minima of four consecutive chunks of one accumulator row, spread over the 4 lanes of a quad (2 columns each),
+// fp16: minima of four consecutive chunks of one accumulator row, spread over the 4 lanes of a quad (2 columns each),
 // reduced and scattered so that lane q of the quad ends with the minimum of chunk q: 3 shuffles for 4 chunks.
-template <typename T>
-__device__ __forceinline__ T quad_min4(T p0, T p1, T p2, T p3, uint32_t q) {
+__device__ __forceinline__ float quad_min4(float p0, float p1, float p2, float p3, uint32_t q) {
   const bool b1 = (q & 2u) != 0, b0 = (q & 1u) != 0;
-  const T k0 = vmin(b1 ? p2 : p0, __shfl_xor_sync(0xffffffffu, b1 ? p0 : p2, 2));
-  const T k1 = vmin(b1 ? p3 : p1, __shfl_xor_sync(0xffffffffu, b1 ? p1 : p3, 2));
-  return vmin(b0 ? k1 : k0, __shfl_xor_sync(0xffffffffu, b0 ? k0 : k1, 1));
+  const float k0 = fminf(b1 ? p2 : p0, __shfl_xor_sync(0xffffffffu, b1 ? p0 : p2, 2));
+  const float k1 = fminf(b1 ? p3 : p1, __shfl_xor_sync(0xffffffffu, b1 ? p1 : p3, 2));
+  return fminf(b0 ? k1 : k0, __shfl_xor_sync(0xffffffffu, b0 ? k0 : k1, 1));
+}
+
+// u8: the minimum of one chunk, held whole by one lane (3 VIMNMX3 + 1 VIMNMX)
+__device__ __forceinline__ int32_t min8(const int32_t (&v)[8]) {
+  return __vimin3_s32(__vimin3_s32(v[0], v[1], v[2]), __vimin3_s32(v[3], v[4], v[5]), min(v[6], v[7]));
 }
 
 // the kNumKeys smallest keys of this lane's set and the set of lane ^ d (the keys of different chunks differ)
@@ -134,8 +136,15 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
             const uint32_t dst = d_base + stage * kStageBytes;
             const bool norms = kU8 && kb == 0;  // the tile's norms travel with its first K-block
             mbar_arrive_expect_tx(bar_full + 8 * stage, kStageBytes + (norms ? kNormBytes : 0u));
-            tma_load_2d(dst, md, (int)(kb * kBoxCols), (int)(t * kTileN), bar_full + 8 * stage);
-            tma_load_2d(dst + kBoxBytes, md, (int)(kb * kBoxCols), (int)(t * kTileN + kTileRows), bar_full + 8 * stage);
+            if constexpr (kU8) {  // the permuted database map (context.cu): 4 groups of 32 rows per box
+              constexpr uint32_t kGroupsPerBox = kTileRows / kGroupRows;
+              tma_load_5d(dst, md, (int)(kb * kBoxCols), 0, 0, 0, (int)(t * 2 * kGroupsPerBox), bar_full + 8 * stage);
+              tma_load_5d(dst + kBoxBytes, md, (int)(kb * kBoxCols), 0, 0, 0, (int)(t * 2 * kGroupsPerBox + kGroupsPerBox),
+                          bar_full + 8 * stage);
+            } else {
+              tma_load_2d(dst, md, (int)(kb * kBoxCols), (int)(t * kTileN), bar_full + 8 * stage);
+              tma_load_2d(dst + kBoxBytes, md, (int)(kb * kBoxCols), (int)(t * kTileN + kTileRows), bar_full + 8 * stage);
+            }
             if (norms) bulk_load(n_base + stage * kNormBytes, pd.normI + t * kTileN, kNormBytes, bar_full + 8 * stage);
           }
           __syncwarp();
@@ -185,42 +194,50 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
         }
         wgmma_commit();
       };
-      // accumulator column 8 j + 2 q + {0, 1} of rows row0 / row0 + 8 is acc[4 j + {0, 1}] / acc[4 j + {2, 3}];
-      // column c of half h of tile t is database row t * 256 + h * 128 + c, i.e. chunk t * 32 + h * 16 + c / 8.
-      // ||q - a||^2 = ||q||^2 + (||a||^2 - 2 q.a): the chunk minima are taken over the bracket, exactly in s32.
-      // All 8 packed keys of the half are formed first (independent chains the scheduler can interleave), then one
-      // vote skips the insertions unless a lane of the warp holds a key below its current largest: the same keys as
-      // an insertion per candidate, without 8 vote-and-branch points in the dependency chain.
+      // Accumulator column 8 j + 2 q + {0, 1} of rows row0 / row0 + 8 is acc[4 j + {0, 1}] / acc[4 j + {2, 3}].  The
+      // database map permutes every 32-row group (context.cu): column 32 g + 8 jj + 2 q + e of half h of tile t holds
+      // database row t * 256 + h * 128 + 32 g + 8 q + 2 jj + e.  So the 8 columns of lane q in group g (j = 4 g + jj)
+      // are the 8 rows of chunk t * 32 + h * 16 + 4 g + q, and their norms are 8 consecutive words of shared memory.
+      // ||q - a||^2 = ||q||^2 + (||a||^2 - 2 q.a): each lane takes the minima of its chunks over the bracket, exactly
+      // in s32 and without leaving its registers.
+      // A candidate can only enter its set if it is below the set's largest key, which never grows: the candidates
+      // that pass are inserted in warp-uniform rounds, one per set and lane per round (FLT_MAX, a no-op of the
+      // network, where a lane has none left).  The keys of a set differ in their chunk bits, so the order of the
+      // insertions does not change the set.
       auto reduce = [&](const int32_t (&acc)[64], uint32_t t, uint32_t h, uint32_t s0) {
-        const int32_t* nrm = (const int32_t*)(smem_raw + (n_base + s0 * kNormBytes - smem_u32(smem_raw))) + h * 128u;
-        const uint32_t chunk0 = t * (kTileN / kChunk) + h * (kTileN / 2 / kChunk);
+        const int32_t* nrm = (const int32_t*)(smem_raw + (n_base + s0 * kNormBytes - smem_u32(smem_raw))) + h * 128u + 8u * q;
+        const uint32_t chunk0 = t * (kTileN / kChunk) + h * (kTileN / 2 / kChunk) + q;
         float x0[4], x1[4];
-        bool any = false;
+        uint32_t p0 = 0, p1 = 0;  // bit g: x0[g] / x1[g] is still to be inserted
 #pragma unroll
         for (uint32_t g = 0; g < 4; ++g) {
-          int32_t p0[4], p1[4];
-#pragma unroll
-          for (uint32_t jj = 0; jj < 4; ++jj) {
-            const uint32_t j = 4 * g + jj;
-            const int2 na = *(const int2*)(nrm + 8 * j + 2 * q);
-            const int32_t* a = acc + 4 * j;
-            p0[jj] = min(na.x - 2 * a[0], na.y - 2 * a[1]);
-            p1[jj] = min(na.x - 2 * a[2], na.y - 2 * a[3]);
-          }
-          const uint32_t cid = chunk0 + 4 * g + q;
+          const int4 na = *(const int4*)(nrm + kGroupRows * g);
+          const int4 nb = *(const int4*)(nrm + kGroupRows * g + 4);
+          const int32_t* a = acc + 16 * g;
+          const int32_t d0[8] = {na.x - 2 * a[0], na.y - 2 * a[1], na.z - 2 * a[4], na.w - 2 * a[5],
+                                 nb.x - 2 * a[8], nb.y - 2 * a[9], nb.z - 2 * a[12], nb.w - 2 * a[13]};
+          const int32_t d1[8] = {na.x - 2 * a[2], na.y - 2 * a[3], na.z - 2 * a[6], na.w - 2 * a[7],
+                                 nb.x - 2 * a[10], nb.y - 2 * a[11], nb.z - 2 * a[14], nb.w - 2 * a[15]};
+          const uint32_t cid = chunk0 + 4 * g;
           // exact: real distances are < 2^24
-          const float m0 = (float)(quad_min4(p0[0], p0[1], p0[2], p0[3], q) + qn0);
-          const float m1 = (float)(quad_min4(p1[0], p1[1], p1[2], p1[3], q) + qn1);
+          const float m0 = (float)(min8(d0) + qn0);
+          const float m1 = (float)(min8(d1) + qn1);
           x0[g] = __uint_as_float((__float_as_uint(m0) & keep_mask) | cid);
           x1[g] = __uint_as_float((__float_as_uint(m1) & keep_mask) | cid);
-          any |= (x0[g] < key0[kNumKeys - 1]) | (x1[g] < key1[kNumKeys - 1]);
+          p0 |= (x0[g] < key0[kNumKeys - 1] ? 1u : 0u) << g;
+          p1 |= (x1[g] < key1[kNumKeys - 1] ? 1u : 0u) << g;
         }
-        if (__any_sync(0xffffffffu, any)) {
+        while (__any_sync(0xffffffffu, (p0 | p1) != 0u)) {
+          float y0 = __uint_as_float(kKeySentinel), y1 = y0;
 #pragma unroll
-          for (uint32_t g = 0; g < 4; ++g) {
-            key_insert_packed(x0[g], key0);
-            key_insert_packed(x1[g], key1);
+          for (int g = 3; g >= 0; --g) {  // the lowest pending candidate of each set
+            if (p0 & (1u << g)) y0 = x0[g];
+            if (p1 & (1u << g)) y1 = x1[g];
           }
+          p0 &= p0 - 1u;
+          p1 &= p1 - 1u;
+          key_insert_packed(y0, key0);
+          key_insert_packed(y1, key1);
         }
       };
       // the epilogue has read the tile's norms and the MMAs its operands: hand its stages back to the producer

@@ -47,10 +47,14 @@ inline int operand_cols(int dim) { return pad_up(pad_up(dim, 16) + kBiasCols, op
 inline bool int_operand(int dtype, uint32_t dim) { return dtype == R3D_U8 && dim > 0 && dim % 16 == 0 && dim <= 256; }
 constexpr int32_t kPadNorm = 1 << 28;  // ||a||^2 of a padding row of the integer path: above every real distance
                                        // (< 2^24 for dim <= 256), and no epilogue sum reaches 2^31
+constexpr uint32_t kGroupRows = 32;    // integer path: database rows permuted together by the database tensor map
+// rows of d_desc on the integer path: whole groups of the database map (zeros beyond n), at least one
+inline uint32_t int_desc_rows(uint32_t n) { return (std::max<uint32_t>(n, 1) + kGroupRows - 1) / kGroupRows * kGroupRows; }
 
 struct ViewDev {
   uint32_t n = 0, dim = 0, dtype = 0, n_pad = 0, kp = 0;
   void* d_desc = nullptr;    // original descriptors [n][dim] (f32 or u8): exact re-rank operand
+                             // (integer path: zero rows up to int_desc_rows(n))
   __half* d_opQ = nullptr;   // query-role operand    [n_pad][kp]: -2*b | S0 S1 q0 q1 0...
   __half* d_opD = nullptr;   // database-role operand [n_pad][kp]:    a  | p0 p1 S0 S1 0...
   int32_t* d_norm = nullptr; // integer path: exact ||a||^2 [n_pad], kPadNorm on padding rows
