@@ -279,6 +279,45 @@ typedef struct {
 void r3d_sfm_ba_default_options(r3d_sfm_ba_options* o);
 int r3d_sfm_bundle_adjust(r3d_ctx* ctx, r3d_sfm_data* sd, const r3d_sfm_ba_options* opt, r3d_ba_summary* summary);
 
+/* ---- relative pose of every image pair (global SfM) ------------------------------------------ */
+#define R3D_RELPOSE_OK 0
+#define R3D_RELPOSE_TOO_FEW 1        /* <= 5 matches */
+#define R3D_RELPOSE_NO_INTRINSIC 2   /* focal <= 0 in either view */
+#define R3D_RELPOSE_NO_MODEL 3       /* AC-RANSAC: minNFA >= 0 or fewer than 2.5 * 5 inliers */
+#define R3D_RELPOSE_CHEIRALITY 4     /* no motion of E puts an inlier in front of both cameras */
+typedef struct {
+  double precision_px;       /* 2.5: RelativePose_Info::initial_residual_tolerance = Square(2.5) */
+  uint32_t max_iter;         /* 256 */
+  int refine;                /* 1: bRefine_using_BA, the two-view bundle adjustment of each pair */
+  r3d_ba_options ba;         /* refine_intrinsics must be 0 (the pair's intrinsics stay fixed); prior_huber_a unused */
+} r3d_relpose_options;
+void r3d_relpose_default_options(r3d_relpose_options* o);  /* 2.5, 256, 1, r3d_ba_default_options with intrinsics fixed */
+typedef struct {
+  uint32_t I, J;
+  int status;                        /* R3D_RELPOSE_* */
+  uint32_t n_inliers;
+  double found_residual_precision;   /* AC-RANSAC errorMax, px */
+  double E[9];                       /* K2^T F K1 of AC-RANSAC's best model F: the 5-point solver's E up to rounding */
+  double rotation[9], translation[3];/* X_J = R X_I + t, R row-major; |t| = 1 before refinement */
+  uint32_t ba_iterations, ba_successful_steps;
+  int ba_termination;                /* as r3d_ba_summary.termination; -1: not refined.  4 (failure): R, t unrefined */
+  double ba_initial_cost, ba_final_cost;
+} r3d_relative_pose;
+/* Replaces the loop body of GlobalSfMReconstructionEngine_RelativeMotions::Compute_Relative_Rotations (OpenMVG 1.4
+ * sfm_global_engine_relative_motions.cpp, reached from src/threads/R3DTriangulationThread.cpp:201-250 on
+ * matches.e.txt) for every pair of `matches`: robustRelativePose (AC-RANSAC with the essential adaptor, 5-point solver,
+ * precision_px / max_iter), MotionFromEssential + the cheirality test, then the two-view Bundle_Adjustment_Ceres of the
+ * pair (both poses and every match's DLT point, intrinsics fixed) and RelativeCameraMotion.  Positions come from
+ * r3d_upload_regions; views[v] gives the size and pinhole K of view v (as for R3D_MODEL_E).  out: one entry per pair
+ * of `matches`, in map order.  inliers (may be NULL): the AC-RANSAC inliers (residual order) of the OK pairs. */
+int r3d_relative_poses(r3d_ctx* ctx, const r3d_matches* matches, const r3d_view_info* views, uint32_t n_views,
+                       const r3d_relpose_options* opt, r3d_relative_pose* out, r3d_matches** inliers);
+typedef struct {
+  double ms_ransac, ms_cheirality, ms_refine, ms_device_total, ms_host;  /* last r3d_relative_poses call */
+  uint64_t kernel_launches, ba_iterations;
+} r3d_relpose_timing;
+int r3d_get_relpose_timing(const r3d_ctx* ctx, r3d_relpose_timing* out);
+
 /* ---- the steps either side of bundle adjustment (SURVEY.md 8f-3) -------------------------------------------------
  * openMVG::tracks::TracksBuilder Build + Filter(min_length) + ExportToSTL, as Regard3D calls them itself
  * (src/threads/PreviewGeneratorThread.cpp:345-352) and as every SfM engine it drives starts: union-find over the

@@ -34,6 +34,7 @@ EXPORTS = [
     "r3d_sfm_add_landmark", "r3d_sfm_get_landmark", "r3d_debug_ba_jacobian_model", "r3d_debug_ba_prior", "r3d_sfm_ba_default_options", "r3d_sfm_bundle_adjust",
     "r3d_tracks_build", "r3d_tracks_count", "r3d_tracks_get", "r3d_tracks_in_images", "r3d_tracks_free",
     "r3d_sfm_structure_from_tracks", "r3d_sfm_remove_outliers", "r3d_cascade_prepare", "r3d_debug_cascade_view",
+    "r3d_relpose_default_options", "r3d_relative_poses", "r3d_get_relpose_timing",
 ]
 
 
@@ -96,6 +97,25 @@ class BASummary(C.Structure):
     _fields_ = [("iterations", C.c_uint32), ("successful_steps", C.c_uint32), ("initial_cost", C.c_double),
                 ("final_cost", C.c_double), ("termination", C.c_int), ("seconds_total", C.c_double),
                 ("seconds_linear", C.c_double), ("seconds_setup", C.c_double)]
+
+
+class RelposeOptions(C.Structure):
+    _fields_ = [("precision_px", C.c_double), ("max_iter", C.c_uint32), ("refine", C.c_int), ("ba", BAOptions)]
+
+
+RELPOSE_OK, RELPOSE_TOO_FEW, RELPOSE_NO_INTRINSIC, RELPOSE_NO_MODEL, RELPOSE_CHEIRALITY = 0, 1, 2, 3, 4
+# r3d_relative_pose
+relpose_dtype = np.dtype([
+    ("I", np.uint32), ("J", np.uint32), ("status", np.int32), ("n_inliers", np.uint32),
+    ("found_residual_precision", np.float64), ("E", np.float64, (3, 3)), ("rotation", np.float64, (3, 3)),
+    ("translation", np.float64, 3), ("ba_iterations", np.uint32), ("ba_successful_steps", np.uint32),
+    ("ba_termination", np.int32), ("ba_initial_cost", np.float64), ("ba_final_cost", np.float64)], align=True)
+
+
+class RelposeTiming(C.Structure):
+    _fields_ = [("ms_ransac", C.c_double), ("ms_cheirality", C.c_double), ("ms_refine", C.c_double),
+                ("ms_device_total", C.c_double), ("ms_host", C.c_double), ("kernel_launches", C.c_uint64),
+                ("ba_iterations", C.c_uint64)]
 
 
 class CMParams(C.Structure):
@@ -611,6 +631,29 @@ class Context:
         self._check(lib().r3d_filter_pairs(self._h, C.c_int(model), C.c_double(precision_px), C.c_uint32(max_iter),
                                            putative.handle, views, C.c_uint32(n), C.byref(h)))
         return Matches(h)
+
+    def relative_poses(self, matches, widths, heights, Ks, precision_px=2.5, max_iter=256, refine=True, **ba):
+        """r3d_relative_poses: relative pose of every pair of `matches` (map order).  Ks: n_views x 3 (focal, ppx, ppy).
+        ba: r3d_ba_options fields of the two-view refinement.  Returns (numpy array of relpose_dtype, Matches of the
+        AC-RANSAC inliers of the OK pairs)."""
+        views = make_views(widths, heights, Ks)
+        o = RelposeOptions()
+        lib().r3d_relpose_default_options(C.byref(o))
+        o.precision_px = precision_px
+        o.max_iter = max_iter
+        o.refine = int(refine)
+        for k, v in ba.items():
+            setattr(o.ba, k, v)
+        out = np.zeros(max(matches.num_pairs, 1), relpose_dtype)
+        h = C.c_void_p()
+        self._check(lib().r3d_relative_poses(self._h, matches.handle, views, C.c_uint32(len(widths)), C.byref(o), _p(out),
+                                             C.byref(h)))
+        return out[:matches.num_pairs].copy(), Matches(h)
+
+    def relpose_timing(self):
+        t = RelposeTiming()
+        self._check(lib().r3d_get_relpose_timing(self._h, C.byref(t)))
+        return {k: getattr(t, k) for k, _ in RelposeTiming._fields_}
 
     def match_timing(self):
         t = MatchTiming()

@@ -57,13 +57,24 @@ struct AcFusedOut {      // per pair, written by the persistent kernel (acransac
 };
 
 // persistent one-CTA-per-pair ACRANSAC (acransac_fused.cu); `order`: pair ids of one size class, largest first;
-// huge: sort buffers / pool in global scratch (cap entries per CTA of the grid)
+// huge: sort buffers / pool in global scratch (cap entries per CTA of the grid); out_model (may be null): 9 doubles per
+// pair id, the best model of every pair with inliers (F = K2^-T E K1^-1 for the essential model)
 size_t acransac_fused_smem_bytes(int model, uint32_t cap, bool huge);
 int acransac_fused_ctas_per_sm(int model, uint32_t cap, bool huge);
 int launch_acransac_fused(r3d_ctx* ctx, DeviceWorker& w, int model, bool huge, const AcPair* pairs, const uint32_t* order,
                           uint32_t n_order, uint32_t* work_counter, const double2* x1, const double2* x2, const float* logc_n,
                           const float* logc_k, uint32_t cap, uint32_t max_iter, double* g_se, uint32_t* g_si, uint32_t* g_pool,
-                          const uint2* matches, uint2* out_matches, AcFusedOut* out, uint32_t grid);
+                          const uint2* matches, uint2* out_matches, AcFusedOut* out, double* out_model, uint32_t grid);
+
+struct AcBestModel {      // per pair of the putative map (r3d_relative_poses): the kept pair's best model, errorMax
+  double model[9];       // row-major; F = K2^-T E K1^-1 for the essential model
+  double errorMax;       // squared residual of the last inlier
+};
+// AC-RANSAC of the pairs [p0, p1) of a putative map on one worker (acransac_host.cu); result[p]: inliers of pair p.
+// best (may be null; device-resident path only): the best model and errorMax of every kept pair
+int filter_pairs_model(r3d_ctx* ctx, DeviceWorker& w, int model, double precision_px, uint32_t max_iter, const r3d_matches* put,
+                       const r3d_view_info* views, uint32_t n_views, uint64_t p0, uint64_t p1, r3d_filter_timing& T,
+                       std::vector<std::vector<r3d_indmatch>>& result, std::vector<AcBestModel>* best = nullptr);
 
 // x1/x2[pt_ofs + k] = normalised positions of putative match k of every pair (double, like MatchesPairToMat)
 int launch_ac_points(r3d_ctx* ctx, DeviceWorker& w, const AcPair* pairs, const AcPointSrc* src, uint32_t n_pairs,

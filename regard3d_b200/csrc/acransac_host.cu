@@ -113,7 +113,8 @@ std::vector<uint32_t> st_src(const std::vector<PairState>& st) {
 int run_fused(r3d_ctx* ctx, DeviceWorker& w, int model, uint32_t max_iter, const r3d_matches* put, const std::vector<uint32_t>& src,
               const std::vector<AcPair>& hpairs, const AcPair* d_pairs, const double2* d_x1, const double2* d_x2,
               const uint2* d_match, const float* d_logc_n, const float* d_logc_k, uint32_t pt_total, uint32_t sizeSample,
-              double t_begin, r3d_filter_timing& T, std::vector<std::vector<r3d_indmatch>>& result) {
+              double t_begin, r3d_filter_timing& T, std::vector<std::vector<r3d_indmatch>>& result,
+              std::vector<AcBestModel>* best) {
   const uint32_t n = (uint32_t)hpairs.size();
   constexpr int kClasses = 6;  // caps 1024, 2048, 4096, 8192, 16384, huge
   std::vector<uint32_t> order[kClasses];
@@ -137,7 +138,9 @@ int run_fused(r3d_ctx* ctx, DeviceWorker& w, int model, uint32_t max_iter, const
   DevBuf<double> d_se(w);
   DevBuf<AcFusedOut> d_out(w);
   DevBuf<uint2> d_outm(w);
+  DevBuf<double> d_model(w);
   R3D_CUDA_TRY(ctx, d_order.ensure(horder.size()));
+  if (best) R3D_CUDA_TRY(ctx, d_model.ensure((size_t)n * 9));
   R3D_CUDA_TRY(ctx, d_work.ensure(kClasses));
   R3D_CUDA_TRY(ctx, d_out.ensure(n));
   R3D_CUDA_TRY(ctx, d_outm.ensure(pt_total));
@@ -175,14 +178,26 @@ int run_fused(r3d_ctx* ctx, DeviceWorker& w, int model, uint32_t max_iter, const
     const uint32_t cnt = class_ofs[c + 1] - class_ofs[c];
     if (!cnt) continue;
     int rc = launch_acransac_fused(ctx, w, model, c == 5, d_pairs, d_order.p + class_ofs[c], cnt, d_work.p + c, d_x1, d_x2, d_logc_n,
-                                   d_logc_k, caps[c], max_iter, d_se.p, d_si.p, d_pool.p, d_match, d_outm.p, d_out.p, grids[c]);
+                                   d_logc_k, caps[c], max_iter, d_se.p, d_si.p, d_pool.p, d_match, d_outm.p, d_out.p,
+                                   best ? d_model.p : nullptr, grids[c]);
     if (rc) return rc;
     T.kernel_launches += 1;
   }
   R3D_CUDA_TRY(ctx, cudaEventRecord(ev[1], w.stream));
   std::vector<AcFusedOut> hout(n);
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(hout.data(), d_out.p, (size_t)n * sizeof(AcFusedOut), cudaMemcpyDeviceToHost, w.stream));
+  std::vector<double> hmodel(best ? (size_t)n * 9 : 0);
+  if (best)
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(hmodel.data(), d_model.p, hmodel.size() * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+  if (best)
+    for (uint32_t a = 0; a < n; ++a) {
+      const AcFusedOut& o = hout[a];
+      if (!(o.minNFA < 0) || !((double)o.n_inliers > sizeSample * 2.5)) continue;
+      AcBestModel& b = (*best)[src[a]];
+      std::memcpy(b.model, &hmodel[9 * (size_t)a], sizeof(b.model));
+      b.errorMax = o.errorMax;
+    }
   float ms = 0.f;
   cudaEventElapsedTime(&ms, ev[0], ev[1]);
   T.ms_score = ms;
@@ -268,7 +283,7 @@ int run_fused(r3d_ctx* ctx, DeviceWorker& w, int model, uint32_t max_iter, const
 // pairs [p0, p1) of the putative map on worker w; result (sized by the caller to the whole map) is indexed by pair
 int filter_pairs_model(r3d_ctx* ctx, DeviceWorker& w, int model, double precision_px, uint32_t max_iter, const r3d_matches* put,
                    const r3d_view_info* views, uint32_t n_views, uint64_t p0, uint64_t p1, r3d_filter_timing& T,
-                   std::vector<std::vector<r3d_indmatch>>& result) {
+                   std::vector<std::vector<r3d_indmatch>>& result, std::vector<AcBestModel>* best) {
   R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
   T = r3d_filter_timing{};
   const double t_begin = now_ms();
@@ -311,6 +326,9 @@ int filter_pairs_model(r3d_ctx* ctx, DeviceWorker& w, int model, double precisio
   // the persistent per-pair kernel draws the sample stream on the device; it needs the restated
   // std::uniform_int_distribution to agree with this process's <random> (acransac_rng.cuh)
   const bool use_fused = rng_selftest() && !getenv("R3D_FILTER_HOST_ROUNDS");
+  if (best && !use_fused)
+    return fail(ctx, R3D_ERR_UNSUPPORTED, "AC-RANSAC model output needs the device-resident path (the device sample stream "
+                                          "disagrees with this process's <random>)");
   // log-combinatorial tables (float, upstream makelogcombi_n / makelogcombi_k).  logcombi(k,n) is a
   // running float sum over i = 1..min(k,n-k): its partial sums ARE the entries for smaller k, so one
   // O(n) pass reproduces the upstream O(n^2) table bit for bit.
@@ -469,7 +487,7 @@ int filter_pairs_model(r3d_ctx* ctx, DeviceWorker& w, int model, double precisio
   if (getenv("R3D_DEBUG_TIMING")) fprintf(stderr, "[r3d] filter host set-up + point upload: %.2f ms\n", now_ms() - t_begin);
   if (use_fused)
     return run_fused(ctx, w, model, max_iter, put, st_src(st), hpairs, d_pairs.p, d_x1.p, d_x2.p, d_match.p, d_logc_n.p, d_logc_k.p,
-                     (uint32_t)n_match_total, sizeSample, t_begin, T, result);
+                     (uint32_t)n_match_total, sizeSample, t_begin, T, result, best);
 
   cudaEvent_t ev[3];
   for (auto& e : ev) R3D_CUDA_TRY(ctx, cudaEventCreate(&e));
