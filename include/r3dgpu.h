@@ -318,6 +318,50 @@ typedef struct {
 } r3d_relpose_timing;
 int r3d_get_relpose_timing(const r3d_ctx* ctx, r3d_relpose_timing* out);
 
+/* ---- global rotations from the relative motions (global SfM, second step) ------------------------------------- */
+#define R3D_ROTAVG_L2 0              /* ROTATION_AVERAGING_L2 (src/threads/R3DTriangulationThread.cpp:201) */
+#define R3D_ROTAVG_L1 1              /* ROTATION_AVERAGING_L1: not implemented, R3D_ERR_UNSUPPORTED */
+#define R3D_ROTAVG_MAX_VIEWS 4096    /* kept views above this (a dense 3n x 3n system): R3D_ERR_UNSUPPORTED */
+typedef struct {
+  int method;                        /* R3D_ROTAVG_L2 */
+  double max_angular_error_deg;      /* 5.0: TripletRotationRejection threshold, a triplet is valid iff float(error) < it */
+  int refine;                        /* 1: L2RotationAveraging_Refine after the linear initialisation */
+  r3d_ba_options lm;                 /* the refinement's trust region; refine_intrinsics and prior_huber_a unused,
+                                      * huber_a <= 0: trivial loss (the default) */
+} r3d_rotavg_options;
+void r3d_rotavg_default_options(r3d_rotavg_options* o);  /* L2, 5.0, 1, r3d_ba_default_options with a trivial loss */
+typedef struct {
+  int success;                       /* 0: no bi-edge-connected component survived (upstream returns false) */
+  uint64_t n_edges;                  /* R3D_RELPOSE_OK entries of the input */
+  uint64_t n_triplets, n_valid_triplets;
+  uint64_t n_kept_edges;
+  uint32_t n_kept_views;
+  uint32_t init_iterations;          /* block inverse iterations of the linear initialisation */
+  uint32_t lm_iterations, lm_successful_steps;
+  int lm_termination;                /* as r3d_ba_summary.termination; -1: not refined */
+  double lm_initial_cost, lm_final_cost;
+  double ms_triplets, ms_init, ms_refine, ms_device_total, ms_host;
+} r3d_rotavg_summary;
+/* Replaces GlobalSfMReconstructionEngine_RelativeMotions::Compute_Global_Rotations = GlobalSfM_Rotation_AveragingSolver::
+ * Run (OpenMVG 1.4, ROTATION_AVERAGING_L2, reached from src/threads/R3DTriangulationThread.cpp:201-250) on the OK entries
+ * of r3d_relative_poses: every OK entry is one edge (I, J) with R_J ~ rotation R_I (X_J = R X_I + t); triplet rotation
+ * rejection (a triangle is valid when its cycle R_ki R_jk R_ij is within max_angular_error_deg of the identity; an edge
+ * survives when a valid triangle holds it), the largest bi-edge-connected component of the surviving edges, the L2
+ * linear initialisation (Martinec-Pajdla), then the non-linear L2 refinement (angle-axis per view, one residual
+ * log(R_ij^T R_j R_i^T) per edge).  Gauge: the lowest kept view id gets R = I exactly.  Outputs: rotations n_views x 9
+ * (X_cam = R X, row-major; zero for views outside the component), view_kept n_views, edge_kept / edge_support n_rel
+ * (may be NULL; support = valid triangles through the edge, 0 for entries that are not OK).  I == J, a view id >=
+ * n_views or an unordered pair given twice among the OK entries: R3D_ERR_INVALID.  One global problem: it runs on the
+ * context's first device. */
+int r3d_rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views,
+                           const r3d_rotavg_options* opt, double* rotations, uint8_t* view_kept, uint8_t* edge_kept,
+                           uint32_t* edge_support, r3d_rotavg_summary* summary);
+/* graph::CleanGraph_KeepLargestBiEdge_Nodes + KeepOnlyReferencedElement on a PairWiseMatches (how upstream's
+ * GlobalSfMReconstructionEngine_RelativeMotions::Process() starts): the pairs whose views both lie in the largest
+ * 2-edge-connected component of the pair graph (most views; a tie keeps the component holding the smallest view id).
+ * Host only, like r3d_tracks_build. */
+int r3d_matches_keep_largest_biedge_component(const r3d_matches* m, r3d_matches** out);
+
 /* ---- the steps either side of bundle adjustment (SURVEY.md 8f-3) -------------------------------------------------
  * openMVG::tracks::TracksBuilder Build + Filter(min_length) + ExportToSTL, as Regard3D calls them itself
  * (src/threads/PreviewGeneratorThread.cpp:345-352) and as every SfM engine it drives starts: union-find over the

@@ -35,6 +35,7 @@ EXPORTS = [
     "r3d_tracks_build", "r3d_tracks_count", "r3d_tracks_get", "r3d_tracks_in_images", "r3d_tracks_free",
     "r3d_sfm_structure_from_tracks", "r3d_sfm_remove_outliers", "r3d_cascade_prepare", "r3d_debug_cascade_view",
     "r3d_relpose_default_options", "r3d_relative_poses", "r3d_get_relpose_timing",
+    "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_matches_keep_largest_biedge_component",
 ]
 
 
@@ -116,6 +117,35 @@ class RelposeTiming(C.Structure):
     _fields_ = [("ms_ransac", C.c_double), ("ms_cheirality", C.c_double), ("ms_refine", C.c_double),
                 ("ms_device_total", C.c_double), ("ms_host", C.c_double), ("kernel_launches", C.c_uint64),
                 ("ba_iterations", C.c_uint64)]
+
+
+ROTAVG_L2, ROTAVG_L1 = 0, 1
+ROTAVG_MAX_VIEWS = 4096
+
+
+class RotavgOptions(C.Structure):
+    _fields_ = [("method", C.c_int), ("max_angular_error_deg", C.c_double), ("refine", C.c_int), ("lm", BAOptions)]
+
+
+class RotavgSummary(C.Structure):
+    _fields_ = [("success", C.c_int), ("n_edges", C.c_uint64), ("n_triplets", C.c_uint64), ("n_valid_triplets", C.c_uint64),
+                ("n_kept_edges", C.c_uint64), ("n_kept_views", C.c_uint32), ("init_iterations", C.c_uint32),
+                ("lm_iterations", C.c_uint32), ("lm_successful_steps", C.c_uint32), ("lm_termination", C.c_int),
+                ("lm_initial_cost", C.c_double), ("lm_final_cost", C.c_double), ("ms_triplets", C.c_double),
+                ("ms_init", C.c_double), ("ms_refine", C.c_double), ("ms_device_total", C.c_double), ("ms_host", C.c_double)]
+
+
+def relative_pose_records(I, J, R, status=None):
+    """r3d_relative_pose records (relpose_dtype) from view ids and rotations (X_J = R X_I + t), e.g. for
+    Context.rotation_averaging on relative motions that did not come from relative_poses."""
+    I = np.asarray(I, np.uint32).ravel()
+    rel = np.zeros(len(I), relpose_dtype)
+    rel["I"] = I
+    rel["J"] = np.asarray(J, np.uint32).ravel()
+    rel["rotation"] = np.asarray(R, np.float64).reshape(-1, 3, 3)
+    rel["status"] = RELPOSE_OK if status is None else np.asarray(status, np.int32)
+    rel["ba_termination"] = -1
+    return rel
 
 
 class CMParams(C.Structure):
@@ -297,6 +327,15 @@ class Matches:
         rc = lib().r3d_load_matches_txt(path.encode(), C.byref(h))
         if rc:
             raise R3DError(rc, "r3d_load_matches_txt(%s)" % path)
+        return Matches(h)
+
+    def keep_largest_biedge_component(self):
+        """graph::CleanGraph_KeepLargestBiEdge_Nodes + KeepOnlyReferencedElement: the pairs inside the largest
+        2-edge-connected component of the pair graph (host only)."""
+        h = C.c_void_p()
+        rc = lib().r3d_matches_keep_largest_biedge_component(self.handle, C.byref(h))
+        if rc:
+            raise R3DError(rc, "r3d_matches_keep_largest_biedge_component")
         return Matches(h)
 
     @staticmethod
@@ -649,6 +688,28 @@ class Context:
         self._check(lib().r3d_relative_poses(self._h, matches.handle, views, C.c_uint32(len(widths)), C.byref(o), _p(out),
                                              C.byref(h)))
         return out[:matches.num_pairs].copy(), Matches(h)
+
+    def rotation_averaging(self, rel, n_views, refine=True, max_angular_error_deg=5.0, method=ROTAVG_L2, **lm):
+        """r3d_rotation_averaging on the OK entries of `rel` (relpose_dtype, e.g. from relative_poses).  lm: r3d_ba_options
+        fields of the refinement (huber_a > 0: Huber loss).  Returns (rotations (n_views, 3, 3), view_kept (n_views,)
+        bool, edge_kept (len(rel),) bool, edge_support (len(rel),) uint32, summary dict)."""
+        rel = np.ascontiguousarray(rel, relpose_dtype)
+        o = RotavgOptions()
+        lib().r3d_rotavg_default_options(C.byref(o))
+        o.method = method
+        o.max_angular_error_deg = max_angular_error_deg
+        o.refine = int(refine)
+        for k, v in lm.items():
+            setattr(o.lm, k, v)
+        rot = np.zeros((max(n_views, 1), 3, 3))
+        vk = np.zeros(max(n_views, 1), np.uint8)
+        ek = np.zeros(max(len(rel), 1), np.uint8)
+        sup = np.zeros(max(len(rel), 1), np.uint32)
+        s = RotavgSummary()
+        self._check(lib().r3d_rotation_averaging(self._h, _p(rel), C.c_uint64(len(rel)), C.c_uint32(n_views), C.byref(o), _p(rot),
+                                                 _p(vk), _p(ek), _p(sup), C.byref(s)))
+        summ = {k: getattr(s, k) for k, _ in RotavgSummary._fields_}
+        return rot[:n_views], vk[:n_views].astype(bool), ek[:len(rel)].astype(bool), sup[:len(rel)].copy(), summ
 
     def relpose_timing(self):
         t = RelposeTiming()

@@ -1024,6 +1024,19 @@ __global__ void __launch_bounds__(256) k_ba_update(Dev d, double inv_radius) {
 }
 
 }  // namespace ba
+
+int dense_cholesky(r3d_ctx* ctx, DeviceWorker& w, double* A, double* L, double* Linv, int n, double* flag, double* x) {
+  static_assert(kCholNB == ba::NB, "Linv layout");
+  int per_sm = 0;
+  R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(ba::k_chol_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ba::kCholSmemBytes));
+  R3D_CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba::k_chol_fused, 1024, ba::kCholSmemBytes));
+  if (per_sm < 1) return fail(ctx, R3D_ERR_CUDA, "dense Cholesky: k_chol_fused does not fit on an SM");
+  void* args[] = {&A, &L, &Linv, &n, &flag, &x};
+  R3D_CUDA_TRY(ctx, cudaLaunchCooperativeKernel((void*)ba::k_chol_fused, dim3(w.sm_count), dim3(32, 32), args, ba::kCholSmemBytes,
+                                                w.stream));
+  return R3D_OK;
+}
+
 }  // namespace r3d
 
 // ------------------------------------------------------------------------------------------------

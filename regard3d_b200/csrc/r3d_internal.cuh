@@ -209,6 +209,13 @@ int ensure_capacity(r3d_ctx* ctx, void** p, size_t* cap, size_t need_elems) {
   return R3D_OK;
 }
 
+// dense Cholesky + both triangular solves of an SPD system on the worker's stream (ba.cu: the cooperative k_chol_fused,
+// one CTA per SM).  A: (n+1) x n row-major, the system with its right-hand side as row n, overwritten; L: (n+1) x n + 64,
+// receives the lower factor (row n: the forward-substituted rhs); Linv: ceil(n / kCholNB) inverses of the kCholNB x kCholNB
+// diagonal blocks of L; *flag (zeroed by the caller) becomes 1 when A is not positive definite; x: n, the solution
+constexpr int kCholNB = 32;
+int dense_cholesky(r3d_ctx* ctx, DeviceWorker& w, double* A, double* L, double* Linv, int n, double* flag, double* x);
+
 int prepare_views(r3d_ctx* ctx, DeviceWorker& w);
 void* pool_alloc(DeviceWorker& w, size_t bytes);  // nullptr on failure
 void pool_release(DeviceWorker& w, void* p);
