@@ -1,25 +1,28 @@
 // k_l2_candidates.cu -- the tensor-core candidate kernel (sm_90a: TMA, mbarrier, wgmma).
 //
-// Work item = (pair, 128-query block of view J).  For every query row the kernel evaluates a squared distance
-// against all database rows of view I and keeps the kNumKeys smallest chunk minima (kChunk consecutive database rows
-// each), packed with the chunk id, in keys_out.  Two operand kinds, one kernel template:
+// Work item = (pair, query block of view J: 128 rows on the fp16 path, 256 on the integer path).  For every query row
+// the kernel evaluates a squared distance against all database rows of view I and keeps the kNumKeys smallest chunk
+// minima (kChunk consecutive database rows each), packed with the chunk id, in keys_out.  Two operand kinds, one
+// kernel template:
 //   fp16 (kU8 = false)  the distance surrogate opQ(J) . opD(I) of the fp16 operands (k_view_prepare), f32 accumulation
 //   u8   (kU8 = true)   uint8 descriptors read in place (int_operand()): ||a||^2 - 2 q.a from u8 x u8 -> s32 MMAs plus
 //                       the exact norms, so the keys are exact up to the chunk-id packing
 //
-// Persistent CTAs (one per SM, 227 KB of shared memory), three warpgroups:
-//   warpgroup 0      one TMA producer warp: the item's query block (nkb boxes of 128 rows x 128 bytes, double
-//                    buffered across items) and a ring of database stages (one 128-byte K-block of a 256-row tile;
-//                    u8: plus the tile's 256 database norms)
-//   warpgroups 1, 2  consumers of query rows 0-63 / 64-127: the MMAs, then the chunk minima and the key insertion in
-//                    registers.
-//     fp16: per 256-row tile, m64n256k16 into 128 f32 registers, then the epilogue.
-//     u8:   per 128-row half tile, m64n128k32 into one of two 64-register s32 accumulators; the epilogue of half h
-//           runs while the MMAs of half h + 1 are in the tensor pipe.  The database map loads every 32-row group
-//           with its row pairs transposed (context.cu), so each lane of a quad holds whole chunks: the chunk minima
-//           take no shuffle, and only the keys below their set's largest are inserted, in warp-uniform rounds.
-// Barriers: full[s] (TMA bytes landed), empty[s] (the 8 consumer warps are done with the stage), qfull / qempty the
-// same for the query buffers.
+// Persistent CTAs (one per SM, 227 KB of shared memory), one producer and kConsumers consumer warpgroups:
+//   warpgroup 0      one TMA producer warp: the item's query block (kConsumers / 2 boxes of 128 rows x 128 bytes per
+//                    K-block, double buffered across items) and a ring of database stages (one 128-byte K-block of a
+//                    256-row tile; u8: plus the tile's 256 database norms)
+//   warpgroup 1 + c  consumer of query rows [64 c, 64 c + 64) of the block: the MMAs, then the chunk minima and the key
+//                    insertion in registers.
+//     fp16: 2 consumers (the 128-register f32 accumulator leaves no room for more); per 256-row tile, m64n256k16,
+//           then the epilogue.
+//     u8:   4 consumers, so every database tile in shared memory feeds 256 query rows; per 128-row half tile,
+//           m64n128k32 into one 64-register s32 accumulator, then the epilogue of that half.  While one consumer
+//           reduces, the other three keep MMAs in the tensor pipe.  The database map loads every 32-row group with
+//           its row pairs transposed (context.cu), so each lane of a quad holds whole chunks: the chunk minima take no
+//           shuffle, and only the keys below their set's largest are inserted, in warp-uniform rounds.
+// Barriers: full[s] (TMA bytes landed), empty[s] (every consumer warp is done with the stage), qfull / qempty the same
+// for the query buffers.
 #include "r3d_internal.cuh"
 #include "tc_ptx.cuh"
 
@@ -33,8 +36,8 @@ constexpr int kMaxStages = 8;
 constexpr uint32_t kTileN = 256;                  // database rows per tile (the wgmma N extent)
 constexpr uint32_t kStageBytes = 2 * kBoxBytes;   // one K-block of a 256-row tile: two 128-row TMA boxes
 constexpr uint32_t kNormBytes = kTileN * 4;       // u8: the int32 norms of a tile's database rows
-constexpr uint32_t kConsumerWarps = 8;
-constexpr uint32_t kThreads = 384;
+constexpr uint32_t kConsumersF16 = kTileRows / 64;  // consumer warpgroups (64 query rows each) of the fp16 path
+constexpr uint32_t kConsumersU8 = kSuperRows / 64;  // ... and of the integer path
 constexpr size_t kSmemOptIn = 232448;             // 227 KB: the largest dynamic shared memory of one block on sm_90
 static_assert(kChunk == 8, "the epilogue reduces one 8-column block of the wgmma accumulator per chunk");
 
@@ -72,18 +75,27 @@ __device__ __forceinline__ void merge_keys(float (&key)[kNumKeys], int d) {
 
 }  // namespace
 
-template <bool kU8>
-__global__ void __launch_bounds__(kThreads, 1)
+template <bool kU8, uint32_t kConsumers>
+__global__ void __launch_bounds__(128 * (kConsumers + 1), 1)
 k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __restrict__ tmapD,
                 const PairDesc* __restrict__ pairs, const WorkItem* __restrict__ items, uint32_t n_items,
                 uint32_t* __restrict__ keys_out, uint32_t nkb, uint32_t ksteps, uint32_t n_stages, uint32_t n_qbuf) {
+  static_assert(kConsumers == 2 || (kU8 && kConsumers == 4), "fp16: 2 consumers; u8: 2 or 4");
   constexpr uint32_t kBoxCols = kU8 ? 128u : (uint32_t)kKBlock;  // elements in a 128-byte box row
+  constexpr uint32_t kQBoxes = kConsumers / 2;                   // 128-row query boxes per K-block
+  constexpr uint32_t kBlockRows = kQBoxes * kTileRows;           // query rows per work item
+  constexpr uint32_t kConsumerWarps = 4 * kConsumers;
+  // Register split (setmaxnreg): 640 threads launch with at most 96 registers each (65536 / 640, in steps of 8), and
+  // the consumers can only take what the producer warpgroup gives back: 128 x 24 + 512 x 112 <= 640 x 96.  384
+  // threads launch with 168: 128 x 40 + 256 x 232 = 384 x 168.
+  constexpr uint32_t kProducerRegs = kConsumers == 4 ? 24u : 40u;
+  constexpr uint32_t kConsumerRegs = kConsumers == 4 ? 112u : 232u;
   extern __shared__ unsigned char smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  // n_qbuf (1 or 2) x nkb boxes: the item's 128 query rows.  With two buffers the next item's query block is loaded
-  // while the current item's last tiles are still in the tensor pipe.
+  // n_qbuf (1 or 2) x kQBoxes x nkb boxes ([buffer][box][K-block]): the item's query rows.  With two buffers the next
+  // item's query block is loaded while the current item's last tiles are still in the tensor pipe.
   const uint32_t q_base = base;
-  const uint32_t q_bytes = nkb * kBoxBytes;
+  const uint32_t q_bytes = kQBoxes * nkb * kBoxBytes;
   const uint32_t d_base = q_base + n_qbuf * q_bytes;            // n_stages stages
   const uint32_t n_base = d_base + n_stages * kStageBytes;      // u8: n_stages x kNormBytes
   const uint32_t bar_full = n_base + (kU8 ? n_stages * kNormBytes : 0u);  // [kMaxStages]
@@ -110,7 +122,7 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
 
   if (wg == 0) {
     // ========================================= TMA producer =========================================
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<kProducerRegs>();
     if (warp != 0) return;
     uint32_t stage = 0, phase = 0, qi = 0;
     for (uint32_t it = blockIdx.x; it < n_items; it += gridDim.x, ++qi) {
@@ -123,10 +135,12 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       const uint32_t quse = n_qbuf == 2 ? (qi >> 1) : qi;
       mbar_wait(bar_qempty + 8 * qb, (quse & 1u) ^ 1u);
       if (elect_one()) {
-        mbar_arrive_expect_tx(bar_qfull + 8 * qb, nkb * kBoxBytes);
-        for (uint32_t kb = 0; kb < nkb; ++kb)
-          tma_load_2d(q_base + qb * q_bytes + kb * kBoxBytes, mq, (int)(kb * kBoxCols), (int)(wi.sb * kTileRows),
-                      bar_qfull + 8 * qb);
+        mbar_arrive_expect_tx(bar_qfull + 8 * qb, q_bytes);
+#pragma unroll
+        for (uint32_t b = 0; b < kQBoxes; ++b)  // rows past the view are zero-filled
+          for (uint32_t kb = 0; kb < nkb; ++kb)
+            tma_load_2d(q_base + qb * q_bytes + (b * nkb + kb) * kBoxBytes, mq, (int)(kb * kBoxCols),
+                        (int)(wi.sb * kBlockRows + b * kTileRows), bar_qfull + 8 * qb);
       }
       __syncwarp();
       for (uint32_t t = 0; t < ntiles; ++t) {
@@ -156,7 +170,7 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
   }
 
   // =========================================== consumers ===========================================
-  setmaxnreg_inc<232>();
+  setmaxnreg_inc<kConsumerRegs>();
   const uint32_t cw = wg - 1u;                                   // query rows [64 cw, 64 cw + 64) of the block
   const uint32_t q = lane & 3u;                                  // lane inside the quad
   const uint32_t row0 = cw * 64u + (warp & 3u) * 16u + (lane >> 2);  // accumulator rows row0 and row0 + 8
@@ -171,14 +185,16 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
     float key0[kNumKeys], key1[kNumKeys];
 #pragma unroll
     for (int i = 0; i < kNumKeys; ++i) key0[i] = key1[i] = __uint_as_float(kKeySentinel);
-    const uint32_t a_base = q_base + qb * q_bytes + cw * (kBoxBytes / 2);  // 64 rows x 128 B into each query box
+    // box cw / 2 of each K-block, 64 rows x 128 B into it
+    const uint32_t a_base = q_base + qb * q_bytes +
+                            (kQBoxes == 1 ? cw * (kBoxBytes / 2) : (cw >> 1) * nkb * kBoxBytes + (cw & 1u) * (kBoxBytes / 2));
     if constexpr (kU8) {
       // ||q||^2 of the two rows (kPadNorm beyond nJ: those rows' keys are never read)
-      const int32_t qn0 = __ldg(pd.normJ + wi.sb * kTileRows + row0);
-      const int32_t qn1 = __ldg(pd.normJ + wi.sb * kTileRows + row0 + 8u);
-      int32_t acc0[64], acc1[64];
+      const int32_t qn0 = __ldg(pd.normJ + wi.sb * kBlockRows + row0);
+      const int32_t qn1 = __ldg(pd.normJ + wi.sb * kBlockRows + row0 + 8u);
+      int32_t acc[64];
       // MMAs of half h (database rows h * 128 .. + 127) of the tile whose K-blocks start at stage s0
-      auto issue = [&](int32_t (&acc)[64], uint32_t h, uint32_t s0) {
+      auto issue = [&](uint32_t h, uint32_t s0) {
         wgmma_fence();
         uint32_t s = s0, ks_left = ksteps;
         for (uint32_t kb = 0; kb < nkb; ++kb) {
@@ -204,7 +220,7 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       // that pass are inserted in warp-uniform rounds, one per set and lane per round (FLT_MAX, a no-op of the
       // network, where a lane has none left).  The keys of a set differ in their chunk bits, so the order of the
       // insertions does not change the set.
-      auto reduce = [&](const int32_t (&acc)[64], uint32_t t, uint32_t h, uint32_t s0) {
+      auto reduce = [&](uint32_t t, uint32_t h, uint32_t s0) {
         const int32_t* nrm = (const int32_t*)(smem_raw + (n_base + s0 * kNormBytes - smem_u32(smem_raw))) + h * 128u + 8u * q;
         const uint32_t chunk0 = t * (kTileN / kChunk) + h * (kTileN / 2 / kChunk) + q;
         float x0[4], x1[4];
@@ -240,41 +256,32 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
           key_insert_packed(y1, key1);
         }
       };
-      // the epilogue has read the tile's norms and the MMAs its operands: hand its stages back to the producer
-      auto release = [&](uint32_t s0) {
-        __syncwarp();
-        if (lane == 0)
-          for (uint32_t kb = 0, s = s0; kb < nkb; ++kb) {
-            mbar_arrive(bar_empty + 8 * s);
-            if (++s == n_stages) s = 0;
-          }
-      };
+      // One accumulator: the MMAs of a half, then its epilogue.  The MMAs of the other consumers fill the tensor pipe
+      // meanwhile (a second accumulator would not fit the register budget of four consumers).
       mbar_wait(bar_qfull + 8 * qb, qf);
-      uint32_t s_prev = 0;
       for (uint32_t t = 0; t < ntiles; ++t) {
         const uint32_t s_t = stage;
         for (uint32_t kb = 0; kb < nkb; ++kb) {
           mbar_wait(bar_full + 8 * stage, phase);
           if (++stage == n_stages) { stage = 0; phase ^= 1u; }
         }
-        issue(acc0, 0, s_t);
-        if (t > 0) {  // half 1 of the previous tile is done: reduce it while half 0 of this tile runs
-          wgmma_wait<1>();
-          wgmma_fence_operand(acc1);
-          reduce(acc1, t - 1, 1, s_prev);
-          release(s_prev);
+#pragma unroll
+        for (uint32_t h = 0; h < 2; ++h) {
+          issue(h, s_t);
+          wgmma_wait<0>();
+          wgmma_fence_operand(acc);
+          // every MMA of the item has read the query block
+          if (h == 1 && t + 1 == ntiles && lane == 0) mbar_arrive(bar_qempty + 8 * qb);
+          reduce(t, h, s_t);
         }
-        issue(acc1, 1, s_t);
-        wgmma_wait<1>();
-        wgmma_fence_operand(acc0);
-        reduce(acc0, t, 0, s_t);
-        s_prev = s_t;
+        // the epilogue has read the tile's norms and the MMAs its operands: hand its stages back to the producer
+        __syncwarp();
+        if (lane == 0)
+          for (uint32_t kb = 0, s = s_t; kb < nkb; ++kb) {
+            mbar_arrive(bar_empty + 8 * s);
+            if (++s == n_stages) s = 0;
+          }
       }
-      wgmma_wait<0>();
-      wgmma_fence_operand(acc1);
-      if (lane == 0) mbar_arrive(bar_qempty + 8 * qb);  // every MMA of the item has read the query block
-      reduce(acc1, ntiles - 1, 1, s_prev);
-      release(s_prev);
     } else {
       float acc[128];
       mbar_wait(bar_qfull + 8 * qb, qf);
@@ -327,7 +334,7 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       float k[kNumKeys];
 #pragma unroll
       for (int i = 0; i < kNumKeys; ++i) k[i] = q == 0 ? key0[i] : key1[i];
-      const uint32_t row = wi.sb * kTileRows + row0 + 8u * q;
+      const uint32_t row = wi.sb * kBlockRows + row0 + 8u * q;
       uint4 o0, o1;
       o0.x = __float_as_uint(k[0]); o0.y = __float_as_uint(k[1]);
       o0.z = __float_as_uint(k[2]); o0.w = __float_as_uint(k[3]);
@@ -340,8 +347,8 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
   }
 }
 
-static int ring_stages(int nkb, int n_qbuf, uint32_t stage_bytes) {
-  const size_t fixed = 1024 + 8 * (2 * kMaxStages + 4) + (size_t)n_qbuf * nkb * kBoxBytes;
+static int ring_stages(uint32_t q_bytes, int n_qbuf, uint32_t stage_bytes) {
+  const size_t fixed = 1024 + 8 * (2 * kMaxStages + 4) + (size_t)n_qbuf * q_bytes;
   const int stages = (int)((kSmemOptIn - fixed) / stage_bytes);
   return stages > kMaxStages ? kMaxStages : stages;
 }
@@ -354,16 +361,20 @@ int launch_l2_candidates(r3d_ctx* ctx, DeviceWorker& w, const PairDesc* d_pairs,
   const int nkb = u8 ? ((int)dim + 127) / 128 : (operand_cols((int)dim) + kKBlock - 1) / kKBlock;
   const int ksteps = u8 ? ((int)dim + 31) / 32 : operand_ksteps((int)dim);
   if (nkb > kMaxKBlocks) return fail(ctx, R3D_ERR_UNSUPPORTED, "descriptor dimension too large for the tensor-core path");
+  const uint32_t consumers = u8 ? kConsumersU8 : kConsumersF16;
   const uint32_t stage_bytes = kStageBytes + (u8 ? kNormBytes : 0u);
-  // u8 consumers hold one tile's stages while they wait for the next tile's: the ring needs two tiles
+  const uint32_t q_bytes = consumers / 2 * nkb * kBoxBytes;  // one query buffer: the item's query rows, nkb K-blocks
+  // The four u8 consumers can be a tile apart: the ring needs two tiles.  Two query buffers when the ring keeps that
+  // depth, else one (very wide descriptors).  u8, 33 KB stages: D <= 128 (nkb = 1) 2 x 32 KB of queries and 4 stages;
+  // D = 256 (nkb = 2) 2 x 64 KB would leave 2 stages, so 1 x 64 KB and 4 stages (two tiles).
   const int min_stages = u8 ? 2 * nkb : 3;
-  const int n_qbuf = ring_stages(nkb, 2, stage_bytes) >= min_stages ? 2 : 1;  // very wide descriptors: keep the ring deep enough instead
-  const int stages = ring_stages(nkb, n_qbuf, stage_bytes);
-  const size_t smem = 1024 + (size_t)n_qbuf * nkb * kBoxBytes + (size_t)stages * stage_bytes + 8 * (2 * kMaxStages + 4);
-  auto kern = u8 ? k_l2_candidates<true> : k_l2_candidates<false>;
+  const int n_qbuf = ring_stages(q_bytes, 2, stage_bytes) >= min_stages ? 2 : 1;
+  const int stages = ring_stages(q_bytes, n_qbuf, stage_bytes);
+  const size_t smem = 1024 + (size_t)n_qbuf * q_bytes + (size_t)stages * stage_bytes + 8 * (2 * kMaxStages + 4);
+  auto kern = u8 ? k_l2_candidates<true, kConsumersU8> : k_l2_candidates<false, kConsumersF16>;
   R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const uint32_t grid = n_items < (uint32_t)w.sm_count ? n_items : (uint32_t)w.sm_count;
-  kern<<<grid, kThreads, smem, w.stream>>>((const CUtensorMap*)w.d_tmapQ, (const CUtensorMap*)w.d_tmapD, d_pairs, d_items,
+  kern<<<grid, 128 * (consumers + 1), smem, w.stream>>>((const CUtensorMap*)w.d_tmapQ, (const CUtensorMap*)w.d_tmapD, d_pairs, d_items,
                                            n_items, d_keys, (uint32_t)nkb, (uint32_t)ksteps, (uint32_t)stages,
                                            (uint32_t)n_qbuf);
   R3D_CUDA_TRY(ctx, cudaGetLastError());

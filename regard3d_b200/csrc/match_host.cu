@@ -211,6 +211,9 @@ static int match_on_worker(r3d_ctx* ctx, DeviceWorker& w, const uint32_t* pairs,
     ~Joiner() { for (auto& x : t) if (x.joinable()) x.join(); }
   } joiner{tails};
 
+  // candidate work items: 256 query rows on the integer path (four consumer warpgroups share each database tile),
+  // 128 on the fp16 path
+  const uint32_t qrows = item_rows(dtype, dim);
   size_t b0 = 0;
   uint32_t batch_no = 0;
   while (b0 < all.size()) {
@@ -226,7 +229,7 @@ static int match_on_worker(r3d_ctx* ctx, DeviceWorker& w, const uint32_t* pairs,
       rows += all[b1].pd.nJ_pad;
       qtotal += all[b1].pd.nJ;
       if (all[b1].pd.use_tc) {
-        n_items += all[b1].pd.nJ_pad / kSuperRows;
+        n_items += all[b1].pd.nJ_pad / qrows;
         max_chunks = std::max(max_chunks, all[b1].pd.nI_pad / (uint32_t)kChunk);
       }
       max_nJ = std::max(max_nJ, all[b1].pd.nJ);
@@ -238,10 +241,10 @@ static int match_on_worker(r3d_ctx* ctx, DeviceWorker& w, const uint32_t* pairs,
     auto hp = std::make_shared<std::vector<PairDesc>>(nb);
     for (uint32_t k = 0; k < nb; ++k) (*hp)[k] = all[b0 + k].pd;
     auto hitems = std::make_shared<std::vector<WorkItem>>();
-    hitems->reserve(2 * n_items + nb);
+    hitems->reserve(n_items + nb);
     for (uint32_t k = 0; k < nb; ++k)
-      if ((*hp)[k].use_tc)  // 128-query blocks
-        for (uint32_t qb = 0; qb < (*hp)[k].nJ_pad / kTileRows; ++qb) hitems->push_back(WorkItem{k, qb});
+      if ((*hp)[k].use_tc)
+        for (uint32_t qb = 0; qb < (*hp)[k].nJ_pad / qrows; ++qb) hitems->push_back(WorkItem{k, qb});
     const bool any_tc = !hitems->empty();
     if (cascade)  // the item array carries (table row of I, table row of J) per pair instead of work items
       for (uint32_t k = 0; k < nb; ++k)

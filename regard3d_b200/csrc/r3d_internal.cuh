@@ -22,10 +22,10 @@
 // ------------------------------------------------------------------------------------------------
 namespace r3d {
 
-constexpr int kTileRows = 128;      // rows of one TMA box / one query block
+constexpr int kTileRows = 128;      // rows of one TMA box; query rows per work item of the fp16 path
 constexpr int kKBlock = 64;         // fp16 elements per 128-byte swizzle row
-constexpr int kQB = 2;              // query blocks (of 128 rows) resident per CTA
-constexpr int kSuperRows = kTileRows * kQB;  // 256 query rows per work item
+constexpr int kQB = 2;              // integer path: 128-row query boxes per work item
+constexpr int kSuperRows = kTileRows * kQB;  // query rows per work item of the integer path
 constexpr int kRowPad = 256;        // every view is padded to a multiple of this many rows
 constexpr int kBiasCols = 16;       // one MMA K-step holding the norm terms
 #ifndef R3D_CHUNK
@@ -50,6 +50,8 @@ constexpr int32_t kPadNorm = 1 << 28;  // ||a||^2 of a padding row of the intege
 constexpr uint32_t kGroupRows = 32;    // integer path: database rows permuted together by the database tensor map
 // rows of d_desc on the integer path: whole groups of the database map (zeros beyond n), at least one
 inline uint32_t int_desc_rows(uint32_t n) { return (std::max<uint32_t>(n, 1) + kGroupRows - 1) / kGroupRows * kGroupRows; }
+// query rows per work item of the candidate kernel (a divisor of kRowPad)
+inline uint32_t item_rows(int dtype, uint32_t dim) { return int_operand(dtype, dim) ? kSuperRows : kTileRows; }
 
 struct ViewDev {
   uint32_t n = 0, dim = 0, dtype = 0, n_pad = 0, kp = 0;
@@ -107,7 +109,7 @@ struct PairDesc {            // one entry per pair of a batch (device + host)
 };
 static_assert(sizeof(PairDesc) == 80, "PairDesc layout");
 
-struct WorkItem { uint32_t pair; uint32_t sb; };  // sb: super-block (256 query rows) index
+struct WorkItem { uint32_t pair; uint32_t sb; };  // sb: query block (item_rows() rows) index
 
 constexpr uint32_t kCounterWords = 16 + 4096;  // 16 scalar counters + one match counter per pair of the batch
 struct OutSlot {  // double-buffered outputs of a matching batch
