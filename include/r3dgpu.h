@@ -362,6 +362,49 @@ int r3d_rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t 
  * Host only, like r3d_tracks_build. */
 int r3d_matches_keep_largest_biedge_component(const r3d_matches* m, r3d_matches** out);
 
+/* ---- global translations from the relative motions and the global rotations (global SfM, third step) ----------- */
+#define R3D_TRANSAVG_L1 1            /* TRANSLATION_AVERAGING_L1 (the linear program): not implemented, R3D_ERR_UNSUPPORTED */
+#define R3D_TRANSAVG_L2_CHORDAL 2    /* TRANSLATION_AVERAGING_L2_DISTANCE_CHORDAL: 1DSfM chordal distance on the centres */
+#define R3D_TRANSAVG_SOFTL1 3        /* TRANSLATION_AVERAGING_SOFTL1: soft-L1 on t_j - (R_ij t_i + s_ij t_ij), s_ij >= 1 */
+/* The method values are Regard3D's transAveraging_ (src/threads/R3DTriangulationThread.cpp:204-208). */
+typedef struct {
+  int method;                        /* R3D_TRANSAVG_L2_CHORDAL (default) or R3D_TRANSAVG_SOFTL1 */
+  double softl1_loss;                /* 0.01: SoftLOneLoss width of R3D_TRANSAVG_SOFTL1 */
+  r3d_ba_options lm;                 /* the trust region.  Honoured: gradient_tolerance, parameter_tolerance,
+                                      * initial_radius; max_iterations if > 0 (0: the method's cap, 500 for chordal,
+                                      * max(50, 2 x kept edges) for soft-L1); function_tolerance if > 0 (0: 1e-7 for
+                                      * chordal, 1e-6 for soft-L1).  huber_a, refine_intrinsics, prior_huber_a unused. */
+} r3d_transavg_options;
+void r3d_transavg_default_options(r3d_transavg_options* o);  /* L2 chordal, 0.01, the methods' upstream tolerances */
+typedef struct {
+  int success;                       /* 0: no bi-edge-connected component among the usable edges */
+  uint64_t n_edges;                  /* usable entries: OK, edge_use set, both views rotation-kept */
+  uint64_t n_kept_edges;
+  uint32_t n_kept_views;
+  uint32_t lm_iterations, lm_successful_steps;
+  int lm_termination;                /* as r3d_ba_summary.termination; -1: not run */
+  double lm_initial_cost, lm_final_cost;
+  double ms_solve, ms_device_total, ms_host;
+} r3d_transavg_summary;
+/* Replaces GlobalSfMReconstructionEngine_RelativeMotions::Compute_Global_Translations (OpenMVG 1.4, reached from
+ * src/threads/R3DTriangulationThread.cpp:201-250) for the chordal and soft-L1 methods, with the pairwise relative
+ * translations of r3d_relative_poses in place of upstream's triplet-wise ones (DESIGN.md sec. 2).  Edges: the OK entries
+ * of rel whose edge_use is set (NULL: every OK entry; pass rotation averaging's edge_kept) and whose views are both in
+ * rot_kept; the largest bi-edge-connected component of them.  rotations: n_views x 9 from r3d_rotation_averaging.
+ *   chordal: unknown centres C, one residual (C_J - C_I) / |C_J - C_I| + R_J^T t_IJ / |t_IJ| per edge, no loss, start
+ *            from a fixed pseudo-random draw in [0, 1).
+ *   soft-L1: unknown translations t and one scale s >= 1 per edge, residual t_J - (R_J R_I^T t_I + s t_IJ / |t_IJ|),
+ *            SoftLOneLoss(softl1_loss), start t = 1, s = 1.
+ * Gauge: the lowest kept view id gets C = 0 (chordal) / t = 0 (soft-L1) exactly and is held.  Outputs: centers and
+ * translations n_views x 3 (t = -R C; zero for views outside the component), view_kept n_views, edge_kept n_rel (may be
+ * NULL).  I == J, a view id >= n_views, an unordered pair given twice or a zero / non-finite translation among the OK
+ * entries with edge_use set: R3D_ERR_INVALID; more than R3D_ROTAVG_MAX_VIEWS kept views or method L1:
+ * R3D_ERR_UNSUPPORTED.  One global problem: it runs on the context's first device. */
+int r3d_translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use,
+                              const double* rotations, const uint8_t* rot_kept, uint32_t n_views,
+                              const r3d_transavg_options* opt, double* centers, double* translations, uint8_t* view_kept,
+                              uint8_t* edge_kept, r3d_transavg_summary* summary);
+
 /* ---- the steps either side of bundle adjustment (SURVEY.md 8f-3) -------------------------------------------------
  * openMVG::tracks::TracksBuilder Build + Filter(min_length) + ExportToSTL, as Regard3D calls them itself
  * (src/threads/PreviewGeneratorThread.cpp:345-352) and as every SfM engine it drives starts: union-find over the

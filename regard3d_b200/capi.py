@@ -36,6 +36,7 @@ EXPORTS = [
     "r3d_sfm_structure_from_tracks", "r3d_sfm_remove_outliers", "r3d_cascade_prepare", "r3d_debug_cascade_view",
     "r3d_relpose_default_options", "r3d_relative_poses", "r3d_get_relpose_timing",
     "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_matches_keep_largest_biedge_component",
+    "r3d_transavg_default_options", "r3d_translation_averaging",
 ]
 
 
@@ -133,6 +134,20 @@ class RotavgSummary(C.Structure):
                 ("lm_iterations", C.c_uint32), ("lm_successful_steps", C.c_uint32), ("lm_termination", C.c_int),
                 ("lm_initial_cost", C.c_double), ("lm_final_cost", C.c_double), ("ms_triplets", C.c_double),
                 ("ms_init", C.c_double), ("ms_refine", C.c_double), ("ms_device_total", C.c_double), ("ms_host", C.c_double)]
+
+
+TRANSAVG_L1, TRANSAVG_L2_CHORDAL, TRANSAVG_SOFTL1 = 1, 2, 3
+
+
+class TransavgOptions(C.Structure):
+    _fields_ = [("method", C.c_int), ("softl1_loss", C.c_double), ("lm", BAOptions)]
+
+
+class TransavgSummary(C.Structure):
+    _fields_ = [("success", C.c_int), ("n_edges", C.c_uint64), ("n_kept_edges", C.c_uint64), ("n_kept_views", C.c_uint32),
+                ("lm_iterations", C.c_uint32), ("lm_successful_steps", C.c_uint32), ("lm_termination", C.c_int),
+                ("lm_initial_cost", C.c_double), ("lm_final_cost", C.c_double), ("ms_solve", C.c_double),
+                ("ms_device_total", C.c_double), ("ms_host", C.c_double)]
 
 
 def relative_pose_records(I, J, R, status=None):
@@ -710,6 +725,40 @@ class Context:
                                                  _p(vk), _p(ek), _p(sup), C.byref(s)))
         summ = {k: getattr(s, k) for k, _ in RotavgSummary._fields_}
         return rot[:n_views], vk[:n_views].astype(bool), ek[:len(rel)].astype(bool), sup[:len(rel)].copy(), summ
+
+    def translation_averaging(self, rel, rotations, rot_kept, n_views, method=TRANSAVG_L2_CHORDAL, edge_use=None,
+                              softl1_loss=0.01, **lm):
+        """r3d_translation_averaging on the OK entries of `rel` (relpose_dtype) with edge_use set (None: all of them, or
+        rotation_averaging's edge_kept) and both views in rot_kept, given the global rotations (n_views, 3, 3) of
+        rotation_averaging.  lm: r3d_ba_options fields (max_iterations / function_tolerance 0: the method's).  Returns
+        (centers (n_views, 3), translations (n_views, 3), view_kept (n_views,) bool, edge_kept (len(rel),) bool,
+        summary dict)."""
+        rel = np.ascontiguousarray(rel, relpose_dtype)
+        rot = np.ascontiguousarray(np.asarray(rotations, np.float64).reshape(-1, 3, 3))
+        rk = np.ascontiguousarray(np.asarray(rot_kept).astype(np.uint8).ravel())
+        if len(rot) < n_views or len(rk) < n_views:
+            raise ValueError("rotations / rot_kept hold fewer than n_views views")
+        use = None
+        if edge_use is not None:
+            use = np.ascontiguousarray(np.asarray(edge_use).astype(np.uint8).ravel())
+            if len(use) != len(rel):
+                raise ValueError("edge_use must have one entry per record")
+        o = TransavgOptions()
+        lib().r3d_transavg_default_options(C.byref(o))
+        o.method = method
+        o.softl1_loss = softl1_loss
+        for k, v in lm.items():
+            setattr(o.lm, k, v)
+        cen = np.zeros((max(n_views, 1), 3))
+        tra = np.zeros((max(n_views, 1), 3))
+        vk = np.zeros(max(n_views, 1), np.uint8)
+        ek = np.zeros(max(len(rel), 1), np.uint8)
+        s = TransavgSummary()
+        self._check(lib().r3d_translation_averaging(self._h, _p(rel), C.c_uint64(len(rel)), None if use is None else _p(use), _p(rot),
+                                                    _p(rk), C.c_uint32(n_views), C.byref(o), _p(cen), _p(tra), _p(vk), _p(ek),
+                                                    C.byref(s)))
+        summ = {k: getattr(s, k) for k, _ in TransavgSummary._fields_}
+        return cen[:n_views], tra[:n_views], vk[:n_views].astype(bool), ek[:len(rel)].astype(bool), summ
 
     def relpose_timing(self):
         t = RelposeTiming()

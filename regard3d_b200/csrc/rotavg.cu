@@ -19,6 +19,7 @@
 //      residual log(R_ij^T R_j R_i^T) with forward-mode duals, dense normal equations by one owner per block row (no
 //      floating-point atomics), k_chol_fused, fixed-order reductions: repeated calls are bit-identical.
 #include "r3d_internal.cuh"
+#include "averaging.cuh"
 #include "ba_model.cuh"
 #include "detmath.cuh"
 #include "relpose_math.cuh"
@@ -123,28 +124,6 @@ __global__ void __launch_bounds__(kTThreads) k_rotavg_triplets(const uint32_t* _
     if (nt) atomicAdd(&counts[0], nt);
     if (nv) atomicAdd(&counts[1], nv);
   }
-}
-
-// ---- fixed-order block reductions -------------------------------------------------------------------------------
-template <int kThreads>
-__device__ double block_sum_fixed(double v, double* red) {
-  for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31u) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < kThreads / 32; ++w) s += red[w];
-  return s;
-}
-template <int kThreads>
-__device__ double block_max_fixed(double v, double* red) {
-  for (int o = 16; o >= 1; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();
-  if ((threadIdx.x & 31u) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < kThreads / 32; ++w) s = fmax(s, red[w]);
-  return s;
 }
 
 // ---- 3. L2 initialisation ---------------------------------------------------------------------------------------
@@ -591,14 +570,6 @@ __global__ void __launch_bounds__(kOThreads) k_rotavg_step(const double* __restr
 }
 
 // ---- host ---------------------------------------------------------------------------------------------------------
-double now_ms() {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
-}
-
-// 2-edge-connected components of an undirected multigraph on nodes 0..n-1 (edge k = (eu[k], ev[k]); parallel edges are
-// not bridges, self-loops are ignored): bridges by Tarjan's low-link (iterative DFS), then connected components of the
-// remaining edges.  Returns the component with the most nodes (>= 2; a tie keeps the one holding the smallest node), or
-// -1; comp[v] = component of v, -1 for nodes without edges.
 int largest_biedge_component(uint32_t n, const std::vector<uint32_t>& eu, const std::vector<uint32_t>& ev, std::vector<int>& comp) {
   const size_t E = eu.size();
   std::vector<uint32_t> ofs(n + 1, 0);
@@ -670,20 +641,6 @@ int largest_biedge_component(uint32_t n, const std::vector<uint32_t>& eu, const 
     if (size[c] >= 2 && (best < 0 || size[c] > size[(size_t)best])) best = (int)c;
   return best;
 }
-
-template <typename T>
-struct DevArr {  // device scratch out of the worker's pool (context.cu)
-  DeviceWorker* w;
-  T* p = nullptr;
-  explicit DevArr(DeviceWorker& worker) : w(&worker) {}
-  DevArr(const DevArr&) = delete;
-  DevArr& operator=(const DevArr&) = delete;
-  ~DevArr() { if (p) pool_release(*w, p); }
-  bool alloc(size_t n) {
-    p = (T*)pool_alloc(*w, std::max<size_t>(n, 1) * sizeof(T));
-    return p != nullptr;
-  }
-};
 
 // the deterministic start of the inverse iteration (the oracle draws the same numbers)
 double init_value(uint64_t k) {
