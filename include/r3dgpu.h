@@ -545,6 +545,23 @@ int r3d_debug_ba_jacobian_model(int model, const double* intr, const double* ext
 /* pose-centre prior block: r[3] = weight .* (C(pose) - center), J[3 x 6] = d r / d (angle-axis, t) */
 int r3d_debug_ba_prior(const double* pose, const double* center, const double* weight, double* r, double* J);
 
+/* Diagnostics (device): the library's dense solvers on a caller's matrix, through the launch code the solvers use.
+ * Factor A = L L^T and solve A x = b.  A is (n+1) x n row-major: rows 0..n-1 the matrix (only the lower triangle is
+ * read), row n the right-hand side b.  method 0 = k_chol_fused, the cooperative kernel of bundle adjustment, rotation
+ * and translation averaging (grid = CTAs, 0 = one per SM as those solvers launch it); method 1 = k_chol_envelope, the
+ * envelope kernel of R3D_BA_CHOL=envelope (n even; ft = first column tile of each of the ceil((n+1)/32) row tiles,
+ * 0 <= ft[t] <= t, at most 24 active row tiles per panel; grid = cluster size 1..8, 0 = 8).  Outputs: L_out (n+1) x n
+ * (the factor, zero above the diagonal; row n = y = L^-1 b), x_out (n) = A^-1 b, Linv_out (method 0 only, may be NULL:
+ * ceil(n/32) row-major 32 x 32 inverses of the diagonal blocks of L, identity-padded), *not_pd = 1 when the
+ * factorisation met a pivot that is not > 0 (or NaN).  Bad arguments return R3D_ERR_INVALID before anything runs. */
+int r3d_debug_cholesky(r3d_ctx* ctx, int method, int n, const double* A, const int* ft, int grid, double* L_out,
+                       double* x_out, double* Linv_out, int* not_pd);
+/* A X = Y for 3 right-hand sides: k_chol_fused as rotation averaging launches it, then k_rotavg_trsm3 exactly as one
+ * inverse iteration of its initialisation runs it.  A n x n row-major (lower triangle read), Y and X_out n x 3
+ * row-major; grid = CTAs of the triangular solves, 0 = the occupancy the initialisation uses.  R3D_ERR_INVALID when
+ * A is not positive definite. */
+int r3d_debug_chol_solve3(r3d_ctx* ctx, int n, const double* A, const double* Y, int grid, double* X_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -36,8 +36,10 @@ EXPORTS = [
     "r3d_sfm_structure_from_tracks", "r3d_sfm_remove_outliers", "r3d_cascade_prepare", "r3d_debug_cascade_view",
     "r3d_relpose_default_options", "r3d_relative_poses", "r3d_get_relpose_timing",
     "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_matches_keep_largest_biedge_component",
-    "r3d_transavg_default_options", "r3d_translation_averaging",
+    "r3d_transavg_default_options", "r3d_translation_averaging", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
 ]
+
+CHOL_DENSE, CHOL_ENVELOPE = 0, 1
 
 
 class R3DError(RuntimeError):
@@ -677,6 +679,39 @@ class Context:
         eps = C.c_float()
         self._check(lib().r3d_debug_candidate_keys(self._h, C.c_uint32(view_db), C.c_uint32(view_query), _p(keys), C.byref(eps)))
         return keys, eps.value
+
+    def debug_cholesky(self, A, method=CHOL_DENSE, ft=None, grid=0):
+        """r3d_debug_cholesky on A ((n+1) x n: the matrix, whose lower triangle is read, and b as row n).  Returns
+        (L (n+1) x n with y = L^-1 b as row n, x = A^-1 b, Linv (ceil(n/32), 32, 32) or None for the envelope
+        kernel, not_pd bool)."""
+        A = np.ascontiguousarray(A, np.float64)
+        if A.ndim != 2 or A.shape[0] != A.shape[1] + 1:
+            raise ValueError("A must be (n+1) x n")
+        n = A.shape[1]
+        ftp = None
+        if ft is not None:
+            ft = np.ascontiguousarray(ft, np.int32).ravel()
+            if len(ft) != (n + 32) // 32:  # the library reads one entry per row tile of rows 0..n
+                raise ValueError("ft must hold ceil((n+1)/32) = %d entries, not %d" % ((n + 32) // 32, len(ft)))
+            ftp = _p(ft)
+        L = np.empty((n + 1, n))
+        x = np.empty(n)
+        Linv = np.empty(((n + 31) // 32, 32, 32)) if method == CHOL_DENSE else None
+        bad = C.c_int()
+        self._check(lib().r3d_debug_cholesky(self._h, C.c_int(method), C.c_int(n), _p(A), ftp, C.c_int(grid), _p(L), _p(x),
+                                             None if Linv is None else _p(Linv), C.byref(bad)))
+        return L, x, Linv, bool(bad.value)
+
+    def debug_chol_solve3(self, A, Y, grid=0):
+        """r3d_debug_chol_solve3: X = A^-1 Y for A n x n (lower triangle read) and Y n x 3."""
+        A = np.ascontiguousarray(A, np.float64)
+        Y = np.ascontiguousarray(Y, np.float64)
+        n = A.shape[1]
+        if A.shape != (n, n) or Y.shape != (n, 3):
+            raise ValueError("A must be n x n and Y n x 3")
+        X = np.empty((n, 3))
+        self._check(lib().r3d_debug_chol_solve3(self._h, C.c_int(n), _p(A), _p(Y), C.c_int(grid), _p(X)))
+        return X
 
     def filter_pairs(self, putative, widths, heights, model=MODEL_F, precision_px=4.0, max_iter=2048, Ks=None):
         n = len(widths)

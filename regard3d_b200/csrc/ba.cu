@@ -727,6 +727,10 @@ __global__ void __launch_bounds__(1024, 1) k_chol_fused(double* A, double* Lm, d
 // with ld.global.cg (L2): the SMs' L1 caches are not coherent.  The backward substitution (CTA 0) skips what lies
 // outside the envelope too.  The host picks this kernel when every |R_k| <= kEnvMaxActive and the tile-pair count says
 // it is cheaper than the dense cooperative kernel.
+// Preconditions (envelope_cholesky checks them on the host): n is EVEN -- rows are loaded as double2, so row r starts
+// 16-byte aligned only when r * n is even (BA's nB = 6 (C + G) always is); A and Lm hold 64 doubles of slack past
+// (n+1) x n (the rhs row is read as whole 32-wide rows); 0 <= ft[t] <= t for the ceil((n+1) / 32) row tiles.  Only
+// the lower triangle of A is read.
 constexpr int kEnvThreads = 512;
 constexpr int kEnvWarps = kEnvThreads / 32;
 constexpr int kEnvMaxActive = 24;
@@ -1025,15 +1029,45 @@ __global__ void __launch_bounds__(256) k_ba_update(Dev d, double inv_radius) {
 
 }  // namespace ba
 
-int dense_cholesky(r3d_ctx* ctx, DeviceWorker& w, double* A, double* L, double* Linv, int n, double* flag, double* x) {
-  static_assert(kCholNB == ba::NB, "Linv layout");
+int dense_cholesky_grid(r3d_ctx* ctx, DeviceWorker& w, int* grid) {
   int per_sm = 0;
   R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(ba::k_chol_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ba::kCholSmemBytes));
   R3D_CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, ba::k_chol_fused, 1024, ba::kCholSmemBytes));
   if (per_sm < 1) return fail(ctx, R3D_ERR_CUDA, "dense Cholesky: k_chol_fused does not fit on an SM");
+  if (*grid == 0) *grid = w.sm_count;
+  if (*grid < 1 || *grid > per_sm * w.sm_count)
+    return fail(ctx, R3D_ERR_INVALID, "dense Cholesky: " + std::to_string(*grid) + " CTAs cannot be co-resident");
+  return R3D_OK;
+}
+
+int dense_cholesky(r3d_ctx* ctx, DeviceWorker& w, double* A, double* L, double* Linv, int n, double* flag, double* x, int grid) {
+  static_assert(kCholNB == ba::NB, "Linv layout");
+  int rc;
+  if ((rc = dense_cholesky_grid(ctx, w, &grid))) return rc;
   void* args[] = {&A, &L, &Linv, &n, &flag, &x};
-  R3D_CUDA_TRY(ctx, cudaLaunchCooperativeKernel((void*)ba::k_chol_fused, dim3(w.sm_count), dim3(32, 32), args, ba::kCholSmemBytes,
+  R3D_CUDA_TRY(ctx, cudaLaunchCooperativeKernel((void*)ba::k_chol_fused, dim3(grid), dim3(32, 32), args, ba::kCholSmemBytes,
                                                 w.stream));
+  return R3D_OK;
+}
+
+int envelope_cholesky(r3d_ctx* ctx, DeviceWorker& w, double* A, double* L, int n, const int* ft, int ctas, double* flag, double* x) {
+  if (ctas < 1 || ctas > ba::kEnvMaxCluster)
+    return fail(ctx, R3D_ERR_INVALID, "envelope Cholesky: cluster of " + std::to_string(ctas) + " CTAs");
+  if (n % 2) return fail(ctx, R3D_ERR_INVALID, "envelope Cholesky: n must be even");
+  R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(ba::k_chol_envelope, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ba::kEnvSmemBytes));
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(ctas);
+  cfg.blockDim = dim3(ba::kEnvThreads);
+  cfg.dynamicSmemBytes = ba::kEnvSmemBytes;
+  cfg.stream = w.stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = ctas;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  R3D_CUDA_TRY(ctx, cudaLaunchKernelEx(&cfg, ba::k_chol_envelope, A, L, n, ft, flag, x));
   return R3D_OK;
 }
 
@@ -1422,13 +1456,6 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
   const int chol_blocks = (nB + r3d::ba::NB - 1) / r3d::ba::NB;
   R3D_CUDA_TRY(ctx, mem.alloc(&d_Lm, ((size_t)nB + 1) * nB + 64));
   R3D_CUDA_TRY(ctx, mem.alloc(&d_Linv, (size_t)chol_blocks * r3d::ba::NB * r3d::ba::NB));
-  int chol_grid = w.sm_count;  // persistent: one CTA per SM, all co-resident (cooperative launch)
-  {
-    int per_sm = 0;
-    R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(r3d::ba::k_chol_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)r3d::ba::kCholSmemBytes));
-    R3D_CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, r3d::ba::k_chol_fused, 1024, r3d::ba::kCholSmemBytes));
-    if (per_sm < 1) return fail(ctx, R3D_ERR_CUDA, "bundle adjustment: k_chol_fused does not fit on an SM");
-  }
   // Envelope of the reduced system at tile granularity (the union over ranks: every rank factors the summed S)
   bool use_env = false;
   int env_ctas = r3d::ba::kEnvMaxCluster;  // CTAs of the envelope kernel's cluster
@@ -1482,7 +1509,6 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
       R3D_CUDA_TRY(ctx, mem.alloc(&d_ft, (size_t)ntr));
       R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_ft, ft.data(), (size_t)ntr * sizeof(int), cudaMemcpyHostToDevice, w.stream));
       R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));  // ft is a local
-      R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(r3d::ba::k_chol_envelope, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)r3d::ba::kEnvSmemBytes));
     }
     static const bool dbg = getenv("R3D_DEBUG_TIMING") != nullptr;
     if (dbg) fprintf(stderr, "[r3d] BA linear solve: %s (n = %d, %d tiles, <= %d active row tiles per panel, estimate %.0f vs %.0f us dense)\n",
@@ -1560,24 +1586,9 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
       r3d::ba::k_ba_finish_S<<<g, b, 0, w.stream>>>(d, inv_radius);
     }
     if (use_env) {
-      cudaLaunchConfig_t cfg = {};
-      cfg.gridDim = dim3(env_ctas);
-      cfg.blockDim = dim3(r3d::ba::kEnvThreads);
-      cfg.dynamicSmemBytes = r3d::ba::kEnvSmemBytes;
-      cfg.stream = w.stream;
-      cudaLaunchAttribute attr[1];
-      attr[0].id = cudaLaunchAttributeClusterDimension;
-      attr[0].val.clusterDim.x = env_ctas;
-      attr[0].val.clusterDim.y = 1;
-      attr[0].val.clusterDim.z = 1;
-      cfg.attrs = attr;
-      cfg.numAttrs = 1;
-      R3D_CUDA_TRY(ctx, cudaLaunchKernelEx(&cfg, r3d::ba::k_chol_envelope, d.S, d_Lm, nB, (const int*)d_ft, d.scal + 4, d.delta));
+      if ((rc = envelope_cholesky(ctx, w, d.S, d_Lm, nB, d_ft, env_ctas, d.scal + 4, d.delta))) return rc;
     } else {
-      double *pA = d.S, *pL = d_Lm, *pI = d_Linv, *pflag = d.scal + 4, *px = d.delta;
-      int pn = nB;
-      void* cargs[] = {&pA, &pL, &pI, &pn, &pflag, &px};
-      R3D_CUDA_TRY(ctx, cudaLaunchCooperativeKernel((void*)r3d::ba::k_chol_fused, dim3(chol_grid), dim3(32, 32), cargs, r3d::ba::kCholSmemBytes, w.stream));
+      if ((rc = dense_cholesky(ctx, w, d.S, d_Lm, d_Linv, nB, d.scal + 4, d.delta))) return rc;
     }
     r3d::ba::k_ba_backsub<<<(d.n_pts + 127) / 128, 128, 0, w.stream>>>(d);
     r3d::ba::k_ba_update<<<w.sm_count * 4, 256, 0, w.stream>>>(d, inv_radius);
@@ -1629,6 +1640,63 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(p->points, d.pts, 3 * (size_t)p->n_pts * 8, cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
   sum->seconds_total = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
+  return R3D_OK;
+}
+
+int r3d_debug_cholesky(r3d_ctx* ctx, int method, int n, const double* A, const int* ft, int grid, double* L_out, double* x_out,
+                       double* Linv_out, int* not_pd) {
+  if (!ctx || !A || !L_out || !x_out || !not_pd || n < 1 || (method != 0 && method != 1) || grid < 0)
+    return fail(ctx, R3D_ERR_INVALID, "r3d_debug_cholesky: bad arguments");
+  const int NB = r3d::ba::NB;
+  const int nblk = (n + NB - 1) / NB, ntr = (n + 1 + NB - 1) / NB;
+  if (method == 1) {  // everything the envelope kernel assumes, before anything reaches the device
+    if (n % 2) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_cholesky: the envelope kernel needs an even n");
+    if (!ft || grid > r3d::ba::kEnvMaxCluster) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_cholesky: bad ft / cluster size");
+    for (int t = 0; t < ntr; ++t)
+      if (ft[t] < 0 || ft[t] > t) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_cholesky: ft[" + std::to_string(t) + "] outside 0.." + std::to_string(t));
+    for (int k = 0; k < nblk; ++k) {
+      int act = 0;
+      for (int ti = k + 1; ti < ntr; ++ti) act += ft[ti] <= k;
+      if (act > r3d::ba::kEnvMaxActive)
+        return fail(ctx, R3D_ERR_INVALID, "r3d_debug_cholesky: panel " + std::to_string(k) + " has " + std::to_string(act) + " active row tiles");
+    }
+  }
+  DeviceWorker& w = ctx->workers[0];
+  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
+  int rc;
+  if (method == 0 && (rc = dense_cholesky_grid(ctx, w, &grid))) return rc;
+  DeviceArrays mem;
+  mem.w = &w;
+  const size_t nA = (size_t)(n + 1) * n;
+  double *dA, *dL, *dLinv, *dx, *dflag;
+  int* dft = nullptr;
+  // as r3d_bundle_adjust allocates S | rhs and Lm: 64 doubles of slack that k_chol_envelope reads past row n
+  R3D_CUDA_TRY(ctx, mem.alloc(&dA, nA + 64));
+  R3D_CUDA_TRY(ctx, mem.alloc(&dL, nA + 64));
+  R3D_CUDA_TRY(ctx, mem.alloc(&dLinv, (size_t)nblk * NB * NB));
+  R3D_CUDA_TRY(ctx, mem.alloc(&dx, (size_t)n));
+  R3D_CUDA_TRY(ctx, mem.alloc(&dflag, 1));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(dA, A, nA * sizeof(double), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(dA + nA, 0, 64 * sizeof(double), w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(dL, 0, (nA + 64) * sizeof(double), w.stream));  // the upper triangle comes back as 0
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(dLinv, 0, (size_t)nblk * NB * NB * sizeof(double), w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(dflag, 0, sizeof(double), w.stream));
+  if (method == 0) {
+    if ((rc = dense_cholesky(ctx, w, dA, dL, dLinv, n, dflag, dx, grid))) return rc;
+  } else {
+    R3D_CUDA_TRY(ctx, mem.alloc(&dft, (size_t)ntr));
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(dft, ft, (size_t)ntr * sizeof(int), cudaMemcpyHostToDevice, w.stream));
+    if ((rc = envelope_cholesky(ctx, w, dA, dL, n, dft, grid ? grid : r3d::ba::kEnvMaxCluster, dflag, dx))) return rc;
+  }
+  R3D_CUDA_TRY(ctx, cudaGetLastError());
+  double flag = 0.0;
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(L_out, dL, nA * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(x_out, dx, (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  if (Linv_out && method == 0)
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(Linv_out, dLinv, (size_t)nblk * NB * NB * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(&flag, dflag, sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+  *not_pd = flag != 0.0;
   return R3D_OK;
 }
 

@@ -214,9 +214,16 @@ int ensure_capacity(r3d_ctx* ctx, void** p, size_t* cap, size_t need_elems) {
 // dense Cholesky + both triangular solves of an SPD system on the worker's stream (ba.cu: the cooperative k_chol_fused,
 // one CTA per SM).  A: (n+1) x n row-major, the system with its right-hand side as row n, overwritten; L: (n+1) x n + 64,
 // receives the lower factor (row n: the forward-substituted rhs); Linv: ceil(n / kCholNB) inverses of the kCholNB x kCholNB
-// diagonal blocks of L; *flag (zeroed by the caller) becomes 1 when A is not positive definite; x: n, the solution
+// diagonal blocks of L; *flag (zeroed by the caller) becomes 1 when A is not positive definite; x: n, the solution.
+// Only the lower triangle of A is read.  grid: CTAs of the cooperative launch, 0 = one per SM (R3D_ERR_INVALID beyond
+// what can be co-resident); the result does not depend on it.
 constexpr int kCholNB = 32;
-int dense_cholesky(r3d_ctx* ctx, DeviceWorker& w, double* A, double* L, double* Linv, int n, double* flag, double* x);
+int dense_cholesky(r3d_ctx* ctx, DeviceWorker& w, double* A, double* L, double* Linv, int n, double* flag, double* x, int grid = 0);
+int dense_cholesky_grid(r3d_ctx* ctx, DeviceWorker& w, int* grid);  // resolves grid 0, checks co-residency
+// the same with the envelope kernel (ba.cu: k_chol_envelope on ONE cluster of `ctas` = 1..8 CTAs, R3D_ERR_INVALID
+// otherwise or for an odd n).  A and L: (n+1) x n + 64 (the slack is read, never used); ft (device): first column tile
+// of each of the ceil((n+1) / kCholNB) row tiles, every panel at most 24 active row tiles (the caller checks); no Linv.
+int envelope_cholesky(r3d_ctx* ctx, DeviceWorker& w, double* A, double* L, int n, const int* ft, int ctas, double* flag, double* x);
 
 int prepare_views(r3d_ctx* ctx, DeviceWorker& w);
 void* pool_alloc(DeviceWorker& w, size_t bytes);  // nullptr on failure

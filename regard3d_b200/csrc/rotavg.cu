@@ -570,6 +570,24 @@ __global__ void __launch_bounds__(kOThreads) k_rotavg_step(const double* __restr
 }
 
 // ---- host ---------------------------------------------------------------------------------------------------------
+// cooperative grid of k_rotavg_trsm3: grid 0 = up to 4 CTAs per SM as occupancy allows (what the inverse iteration
+// runs), otherwise the caller's, R3D_ERR_INVALID when that many CTAs cannot be co-resident
+int trsm3_grid(r3d_ctx* ctx, DeviceWorker& w, int* grid) {
+  int per_sm = 0;
+  R3D_CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rotavg_trsm3, kSThreads, 0));
+  if (*grid == 0) *grid = w.sm_count * std::max(1, std::min(per_sm, 4));
+  if (*grid < 1 || *grid > std::max(per_sm, 0) * w.sm_count)
+    return fail(ctx, R3D_ERR_INVALID, "k_rotavg_trsm3: " + std::to_string(*grid) + " CTAs cannot be co-resident");
+  return R3D_OK;
+}
+
+// L Lt X = Y in place of Y (n x 3), Z: n x 3 scratch; L, Linv from dense_cholesky; grid from trsm3_grid
+int trsm3(r3d_ctx* ctx, DeviceWorker& w, const double* L, const double* Linv, int n, double* Y, double* Z, int grid) {
+  void* args[] = {&L, &Linv, &n, &Y, &Z};
+  R3D_CUDA_TRY(ctx, cudaLaunchCooperativeKernel((void*)k_rotavg_trsm3, dim3(grid), dim3(kSThreads), args, 0, w.stream));
+  return R3D_OK;
+}
+
 int largest_biedge_component(uint32_t n, const std::vector<uint32_t>& eu, const std::vector<uint32_t>& ev, std::vector<int>& comp) {
   const size_t E = eu.size();
   std::vector<uint32_t> ofs(n + 1, 0);
@@ -827,18 +845,11 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
   if ((rc = read_scal())) return rc;
   if (scal[7] != 0.0) return fail(ctx, R3D_ERR_CUDA, "r3d_rotation_averaging: M + sigma I is not positive definite");
   int trsm_grid = 0;
-  {
-    int per_sm = 0;
-    R3D_CUDA_TRY(ctx, cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_rotavg_trsm3, kSThreads, 0));
-    trsm_grid = w.sm_count * std::max(1, std::min(per_sm, 4));
-  }
+  if ((rc = trsm3_grid(ctx, w, &trsm_grid))) return rc;
   uint32_t it = 0;
   for (; it < kInitMaxIter;) {
     ++it;
-    double *pL = d_L.p, *pI = d_Linv.p, *pY = d_Y.p, *pZ = d_Z.p;
-    int pn = N;
-    void* args[] = {&pL, &pI, &pn, &pY, &pZ};
-    R3D_CUDA_TRY(ctx, cudaLaunchCooperativeKernel((void*)k_rotavg_trsm3, dim3(trsm_grid), dim3(kSThreads), args, 0, w.stream));
+    if ((rc = trsm3(ctx, w, d_L.p, d_Linv.p, N, d_Y.p, d_Z.p, trsm_grid))) return rc;
     k_rotavg_orth<<<1, kOThreads, 0, w.stream>>>(d_Y.p, d_Q.p, N, 0, d_scal.p);
     R3D_CUDA_TRY(ctx, cudaGetLastError());
     if ((rc = read_scal())) return rc;
@@ -1005,6 +1016,32 @@ extern "C" int r3d_rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel
   if (opt->method != R3D_ROTAVG_L2) return fail(ctx, R3D_ERR_INVALID, "r3d_rotation_averaging: unknown method");
   if (!(opt->max_angular_error_deg > 0.0)) return fail(ctx, R3D_ERR_INVALID, "r3d_rotation_averaging: max_angular_error_deg <= 0");
   return ra::rotation_averaging(ctx, rel, n_rel, n_views, *opt, rotations, view_kept, edge_kept, edge_support, *summary);
+}
+
+extern "C" int r3d_debug_chol_solve3(r3d_ctx* ctx, int n, const double* A, const double* Y, int grid, double* X_out) {
+  if (!ctx || n < 1 || !A || !Y || !X_out || grid < 0) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_chol_solve3: bad arguments");
+  DeviceWorker& w = ctx->workers[0];
+  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
+  int rc;
+  if ((rc = ra::trsm3_grid(ctx, w, &grid))) return rc;
+  const int nblk = (n + kCholNB - 1) / kCholNB;
+  // as rotation_averaging allocates them: M | unused rhs row, L with the slack of dense_cholesky's contract
+  ra::DevArr<double> d_A(w), d_L(w), d_Linv(w), d_x(w), d_Y(w), d_Z(w), d_flag(w);
+  if (!d_A.alloc((size_t)(n + 1) * n) || !d_L.alloc((size_t)(n + 1) * n + 64) || !d_Linv.alloc((size_t)nblk * kCholNB * kCholNB) ||
+      !d_x.alloc(n) || !d_Y.alloc(3 * (size_t)n) || !d_Z.alloc(3 * (size_t)n) || !d_flag.alloc(1))
+    return fail(ctx, R3D_ERR_NOMEM, "r3d_debug_chol_solve3: device scratch");
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_A.p, A, (size_t)n * n * sizeof(double), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_A.p + (size_t)n * n, 0, (size_t)n * sizeof(double), w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_Y.p, Y, 3 * (size_t)n * sizeof(double), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_flag.p, 0, sizeof(double), w.stream));
+  if ((rc = dense_cholesky(ctx, w, d_A.p, d_L.p, d_Linv.p, n, d_flag.p, d_x.p))) return rc;
+  if ((rc = ra::trsm3(ctx, w, d_L.p, d_Linv.p, n, d_Y.p, d_Z.p, grid))) return rc;
+  double flag = 0.0;
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(&flag, d_flag.p, sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(X_out, d_Y.p, 3 * (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+  if (flag != 0.0) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_chol_solve3: A is not positive definite");
+  return R3D_OK;
 }
 
 extern "C" int r3d_matches_keep_largest_biedge_component(const r3d_matches* m, r3d_matches** out) {

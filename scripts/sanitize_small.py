@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Small-shape pass over every kernel family for `compute-sanitizer` (memcheck / racecheck / synccheck / initcheck):
 
-    compute-sanitizer --tool racecheck python scripts/sanitize_small.py [match|filter|ba|liop|cascade|ba_envelope|all]
+    compute-sanitizer --tool racecheck python scripts/sanitize_small.py [match|filter|ba|liop|cascade|ba_envelope|chol|all]
 
 Shapes are tiny on purpose (the sanitizer serialises everything); correctness of the results is checked by the
 `-m gpu` tests, this script only has to execute every kernel once."""
@@ -74,6 +74,21 @@ if what in ("ba_envelope", "all"):
     s, trace = ctx.bundle_adjust(arrs, max_iterations=2)
     print("ba (envelope Cholesky, cluster of 8):", s["iterations"], "iterations, cost", trace[0], "->", trace[-1])
     del os.environ["R3D_BA_CHOL"]
+if what in ("chol", "all"):
+    # the dense solvers through their debug entry points: k_chol_fused at n = 33 (a partial second panel, rhs row in
+    # the last diagonal tile), k_chol_envelope at n = 64 on a cluster of 2 (rhs row in a tile of its own), and
+    # k_chol_fused + k_rotavg_trsm3 on 33 x 3 right-hand sides
+    rng = np.random.default_rng(3)
+    for n, method, ft, grid in ((33, capi.CHOL_DENSE, None, 0), (64, capi.CHOL_ENVELOPE, np.array([0, 0, 0], np.int32), 2)):
+        G = rng.standard_normal((n, n))
+        A = np.vstack([G @ G.T + n * np.eye(n), rng.standard_normal((1, n))])
+        L, x, _, bad = ctx.debug_cholesky(A, method, ft=ft, grid=grid)
+        print("chol method %d n %d: residual %.2e, not_pd %d" % (method, n, np.abs(A[:n] @ x - A[n]).max(), bad))
+    G = rng.standard_normal((33, 33))
+    A = G @ G.T + 33 * np.eye(33)
+    Y = rng.standard_normal((33, 3))
+    X = ctx.debug_chol_solve3(A, Y)
+    print("chol_solve3 n 33: residual %.2e" % np.abs(A @ X - Y).max())
 if what in ("liop", "all"):
     rng = np.random.default_rng(1)
     img = rng.random((120, 160)).astype(np.float32)

@@ -174,6 +174,22 @@ def test_envelope_cholesky_equals_the_dense_solve(gpu_ctx, monkeypatch, ctas):
     iterates as the dense cooperative kernel on a sequence-like scene whose reduced system is banded + bordered
     (ring of cameras, shared intrinsics, the rhs row inside the last diagonal tile: 6 * 37 + 6 = 228 = 7 * 32 + 4)."""
     prob = synth.make_ba_problem(n_cams=37, n_pts=4000, obs_per_pt=4, seed=41)
+    _envelope_equals_dense(gpu_ctx, monkeypatch, prob, ctas)
+
+
+@pytest.mark.parametrize("ctas", ["1", "8"])
+def test_envelope_cholesky_rhs_in_its_own_tile(gpu_ctx, monkeypatch, ctas):
+    """The same with nB % 32 == 0 (47 cameras, one refined intrinsic group: 6 * 48 = 288 = 9 * 32): the rhs row of the
+    reduced system lies in a row tile of its own, so the envelope kernel takes its other forward-substitution path."""
+    prob = synth.make_ba_problem(n_cams=47, n_pts=4000, obs_per_pt=4, seed=47)
+    assert 6 * (len(prob["poses"]) + len(prob["intrinsics"])) == 288
+    _envelope_equals_dense(gpu_ctx, monkeypatch, prob, ctas)
+
+
+def _envelope_equals_dense(gpu_ctx, monkeypatch, prob, ctas):
+    # A tolerance, not bits: two BA runs with identical settings already differ in the last bits (the gradient, the
+    # cost and the reduced system are summed with floating-point atomics).  That the cluster size changes no bit of
+    # the factorisation itself is asserted on the kernel (test_gpu_dense_cholesky.py).
     out = {}
     for mode in ("dense", "envelope"):
         monkeypatch.setenv("R3D_BA_CHOL", mode)
