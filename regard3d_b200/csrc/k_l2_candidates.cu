@@ -17,10 +17,12 @@
 //     fp16: 2 consumers (the 128-register f32 accumulator leaves no room for more); per 256-row tile, m64n256k16,
 //           then the epilogue.
 //     u8:   4 consumers, so every database tile in shared memory feeds 256 query rows; per 128-row half tile,
-//           m64n128k32 into one 64-register s32 accumulator, then the epilogue of that half.  While one consumer
-//           reduces, the other three keep MMAs in the tensor pipe.  The database map loads every 32-row group with
-//           its row pairs transposed (context.cu), so each lane of a quad holds whole chunks: the chunk minima take no
-//           shuffle, and only the keys below their set's largest are inserted, in warp-uniform rounds.
+//           m64n128k32 (the K extent fixed at compile time: back-to-back MMAs, no branch) into one 64-register s32
+//           accumulator, then the epilogue of that half.  While one consumer reduces, the other three keep MMAs in the
+//           tensor pipe.  The database map loads every 32-row group with its row pairs transposed (context.cu), so
+//           each lane of a quad holds whole chunks: the chunk minima take no shuffle.  An integer bound taken once per
+//           half from each set's largest key rejects nearly every chunk before its key is formed; the rest are
+//           inserted in warp-uniform rounds.
 // Barriers: full[s] (TMA bytes landed), empty[s] (every consumer warp is done with the stage), qfull / qempty the same
 // for the query buffers.
 #include "r3d_internal.cuh"
@@ -55,6 +57,21 @@ __device__ __forceinline__ int32_t min8(const int32_t (&v)[8]) {
   return __vimin3_s32(__vimin3_s32(v[0], v[1], v[2]), __vimin3_s32(v[3], v[4], v[5]), min(v[6], v[7]));
 }
 
+// u8: the packed key of a chunk whose bracket minimum (min of ||a||^2 - 2 q.a) is m; exact: real distances are < 2^24
+__device__ __forceinline__ float chunk_key(int32_t m, int32_t qn, uint32_t cid, uint32_t keep_mask) {
+  return __uint_as_float((__float_as_uint((float)(m + qn)) & keep_mask) | cid);
+}
+
+// u8: an integer bound on the bracket minima whose keys can be below kmax.  Such a key's bits above the chunk bits are
+// at most those of kmax, so its distance converts to a float below F = ((kmax & keep_mask) + 2^chunk_bits) as bits.
+// Rounding to nearest is monotone and F is a float, so every integer distance >= F converts to a float >= F:
+// m + qn <= ceil(F) - 1 keeps every chunk that can enter the set (and a few that cannot: the network drops those).
+// F is +inf while the set holds the FLT_MAX sentinel; the conversion saturates to INT_MAX there.
+__device__ __forceinline__ int32_t bracket_bound(float kmax, uint32_t keep_mask, int32_t qn) {
+  const float f = __uint_as_float((__float_as_uint(kmax) & keep_mask) - keep_mask);  // - keep_mask = + 2^chunk_bits
+  return __float2int_ru(f) - 1 - qn;
+}
+
 // the kNumKeys smallest keys of this lane's set and the set of lane ^ d (the keys of different chunks differ)
 __device__ __forceinline__ void merge_keys(float (&key)[kNumKeys], int d) {
   float y[kNumKeys];
@@ -75,12 +92,15 @@ __device__ __forceinline__ void merge_keys(float (&key)[kNumKeys], int d) {
 
 }  // namespace
 
-template <bool kU8, uint32_t kConsumers>
+// kKSteps: u8, the k32 steps of the descriptor (ceil(D / 32), so ceil(kKSteps / 4) K-blocks); 0 on the fp16 path,
+// which takes nkb and ksteps at run time.
+template <bool kU8, uint32_t kConsumers, uint32_t kKSteps>
 __global__ void __launch_bounds__(128 * (kConsumers + 1), 1)
 k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __restrict__ tmapD,
                 const PairDesc* __restrict__ pairs, const WorkItem* __restrict__ items, uint32_t n_items,
                 uint32_t* __restrict__ keys_out, uint32_t nkb, uint32_t ksteps, uint32_t n_stages, uint32_t n_qbuf) {
   static_assert(kConsumers == 2 || (kU8 && kConsumers == 4), "fp16: 2 consumers; u8: 2 or 4");
+  static_assert(kU8 ? (kKSteps >= 1 && kKSteps <= 8) : kKSteps == 0, "u8: 1 .. 8 k32 steps (D <= 256); fp16: 0");
   constexpr uint32_t kBoxCols = kU8 ? 128u : (uint32_t)kKBlock;  // elements in a 128-byte box row
   constexpr uint32_t kQBoxes = kConsumers / 2;                   // 128-row query boxes per K-block
   constexpr uint32_t kBlockRows = kQBoxes * kTileRows;           // query rows per work item
@@ -193,20 +213,20 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       const int32_t qn0 = __ldg(pd.normJ + wi.sb * kBlockRows + row0);
       const int32_t qn1 = __ldg(pd.normJ + wi.sb * kBlockRows + row0 + 8u);
       int32_t acc[64];
-      // MMAs of half h (database rows h * 128 .. + 127) of the tile whose K-blocks start at stage s0
+      constexpr uint32_t kNkb = (kKSteps + 3) / 4;
+      // MMAs of half h (database rows h * 128 .. + 127) of the tile whose K-blocks start at stage s0: kKSteps
+      // back-to-back m64n128k32 behind one fence, no branch
       auto issue = [&](uint32_t h, uint32_t s0) {
         wgmma_fence();
-        uint32_t s = s0, ks_left = ksteps;
-        for (uint32_t kb = 0; kb < nkb; ++kb) {
+        uint32_t s = s0;
+#pragma unroll
+        for (uint32_t kb = 0; kb < kNkb; ++kb) {
           const uint32_t a_lo = desc_lo(a_base + kb * kBoxBytes);
           const uint32_t b_lo = desc_lo(d_base + s * kStageBytes + h * kBoxBytes);
-          const uint32_t ks_here = ks_left < 4u ? ks_left : 4u;
 #pragma unroll
-          for (uint32_t k = 0; k < 4; ++k) {
-            if (k < ks_here) wgmma_m64n128k32_u8(acc, make_desc(a_lo + 2 * k), make_desc(b_lo + 2 * k), (kb | k) != 0u ? 1u : 0u);
-          }
-          ks_left -= ks_here;
-          if (++s == n_stages) s = 0;
+          for (uint32_t k = 0; k < 4 && 4 * kb + k < kKSteps; ++k)
+            wgmma_m64n128k32_u8(acc, make_desc(a_lo + 2 * k), make_desc(b_lo + 2 * k), (kb | k) != 0u ? 1u : 0u);
+          if (kb + 1 < kNkb && ++s == n_stages) s = 0;
         }
         wgmma_commit();
       };
@@ -216,15 +236,19 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       // are the 8 rows of chunk t * 32 + h * 16 + 4 g + q, and their norms are 8 consecutive words of shared memory.
       // ||q - a||^2 = ||q||^2 + (||a||^2 - 2 q.a): each lane takes the minima of its chunks over the bracket, exactly
       // in s32 and without leaving its registers.
-      // A candidate can only enter its set if it is below the set's largest key, which never grows: the candidates
-      // that pass are inserted in warp-uniform rounds, one per set and lane per round (FLT_MAX, a no-op of the
-      // network, where a lane has none left).  The keys of a set differ in their chunk bits, so the order of the
-      // insertions does not change the set.
+      // A chunk can only enter its set if its key is below the set's largest, which never grows: bracket_bound turns
+      // that largest key, once per half, into an integer bound on the bracket minimum, so a chunk costs one compare
+      // and its key is only formed if it passes.  The chunks that pass are inserted in warp-uniform rounds, one per set
+      // and lane per round (FLT_MAX, a no-op of the network, where a lane has none left); a key that passed the bound
+      // but is not below the set's largest is a no-op too.  The keys of a set differ in their chunk bits, so the order
+      // of the insertions does not change the set.
       auto reduce = [&](uint32_t t, uint32_t h, uint32_t s0) {
         const int32_t* nrm = (const int32_t*)(smem_raw + (n_base + s0 * kNormBytes - smem_u32(smem_raw))) + h * 128u + 8u * q;
         const uint32_t chunk0 = t * (kTileN / kChunk) + h * (kTileN / 2 / kChunk) + q;
-        float x0[4], x1[4];
-        uint32_t p0 = 0, p1 = 0;  // bit g: x0[g] / x1[g] is still to be inserted
+        const int32_t b0 = bracket_bound(key0[kNumKeys - 1], keep_mask, qn0);
+        const int32_t b1 = bracket_bound(key1[kNumKeys - 1], keep_mask, qn1);
+        int32_t m0[4], m1[4];
+        uint32_t p0 = 0, p1 = 0;  // bit g: m0[g] / m1[g] is still to be inserted
 #pragma unroll
         for (uint32_t g = 0; g < 4; ++g) {
           const int4 na = *(const int4*)(nrm + kGroupRows * g);
@@ -234,26 +258,25 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
                                  nb.x - 2 * a[8], nb.y - 2 * a[9], nb.z - 2 * a[12], nb.w - 2 * a[13]};
           const int32_t d1[8] = {na.x - 2 * a[2], na.y - 2 * a[3], na.z - 2 * a[6], na.w - 2 * a[7],
                                  nb.x - 2 * a[10], nb.y - 2 * a[11], nb.z - 2 * a[14], nb.w - 2 * a[15]};
-          const uint32_t cid = chunk0 + 4 * g;
-          // exact: real distances are < 2^24
-          const float m0 = (float)(min8(d0) + qn0);
-          const float m1 = (float)(min8(d1) + qn1);
-          x0[g] = __uint_as_float((__float_as_uint(m0) & keep_mask) | cid);
-          x1[g] = __uint_as_float((__float_as_uint(m1) & keep_mask) | cid);
-          p0 |= (x0[g] < key0[kNumKeys - 1] ? 1u : 0u) << g;
-          p1 |= (x1[g] < key1[kNumKeys - 1] ? 1u : 0u) << g;
+          m0[g] = min8(d0);
+          m1[g] = min8(d1);
+          p0 |= (m0[g] <= b0 ? 1u : 0u) << g;
+          p1 |= (m1[g] <= b1 ? 1u : 0u) << g;
         }
         while (__any_sync(0xffffffffu, (p0 | p1) != 0u)) {
-          float y0 = __uint_as_float(kKeySentinel), y1 = y0;
+          int32_t y0 = 0, y1 = 0;
+          uint32_t g0 = 0, g1 = 0;
 #pragma unroll
-          for (int g = 3; g >= 0; --g) {  // the lowest pending candidate of each set
-            if (p0 & (1u << g)) y0 = x0[g];
-            if (p1 & (1u << g)) y1 = x1[g];
+          for (int g = 3; g >= 0; --g) {  // the lowest pending chunk of each set
+            if (p0 & (1u << g)) { y0 = m0[g]; g0 = g; }
+            if (p1 & (1u << g)) { y1 = m1[g]; g1 = g; }
           }
+          const float x0 = p0 != 0u ? chunk_key(y0, qn0, chunk0 + 4 * g0, keep_mask) : __uint_as_float(kKeySentinel);
+          const float x1 = p1 != 0u ? chunk_key(y1, qn1, chunk0 + 4 * g1, keep_mask) : __uint_as_float(kKeySentinel);
           p0 &= p0 - 1u;
           p1 &= p1 - 1u;
-          key_insert_packed(y0, key0);
-          key_insert_packed(y1, key1);
+          key_insert_packed(x0, key0);
+          key_insert_packed(x1, key1);
         }
       };
       // One accumulator: the MMAs of a half, then its epilogue.  The MMAs of the other consumers fill the tensor pipe
@@ -261,7 +284,8 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       mbar_wait(bar_qfull + 8 * qb, qf);
       for (uint32_t t = 0; t < ntiles; ++t) {
         const uint32_t s_t = stage;
-        for (uint32_t kb = 0; kb < nkb; ++kb) {
+#pragma unroll
+        for (uint32_t kb = 0; kb < kNkb; ++kb) {
           mbar_wait(bar_full + 8 * stage, phase);
           if (++stage == n_stages) { stage = 0; phase ^= 1u; }
         }
@@ -277,7 +301,8 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
         // the epilogue has read the tile's norms and the MMAs its operands: hand its stages back to the producer
         __syncwarp();
         if (lane == 0)
-          for (uint32_t kb = 0, s = s_t; kb < nkb; ++kb) {
+#pragma unroll
+          for (uint32_t kb = 0, s = s_t; kb < kNkb; ++kb) {
             mbar_arrive(bar_empty + 8 * s);
             if (++s == n_stages) s = 0;
           }
@@ -371,7 +396,13 @@ int launch_l2_candidates(r3d_ctx* ctx, DeviceWorker& w, const PairDesc* d_pairs,
   const int n_qbuf = ring_stages(q_bytes, 2, stage_bytes) >= min_stages ? 2 : 1;
   const int stages = ring_stages(q_bytes, n_qbuf, stage_bytes);
   const size_t smem = 1024 + (size_t)n_qbuf * q_bytes + (size_t)stages * stage_bytes + 8 * (2 * kMaxStages + 4);
-  auto kern = u8 ? k_l2_candidates<true, kConsumersU8> : k_l2_candidates<false, kConsumersF16>;
+  using Kernel = decltype(&k_l2_candidates<false, kConsumersF16, 0>);
+  // u8: the K extent is a template parameter, so each consumer issues its k32 steps back to back without a branch
+  static const Kernel kU8Kernels[8] = {
+      k_l2_candidates<true, kConsumersU8, 1>, k_l2_candidates<true, kConsumersU8, 2>, k_l2_candidates<true, kConsumersU8, 3>,
+      k_l2_candidates<true, kConsumersU8, 4>, k_l2_candidates<true, kConsumersU8, 5>, k_l2_candidates<true, kConsumersU8, 6>,
+      k_l2_candidates<true, kConsumersU8, 7>, k_l2_candidates<true, kConsumersU8, 8>};
+  const Kernel kern = u8 ? kU8Kernels[ksteps - 1] : k_l2_candidates<false, kConsumersF16, 0>;
   R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   const uint32_t grid = n_items < (uint32_t)w.sm_count ? n_items : (uint32_t)w.sm_count;
   kern<<<grid, 128 * (consumers + 1), smem, w.stream>>>((const CUtensorMap*)w.d_tmapQ, (const CUtensorMap*)w.d_tmapD, d_pairs, d_items,
