@@ -318,6 +318,60 @@ typedef struct {
 } r3d_relpose_timing;
 int r3d_get_relpose_timing(const r3d_ctx* ctx, r3d_relpose_timing* out);
 
+/* ---- resection: the absolute pose of views from 2D-3D correspondences (incremental SfM's first step) ----------- */
+#define R3D_RESECT_OK 0
+#define R3D_RESECT_TOO_FEW 1         /* <= 3 correspondences */
+#define R3D_RESECT_NO_INTRINSIC 2    /* focal <= 0 (upstream falls back to a 6-point DLT there; not implemented) */
+#define R3D_RESECT_NO_MODEL 3        /* AC-RANSAC: minNFA >= 0 or <= 2.5 * 3 inliers */
+typedef struct {
+  double precision_px;       /* +inf: SfM_Localizer's error_max = infinity (pure a-contrario); finite: the upper bound */
+  uint32_t max_iter;         /* 4096 */
+  int refine;                /* 1: SfM_Localizer::RefinePose(b_refine_pose = true, b_refine_intrinsic = false) */
+  r3d_ba_options ba;         /* the refinement's trust region and Huber loss; refine_intrinsics must be 0 */
+} r3d_resection_options;
+void r3d_resection_default_options(r3d_resection_options* o);  /* +inf, 4096, 1, r3d_ba_default_options with intrinsics fixed */
+typedef struct {
+  uint32_t view_id, width, height;
+  r3d_sfm_intrinsic intrinsic;       /* any R3D_CAM_* model; focal <= 0: no pinhole intrinsic */
+  uint64_t first, count;             /* the view's correspondences in X / x */
+} r3d_resection_view;
+typedef struct {
+  uint32_t view_id;
+  int status;                        /* R3D_RESECT_* */
+  uint32_t n_inliers;
+  double found_residual_precision;   /* AC-RANSAC errorMax, px */
+  double rotation[9], center[3], translation[3];     /* X_cam = R X + t, C = -R^T t; refined when refine is set and
+                                                      * the solve did not fail, else the AC-RANSAC pose */
+  double rotation_ransac[9], translation_ransac[3];  /* the AC-RANSAC model */
+  uint32_t lm_iterations, lm_successful_steps;
+  int lm_termination;                /* as r3d_ba_summary.termination; -1: not refined */
+  double lm_initial_cost, lm_final_cost;
+} r3d_resection;
+/* Replaces SfM_Localizer::Localize + SfM_Localizer::RefinePose (OpenMVG 1.4 sfm_localizer.cpp; the resection step of
+ * both incremental engines, src/threads/R3DTriangulationThread.cpp:416-512) for a batch of views.  Per view: the pixels
+ * undistorted once by the inverse of its camera model, AC-RANSAC with the a-contrario adaptor for resection with known K
+ * (P3P on bearing vectors, up to 4 models per sample, squared pixel reprojection error of P = K [R | t], point-to-point
+ * model log10(pi / (w h))), then Levenberg-Marquardt on the six pose parameters over the inliers, residuals on the
+ * original pixels through the full camera model, HuberLoss(ba.huber_a), structure and intrinsics held.
+ * X: 3 doubles per correspondence, x: 2 (pixels).  inliers (may be NULL; capacity: every view's count): per view its
+ * AC-RANSAC inliers as indices into its correspondences, in residual order; inlier_ofs (n_views + 1; required with
+ * inliers, else may be NULL).  Non-finite X or x, an unknown camera model, a view without a size or
+ * ba.refine_intrinsics != 0: R3D_ERR_INVALID before anything runs.  Views are spread over the context's devices. */
+int r3d_resect_views(r3d_ctx* ctx, const r3d_resection_view* views, uint32_t n_views, const double* X, const double* x,
+                     const r3d_resection_options* opt, r3d_resection* out, uint32_t* inliers, uint64_t* inlier_ofs);
+/* The same on an SfM_Data: the correspondences of a view are the landmarks of sd.structure that hold an observation of
+ * it (X from the landmark, x from the observation, landmark-id order).  view_ids / n: the views to resect; n = 0: every
+ * view without a pose.  out: one entry per resected view (capacity n, or the number of views without a pose), in
+ * view_ids order (n = 0: view-id order); *n_out (may be NULL) their number.  Every OK view gets a Pose3 (R, C) under its
+ * id_pose; nothing else changes.  A view that already has a pose, an unknown view or intrinsic id: R3D_ERR_INVALID. */
+int r3d_sfm_resect_views(r3d_ctx* ctx, r3d_sfm_data* sd, const uint32_t* view_ids, uint32_t n,
+                         const r3d_resection_options* opt, r3d_resection* out, uint32_t* n_out);
+typedef struct {
+  double ms_ransac, ms_refine, ms_device_total, ms_host;  /* last r3d_resect_views call; ms_ransac includes the point kernel */
+  uint64_t kernel_launches, lm_iterations;
+} r3d_resection_timing;
+int r3d_get_resection_timing(const r3d_ctx* ctx, r3d_resection_timing* out);
+
 /* ---- global rotations from the relative motions (global SfM, second step) ------------------------------------- */
 #define R3D_ROTAVG_L2 0              /* ROTATION_AVERAGING_L2 (src/threads/R3DTriangulationThread.cpp:201) */
 #define R3D_ROTAVG_L1 1              /* ROTATION_AVERAGING_L1: not implemented, R3D_ERR_UNSUPPORTED */

@@ -35,6 +35,7 @@ EXPORTS = [
     "r3d_tracks_build", "r3d_tracks_count", "r3d_tracks_get", "r3d_tracks_in_images", "r3d_tracks_free",
     "r3d_sfm_structure_from_tracks", "r3d_sfm_remove_outliers", "r3d_cascade_prepare", "r3d_debug_cascade_view",
     "r3d_relpose_default_options", "r3d_relative_poses", "r3d_get_relpose_timing",
+    "r3d_resection_default_options", "r3d_resect_views", "r3d_sfm_resect_views", "r3d_get_resection_timing",
     "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_matches_keep_largest_biedge_component",
     "r3d_transavg_default_options", "r3d_translation_averaging", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
 ]
@@ -236,6 +237,9 @@ def lib():
         L.r3d_save_matches.argtypes = [C.c_void_p, C.c_char_p]
         L.r3d_save_matches_bin.argtypes = [C.c_void_p, C.c_char_p]
         L.r3d_comm_world.argtypes = [C.c_void_p]
+        L.r3d_resect_views.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p]
+        L.r3d_sfm_resect_views.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.r3d_debug_post_process.restype = C.c_int64
         L.r3d_debug_post_process_ranked.restype = C.c_int64
         _lib = L
@@ -388,6 +392,50 @@ class SfmObservation(C.Structure):
 
 SFM_VIEWS, SFM_EXTRINSICS, SFM_INTRINSICS, SFM_STRUCTURE, SFM_CONTROL_POINTS, SFM_ALL = 1, 2, 4, 8, 16, 31
 CAM_PINHOLE, CAM_RADIAL1, CAM_RADIAL3, CAM_BROWN, CAM_FISHEYE = 1, 2, 3, 4, 5
+
+
+class ResectionOptions(C.Structure):
+    _fields_ = [("precision_px", C.c_double), ("max_iter", C.c_uint32), ("refine", C.c_int), ("ba", BAOptions)]
+
+
+class ResectionView(C.Structure):
+    _fields_ = [("view_id", C.c_uint32), ("width", C.c_uint32), ("height", C.c_uint32), ("intrinsic", SfmIntrinsic),
+                ("first", C.c_uint64), ("count", C.c_uint64)]
+
+
+class ResectionTiming(C.Structure):
+    _fields_ = [("ms_ransac", C.c_double), ("ms_refine", C.c_double), ("ms_device_total", C.c_double), ("ms_host", C.c_double),
+                ("kernel_launches", C.c_uint64), ("lm_iterations", C.c_uint64)]
+
+
+RESECT_OK, RESECT_TOO_FEW, RESECT_NO_INTRINSIC, RESECT_NO_MODEL = 0, 1, 2, 3
+resection_dtype = np.dtype([
+    ("view_id", np.uint32), ("status", np.int32), ("n_inliers", np.uint32), ("found_residual_precision", np.float64),
+    ("rotation", np.float64, (3, 3)), ("center", np.float64, 3), ("translation", np.float64, 3),
+    ("rotation_ransac", np.float64, (3, 3)), ("translation_ransac", np.float64, 3), ("lm_iterations", np.uint32),
+    ("lm_successful_steps", np.uint32), ("lm_termination", np.int32), ("lm_initial_cost", np.float64),
+    ("lm_final_cost", np.float64)], align=True)
+
+
+def resection_views(counts, widths, heights, models, focals, ppxs, ppys, distos=None, view_ids=None):
+    """r3d_resection_view array for views whose correspondences lie one after the other in X / x."""
+    n = len(counts)
+    arr = (ResectionView * n)()
+    first = 0
+    for v in range(n):
+        a = arr[v]
+        a.view_id = int(view_ids[v]) if view_ids is not None else v
+        a.width, a.height = int(widths[v]), int(heights[v])
+        a.intrinsic.id = v
+        a.intrinsic.model = int(models[v])
+        a.intrinsic.width, a.intrinsic.height = int(widths[v]), int(heights[v])
+        a.intrinsic.focal, a.intrinsic.ppx, a.intrinsic.ppy = float(focals[v]), float(ppxs[v]), float(ppys[v])
+        if distos is not None:
+            for i, d in enumerate(distos[v]):
+                a.intrinsic.disto[i] = float(d)
+        a.first, a.count = first, int(counts[v])
+        first += int(counts[v])
+    return arr
 
 
 class SfmData:
@@ -738,6 +786,49 @@ class Context:
         self._check(lib().r3d_relative_poses(self._h, matches.handle, views, C.c_uint32(len(widths)), C.byref(o), _p(out),
                                              C.byref(h)))
         return out[:matches.num_pairs].copy(), Matches(h)
+
+    @staticmethod
+    def _resection_options(precision_px, max_iter, refine, ba):
+        o = ResectionOptions()
+        lib().r3d_resection_default_options(C.byref(o))
+        o.precision_px = precision_px
+        o.max_iter = max_iter
+        o.refine = int(refine)
+        for k, v in ba.items():
+            setattr(o.ba, k, v)
+        return o
+
+    def resect_views(self, views, X, x, precision_px=float("inf"), max_iter=4096, refine=True, **ba):
+        """r3d_resect_views: absolute pose of every view of `views` (a ResectionView array, e.g. from resection_views)
+        from its 2D-3D correspondences X (n x 3), x (n x 2, pixels).  ba: r3d_ba_options fields of the pose refinement.
+        Returns (numpy array of resection_dtype, inlier offsets [n_views + 1], inlier indices into each view's
+        correspondences, in AC-RANSAC's residual order)."""
+        X = np.ascontiguousarray(X, np.float64).reshape(-1, 3)
+        x = np.ascontiguousarray(x, np.float64).reshape(-1, 2)
+        n = len(views)
+        o = self._resection_options(precision_px, max_iter, refine, ba)
+        out = np.zeros(max(n, 1), resection_dtype)
+        inl = np.zeros(max(len(x), 1), np.uint32)
+        ofs = np.zeros(n + 1, np.uint64)
+        self._check(lib().r3d_resect_views(self._h, views, C.c_uint32(n), _p(X), _p(x), C.byref(o), _p(out), _p(inl), _p(ofs)))
+        return out[:n].copy(), ofs, inl[:int(ofs[n])].copy()
+
+    def sfm_resect_views(self, sd, view_ids=None, precision_px=float("inf"), max_iter=4096, refine=True, **ba):
+        """r3d_sfm_resect_views: resect the listed views of the SfmData (None: every view without a pose) against its
+        structure and store the poses of the OK ones.  Returns a numpy array of resection_dtype."""
+        o = self._resection_options(precision_px, max_iter, refine, ba)
+        ids = np.ascontiguousarray([] if view_ids is None else view_ids, np.uint32)
+        cap = len(ids) if len(ids) else lib().r3d_sfm_num_views(sd.h)
+        out = np.zeros(max(cap, 1), resection_dtype)
+        n_out = C.c_uint32(0)
+        self._check(lib().r3d_sfm_resect_views(self._h, sd.h, _p(ids) if len(ids) else None, C.c_uint32(len(ids)), C.byref(o),
+                                               _p(out), C.byref(n_out)))
+        return out[:n_out.value].copy()
+
+    def resection_timing(self):
+        t = ResectionTiming()
+        self._check(lib().r3d_get_resection_timing(self._h, C.byref(t)))
+        return {k: getattr(t, k) for k, _ in ResectionTiming._fields_}
 
     def rotation_averaging(self, rel, n_views, refine=True, max_angular_error_deg=5.0, method=ROTAVG_L2, **lm):
         """r3d_rotation_averaging on the OK entries of `rel` (relpose_dtype, e.g. from relative_poses).  lm: r3d_ba_options

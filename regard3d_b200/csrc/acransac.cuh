@@ -12,12 +12,20 @@ struct AcPair {          // per image pair (device)
   double max_thr;        // precision^2 * N2(0,0)^2
   double logalpha0;      // F: log10(2 D / A / N2(0,0)) ; H: log10(pi / (w h) / N2(0,0)^2), image J
   double loge0;          // log10(MAX_MODELS * (M - MINIMUM_SAMPLES))
-  double K[6];           // essential model only: f, ppx, ppy of image I, then of image J (pinhole K)
+  double K[6];           // essential model: f, ppx, ppy of image I, then of image J (pinhole K)
+                         // resection model: f, ppx, ppy of the view, then K[3] = the squared residual the tier-1
+                         // histogram's top bin starts at (the precision may be infinite there)
 };
 
-// internal model ids: 0 = F (7-point), 1 = H (4-point), 2 = E (5-point); Kernel::MINIMUM_SAMPLES / MAX_MODELS
-__host__ __device__ constexpr uint32_t ac_min_samples(int model) { return model == 0 ? 7u : (model == 1 ? 4u : 5u); }
-__host__ __device__ constexpr uint32_t ac_max_models(int model) { return model == 0 ? 3u : (model == 1 ? 1u : 10u); }
+// internal model ids: 0 = F (7-point), 1 = H (4-point), 2 = E (5-point), 3 = resection with known K (P3P: x1 holds
+// X.xy, x3 holds X.z, x2 the undistorted pixel; the model is P = K [R | t], 3 x 4); Kernel::MINIMUM_SAMPLES / MAX_MODELS
+__host__ __device__ constexpr uint32_t ac_min_samples(int model) {
+  return model == 0 ? 7u : (model == 1 ? 4u : (model == 2 ? 5u : 3u));
+}
+__host__ __device__ constexpr uint32_t ac_max_models(int model) {
+  return model == 0 ? 3u : (model == 1 ? 1u : (model == 2 ? 10u : 4u));
+}
+__host__ __device__ constexpr uint32_t ac_model_size(int model) { return model == 3 ? 12u : 9u; }  // doubles per model
 
 struct AcPointSrc {      // per pair: where its matched positions come from and how they are normalised
   const float2* xyI;     // positions of view I / J on the device (uploaded with the regions)
@@ -57,14 +65,16 @@ struct AcFusedOut {      // per pair, written by the persistent kernel (acransac
 };
 
 // persistent one-CTA-per-pair ACRANSAC (acransac_fused.cu); `order`: pair ids of one size class, largest first;
-// huge: sort buffers / pool in global scratch (cap entries per CTA of the grid); out_model (may be null): 9 doubles per
-// pair id, the best model of every pair with inliers (F = K2^-T E K1^-1 for the essential model)
+// huge: sort buffers / pool in global scratch (cap entries per CTA of the grid); out_model (may be null):
+// ac_model_size(model) doubles per pair id, the best model of every pair with inliers (F = K2^-T E K1^-1 for the
+// essential model); x3: the resection model's third point coordinate, null for the others
 size_t acransac_fused_smem_bytes(int model, uint32_t cap, bool huge);
 int acransac_fused_ctas_per_sm(int model, uint32_t cap, bool huge);
 int launch_acransac_fused(r3d_ctx* ctx, DeviceWorker& w, int model, bool huge, const AcPair* pairs, const uint32_t* order,
                           uint32_t n_order, uint32_t* work_counter, const double2* x1, const double2* x2, const float* logc_n,
                           const float* logc_k, uint32_t cap, uint32_t max_iter, double* g_se, uint32_t* g_si, uint32_t* g_pool,
-                          const uint2* matches, uint2* out_matches, AcFusedOut* out, double* out_model, uint32_t grid);
+                          const uint2* matches, uint2* out_matches, AcFusedOut* out, double* out_model, uint32_t grid,
+                          const double* x3 = nullptr);
 
 struct AcBestModel {      // per pair of the putative map (r3d_relative_poses): the kept pair's best model, errorMax
   double model[9];       // row-major; F = K2^-T E K1^-1 for the essential model

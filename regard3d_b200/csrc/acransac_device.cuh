@@ -263,6 +263,16 @@ __device__ __forceinline__ double asym_error(const double* H, double x1x, double
   return ex * ex + ey * ey;
 }
 
+// resection::kernel::PoseResectionKernel / SquaredPixelReprojectionError: |x - (P X)_xy / (P X)_w|^2, P 3 x 4 row-major
+__device__ __forceinline__ double resect_error(const double* P, double X, double Y, double Z, double x, double y) {
+  const double px = P[0] * X + P[1] * Y + P[2] * Z + P[3];
+  const double py = P[4] * X + P[5] * Y + P[6] * Z + P[7];
+  const double pw = P[8] * X + P[9] * Y + P[10] * Z + P[11];
+  const double ex = x - px / pw;
+  const double ey = y - py / pw;
+  return ex * ex + ey * ey;
+}
+
 __device__ __forceinline__ bool key_less(double ea, uint32_t ia, double eb, uint32_t ib) {
   return (ea < eb) || (ea == eb && ia < ib);
 }
@@ -273,7 +283,8 @@ __device__ __forceinline__ bool key_less(double ea, uint32_t ia, double eb, uint
 // ties are indistinguishable there -- which halves the shared-memory traffic of the bitonic network.
 template <int MODEL, bool WITH_INDEX>
 __device__ uint32_t residuals_sorted(const AcPair& pr, const double2* __restrict__ x1, const double2* __restrict__ x2,
-                                     const double* Fm, double* se, uint32_t* si, uint32_t cap, uint32_t* s_count) {
+                                     const double* Fm, double* se, uint32_t* si, uint32_t cap, uint32_t* s_count,
+                                     const double* __restrict__ x3 = nullptr) {
   if (threadIdx.x == 0) *s_count = 0;
   __syncthreads();
   for (uint32_t i = threadIdx.x; i < pr.M; i += blockDim.x) {
@@ -281,7 +292,8 @@ __device__ uint32_t residuals_sorted(const AcPair& pr, const double2* __restrict
     const double2 b = x2[pr.pt_ofs + i];
     const double e = MODEL == 0   ? sym_epi_error(Fm, a.x, a.y, b.x, b.y)
                      : MODEL == 1 ? asym_error(Fm, a.x, a.y, b.x, b.y)
-                                  : epi_dist_error(Fm, a.x, a.y, b.x, b.y);
+                     : MODEL == 2 ? epi_dist_error(Fm, a.x, a.y, b.x, b.y)
+                                  : resect_error(Fm, a.x, a.y, x3[pr.pt_ofs + i], b.x, b.y);
     if (e <= pr.max_thr) {  // false for NaN
       const uint32_t pos = atomicAdd(s_count, 1u);
       if (pos < cap) {
@@ -331,7 +343,7 @@ template <int MODEL>
 __device__ NfaBest nfa_scan_sorted(const AcPair& pr, const double* se, uint32_t c, const float* __restrict__ lcn,
                                    const float* __restrict__ logc_k, double* s_nfa, uint32_t* s_k) {
   constexpr uint32_t NS = ac_min_samples(MODEL);      // Kernel::MINIMUM_SAMPLES
-  const double mult_error = MODEL == 1 ? 1.0 : 0.5;   // point-to-point : point-to-line
+  const double mult_error = (MODEL == 1 || MODEL == 3) ? 1.0 : 0.5;   // point-to-point : point-to-line
   double best = DBL_MAX * 2.0;  // +inf
   uint32_t best_k = NS;
   for (uint32_t k = NS + 1 + threadIdx.x; k <= c; k += blockDim.x) {

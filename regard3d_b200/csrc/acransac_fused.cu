@@ -21,6 +21,7 @@
 // (nfa >= minNFA: "not better") is already certain.
 #include "acransac_device.cuh"
 #include "acransac_rng.cuh"
+#include "p3p.cuh"
 
 #include <random>
 #include <type_traits>
@@ -43,7 +44,7 @@ constexpr int kBinShift = 52 - 5;
 template <int MODEL>
 struct BatchBuf {                     // one speculative batch of RANSAC iterations
   Mt19937 snap;                       // generator state before the batch's first draw
-  double models[kBatch][ac_max_models(MODEL)][9];
+  double models[kBatch][ac_max_models(MODEL)][ac_model_size(MODEL)];
   double lb[kBatch][ac_max_models(MODEL)];
   uint32_t cnt[kBatch][ac_max_models(MODEL)];      // residuals that may be <= the bound (upper count)
   uint32_t cnt_lo[kBatch][ac_max_models(MODEL)];   // residuals that certainly are (lower count)
@@ -58,7 +59,7 @@ struct FusedSmem {                    // fixed part of the shared memory (the so
   Mt19937 rng;
   BatchBuf<MODEL> q[2];               // the batch being scored / replayed and the one warp 0 prepares meanwhile
   double la[kHistStride];             // logalpha of every bin's lower edge (at bin_slot(b))
-  double bestF[9];
+  double bestF[ac_model_size(MODEL)];
   double s_nfa[kFWarps];
   uint32_t s_k[kFWarps];
   uint32_t gcnt[2 * (kFWarps - 1)];   // per model of the tier-1 group: upper / lower count
@@ -67,16 +68,20 @@ struct FusedSmem {                    // fixed part of the shared memory (the so
 };
 
 template <int MODEL>
-__device__ __forceinline__ double model_error(const double* F, const double2 a, const double2 b) {
-  return MODEL == 0 ? sym_epi_error(F, a.x, a.y, b.x, b.y)
-                    : MODEL == 1 ? asym_error(F, a.x, a.y, b.x, b.y) : epi_dist_error(F, a.x, a.y, b.x, b.y);
+__device__ __forceinline__ double model_error(const double* F, const double2 a, const double2 b, double z) {
+  return MODEL == 0   ? sym_epi_error(F, a.x, a.y, b.x, b.y)
+         : MODEL == 1 ? asym_error(F, a.x, a.y, b.x, b.y)
+         : MODEL == 2 ? epi_dist_error(F, a.x, a.y, b.x, b.y)
+                      : resect_error(F, a.x, a.y, z, b.x, b.y);
 }
 
 // ---- tier-1 residuals: fused multiply-adds, one reciprocal instead of IEEE divisions ---------------------------
 // Tier 1 only BOUNDS the exact computation, so it need not reproduce the reference's rounding.  approx_bounds()
 // returns an interval [*lo, *hi] that contains the residual the tier-2 / CPU code computes (the same rational
 // function of the same inputs, rounded differently):
-//   * the cancelling term (x2^T F x1 for the epipolar errors, x2 - H x1 for the transfer error) carries an ABSOLUTE
+//   * the cancelling term (x2^T F x1 for the epipolar errors, x2 - H x1 for the transfer error, x - P X for the
+//     reprojection error of the resection model: the transfer error with one more column, z = the point's third
+//     coordinate) carries an ABSOLUTE
 //     error eta = 64 ulp x (largest model entry) x (2 R + 1)^2, R = the pair's largest |coordinate|: both evaluations
 //     stay within that of the exact value (<= 12 roundings of terms bounded by that magnitude);
 //   * everything else is cancellation-free: relative error <= kApproxRel (2^-53 per operation; the reciprocal is
@@ -92,13 +97,21 @@ __device__ __forceinline__ double rcp_fast(double x, bool* ok) {
 }
 
 template <int MODEL>
-__device__ __forceinline__ void approx_bounds(const double* F, double eta, const double2 a, const double2 b, double* lo, double* hi) {
+__device__ __forceinline__ void approx_bounds(const double* F, double eta, const double2 a, const double2 b, double z, double* lo,
+                                              double* hi) {
   bool ok = true;
   double l, h;
-  if (MODEL == 1) {  // asymmetric transfer error of a homography: |x2 - (H x1)_xy / (H x1)_w|^2
-    const double hx = __fma_rn(F[0], a.x, __fma_rn(F[1], a.y, F[2]));
-    const double hy = __fma_rn(F[3], a.x, __fma_rn(F[4], a.y, F[5]));
-    const double hw = __fma_rn(F[6], a.x, __fma_rn(F[7], a.y, F[8]));
+  if (MODEL == 1 || MODEL == 3) {  // asymmetric transfer error of a homography: |x2 - (H x1)_xy / (H x1)_w|^2
+    double hx, hy, hw;
+    if (MODEL == 3) {              // reprojection error: |x - (P X)_xy / (P X)_w|^2
+      hx = __fma_rn(F[0], a.x, __fma_rn(F[1], a.y, __fma_rn(F[2], z, F[3])));
+      hy = __fma_rn(F[4], a.x, __fma_rn(F[5], a.y, __fma_rn(F[6], z, F[7])));
+      hw = __fma_rn(F[8], a.x, __fma_rn(F[9], a.y, __fma_rn(F[10], z, F[11])));
+    } else {
+      hx = __fma_rn(F[0], a.x, __fma_rn(F[1], a.y, F[2]));
+      hy = __fma_rn(F[3], a.x, __fma_rn(F[4], a.y, F[5]));
+      hw = __fma_rn(F[6], a.x, __fma_rn(F[7], a.y, F[8]));
+    }
     const double iw = rcp_fast(hw, &ok);
     const double ex = fabs(__fma_rn(-hx, iw, b.x)), ey = fabs(__fma_rn(-hy, iw, b.y));
     // eta bounds the absolute error of hx, hy, hw; propagated through the quotient (|hw| >> eta or the point is flagged)
@@ -140,7 +153,10 @@ __device__ __forceinline__ void approx_bounds(const double* F, double eta, const
 }  // namespace
 
 size_t acransac_fused_smem_bytes(int model, uint32_t cap, bool huge) {
-  const size_t fixed = model == 0 ? sizeof(FusedSmem<0>) : (model == 1 ? sizeof(FusedSmem<1>) : sizeof(FusedSmem<2>));
+  const size_t fixed = model == 0   ? sizeof(FusedSmem<0>)
+                       : model == 1 ? sizeof(FusedSmem<1>)
+                       : model == 2 ? sizeof(FusedSmem<2>)
+                                    : sizeof(FusedSmem<3>);
   const size_t hist = (size_t)kFWarps * kBins * sizeof(uint32_t);
   const size_t sortb = huge ? 0 : (size_t)cap * 8;  // residual values; the index array of the inlier sort is global
   const size_t pool = huge ? 0 : (size_t)cap * 2;   // 16-bit pool entries
@@ -149,13 +165,13 @@ size_t acransac_fused_smem_bytes(int model, uint32_t cap, bool huge) {
 
 // exact count of the residuals <= the precision bound (the classic-RANSAC phase needs it exactly; tier 1 brackets it)
 template <int MODEL>
-__device__ uint32_t exact_count(const AcPair& pr, const double2* __restrict__ p1, const double2* __restrict__ p2, const double* Fm,
-                                uint32_t* s_count) {
+__device__ uint32_t exact_count(const AcPair& pr, const double2* __restrict__ p1, const double2* __restrict__ p2,
+                                const double* __restrict__ pz, const double* Fm, uint32_t* s_count) {
   if (threadIdx.x == 0) *s_count = 0;
   __syncthreads();
   uint32_t c = 0;
   for (uint32_t i = threadIdx.x; i < pr.M; i += blockDim.x)
-    if (model_error<MODEL>(Fm, p1[i], p2[i]) <= pr.max_thr) ++c;
+    if (model_error<MODEL>(Fm, p1[i], p2[i], MODEL == 3 ? pz[i] : 0.0) <= pr.max_thr) ++c;
   for (int o = 16; o >= 1; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
   if ((threadIdx.x & 31u) == 0 && c) atomicAdd(s_count, c);
   __syncthreads();
@@ -170,16 +186,16 @@ __device__ uint32_t exact_count(const AcPair& pr, const double2* __restrict__ p1
 // (rare) inlier sorts.  HUGE: values and pool too live in global scratch (g_se / g_pool) -- the slow-but-correct path
 // for pairs with more putative matches than shared memory can sort.
 template <int MODEL, bool HUGE>
-__global__ void __launch_bounds__(kFThreads, MODEL == 2 ? 1 : 2) k_acransac_fused(
+__global__ void __launch_bounds__(kFThreads, MODEL >= 2 ? 1 : 2) k_acransac_fused(
     const AcPair* __restrict__ pairs, const uint32_t* __restrict__ order, uint32_t n_order, uint32_t* __restrict__ work_counter,
     const double2* __restrict__ x1, const double2* __restrict__ x2, const float* __restrict__ logc_n,
     const float* __restrict__ logc_k, uint32_t cap, uint32_t max_iter, double* __restrict__ g_se, uint32_t* __restrict__ g_si,
     uint32_t* __restrict__ g_pool, const uint2* __restrict__ matches, uint2* __restrict__ out_matches,
-    AcFusedOut* __restrict__ out, double* __restrict__ out_model) {
+    AcFusedOut* __restrict__ out, double* __restrict__ out_model, const double* __restrict__ x3) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  constexpr uint32_t NS = ac_min_samples(MODEL), MAXM = ac_max_models(MODEL);
+  constexpr uint32_t NS = ac_min_samples(MODEL), MAXM = ac_max_models(MODEL), MS = ac_model_size(MODEL);
   typedef typename std::conditional<HUGE, uint32_t, uint16_t>::type PoolT;
-  const double mult_error = MODEL == 1 ? 1.0 : 0.5;
+  const double mult_error = (MODEL == 1 || MODEL == 3) ? 1.0 : 0.5;
   FusedSmem<MODEL>& S = *reinterpret_cast<FusedSmem<MODEL>*>(smem_raw);
   unsigned char* region = smem_raw + ((sizeof(FusedSmem<MODEL>) + 15) & ~(size_t)15);
   uint32_t* hist_all = reinterpret_cast<uint32_t*>(region);                 // tier 1: kFWarps x kBins
@@ -202,6 +218,7 @@ __global__ void __launch_bounds__(kFThreads, MODEL == 2 ? 1 : 2) k_acransac_fuse
     const float* lcn = logc_n + pr.tbl_ofs;
     const double2* p1 = x1 + pr.pt_ofs;
     const double2* p2 = x2 + pr.pt_ofs;
+    const double* pz = MODEL == 3 ? x3 + pr.pt_ofs : nullptr;
 
     // ---- per-pair set-up: sampling pool, generator, bin edges, coordinate bound --------------------------------
     double rmax = 0.0;
@@ -209,11 +226,14 @@ __global__ void __launch_bounds__(kFThreads, MODEL == 2 ? 1 : 2) k_acransac_fuse
       pool[i] = (PoolT)i;
       const double2 a = p1[i], b = p2[i];
       rmax = fmax(rmax, fmax(fmax(fabs(a.x), fabs(a.y)), fmax(fabs(b.x), fabs(b.y))));
+      if (MODEL == 3) rmax = fmax(rmax, fabs(pz[i]));
     }
     for (int o = 16; o >= 1; o >>= 1) rmax = fmax(rmax, __shfl_xor_sync(0xffffffffu, rmax, o));
     if (lane == 0) S.s_nfa[warp] = rmax;
-    // bin(e) = clamp((bits(e) >> kBinShift) - bin_base, 0, kBins - 1): the precision bound falls in the top bin
-    const long long thr_key = __double_as_longlong(pr.max_thr) >> kBinShift;
+    // bin(e) = clamp((bits(e) >> kBinShift) - bin_base, 0, kBins - 1): the precision bound falls in the top bin (the
+    // resection model's bound may be infinite: its top bin starts at pr.K[3]; larger residuals are clamped into it,
+    // whose lower edge still bounds them from below)
+    const long long thr_key = __double_as_longlong(MODEL == 3 ? fmin(pr.max_thr, pr.K[3]) : pr.max_thr) >> kBinShift;
     const long long bin_base = thr_key - (kBins - 1);
     for (uint32_t b = tid; b < (uint32_t)kBins; b += kFThreads) {
       const long long kb = bin_base + (long long)b;
@@ -259,9 +279,18 @@ __global__ void __launch_bounds__(kFThreads, MODEL == 2 ? 1 : 2) k_acransac_fuse
       }
       __syncwarp();
       if (lane < Bq) {
-        double models[9 * MAXM];
+        double models[MS * MAXM];
         int nm;
-        if (MODEL == 2) {
+        if (MODEL == 3) {
+          double Xs[9], xs[6];
+          for (int t = 0; t < 3; ++t) {
+            const uint32_t s = Q.sample[lane][t];
+            const double2 a = p1[s], b = p2[s];
+            Xs[3 * t] = a.x; Xs[3 * t + 1] = a.y; Xs[3 * t + 2] = pz[s];
+            xs[2 * t] = b.x; xs[2 * t + 1] = b.y;
+          }
+          nm = p3p::solve(pr.K, Xs, xs, models);
+        } else if (MODEL == 2) {
           double b1[15], b2[15], Es[90];
           for (int t = 0; t < 5; ++t) {
             const double2 a = p1[Q.sample[lane][t]];
@@ -283,7 +312,7 @@ __global__ void __launch_bounds__(kFThreads, MODEL == 2 ? 1 : 2) k_acransac_fuse
         }
         Q.nm[lane] = (uint32_t)nm;
         for (int mi = 0; mi < nm; ++mi)
-          for (int t = 0; t < 9; ++t) Q.models[lane][mi][t] = models[9 * mi + t];
+          for (int t = 0; t < (int)MS; ++t) Q.models[lane][mi][t] = models[MS * mi + t];
       }
       __syncwarp();
     };
@@ -335,18 +364,19 @@ __global__ void __launch_bounds__(kFThreads, MODEL == 2 ? 1 : 2) k_acransac_fuse
           for (uint32_t k = 0; k < gn; ++k) {
             const double* Fm = &Q.models[gb[k]][gm[k]][0];
             double fmax_abs = 0.0;
-            for (int t = 0; t < 9; ++t) fmax_abs = fmax(fmax_abs, fabs(Fm[t]));
+            for (int t = 0; t < (int)MS; ++t) fmax_abs = fmax(fmax_abs, fabs(Fm[t]));
             eta[k] = 7.2e-15 * fmax_abs * coord_span;            // 64 ulp x the largest term of x2^T F x1 (or H x1)
           }
           uint32_t c_hi[kGroup], c_lo[kGroup];
           for (uint32_t k = 0; k < kGroup; ++k) { c_hi[k] = 0; c_lo[k] = 0; }
           for (uint32_t i = ctid; i < M; i += kConsumers) {
             const double2 a = p1[i], b2 = p2[i];
+            const double z = MODEL == 3 ? pz[i] : 0.0;
 #pragma unroll
             for (uint32_t k = 0; k < kGroup; ++k) {
               if (k >= gn) break;
               double elo, ehi;
-              approx_bounds<MODEL>(&Q.models[gb[k]][gm[k]][0], eta[k], a, b2, &elo, &ehi);
+              approx_bounds<MODEL>(&Q.models[gb[k]][gm[k]][0], eta[k], a, b2, z, &elo, &ehi);
               if (elo <= pr.max_thr) {  // may be an inlier of the precision bound
                 long long bin = (__double_as_longlong(elo) >> kBinShift) - bin_base;
                 bin = bin < 0 ? 0 : (bin > kBins - 1 ? kBins - 1 : bin);
@@ -434,19 +464,19 @@ __global__ void __launch_bounds__(kFThreads, MODEL == 2 ? 1 : 2) k_acransac_fuse
         const uint32_t nm = Q.nm[it];
         for (uint32_t mi = 0; mi < nm; ++mi) {
           ++n_models;
-          double Fm[9];
+          double Fm[MS];
           if (!ac_mode) {  // classic-RANSAC phase: the exact number of residuals within the bound decides the switch
             uint32_t c = Q.cnt_lo[it][mi];
             if (c != Q.cnt[it][mi] && (double)c <= 2.5 * NS && (double)Q.cnt[it][mi] > 2.5 * NS) {
-              for (int t = 0; t < 9; ++t) Fm[t] = Q.models[it][mi][t];
-              c = exact_count<MODEL>(pr, p1, p2, Fm, &S.s_count);
+              for (int t = 0; t < (int)MS; ++t) Fm[t] = Q.models[it][mi][t];
+              c = exact_count<MODEL>(pr, p1, p2, pz, Fm, &S.s_count);
             }
             if ((double)c > 2.5 * NS) ac_mode = true;
           }
           if (ac_mode && Q.lb[it][mi] < minNFA) {  // the model may improve on the best one: exact NFA (tier 2)
             ++n_exact;
-            for (int t = 0; t < 9; ++t) Fm[t] = Q.models[it][mi][t];
-            const uint32_t c = residuals_sorted<MODEL, false>(pr, x1, x2, Fm, se, si, cap, &S.s_count);
+            for (int t = 0; t < (int)MS; ++t) Fm[t] = Q.models[it][mi][t];
+            const uint32_t c = residuals_sorted<MODEL, false>(pr, x1, x2, Fm, se, si, cap, &S.s_count, x3);
             const NfaBest r = nfa_scan_sorted<MODEL>(pr, se, c, lcn, logc_k, S.s_nfa, S.s_k);
             if (r.nfa < minNFA) {
               better = true;
@@ -454,7 +484,7 @@ __global__ void __launch_bounds__(kFThreads, MODEL == 2 ? 1 : 2) k_acransac_fuse
               errorMax = r.err;
               best_k = r.k;
               have_inliers = true;
-              if (tid < 9) S.bestF[tid] = Fm[tid];
+              if (tid < MS) S.bestF[tid] = Fm[tid];
             }
           }
         }
@@ -477,9 +507,9 @@ __global__ void __launch_bounds__(kFThreads, MODEL == 2 ? 1 : 2) k_acransac_fuse
       if (event) {
         ++n_events;
         __syncthreads();  // bestF
-        double Fm[9];
-        for (int t = 0; t < 9; ++t) Fm[t] = S.bestF[t];
-        const uint32_t c = residuals_sorted<MODEL, true>(pr, x1, x2, Fm, se, si, cap, &S.s_count);
+        double Fm[MS];
+        for (int t = 0; t < (int)MS; ++t) Fm[t] = S.bestF[t];
+        const uint32_t c = residuals_sorted<MODEL, true>(pr, x1, x2, Fm, se, si, cap, &S.s_count, x3);
         pool_size = best_k < c ? best_k : c;
         for (uint32_t i = tid; i < pool_size; i += kFThreads) pool[i] = (PoolT)si[i];
         if (nIterReserve) {
@@ -507,12 +537,12 @@ __global__ void __launch_bounds__(kFThreads, MODEL == 2 ? 1 : 2) k_acransac_fuse
     uint32_t n_out = 0;
     if (have_inliers && minNFA < 0) {
       __syncthreads();
-      double Fm[9];
-      for (int t = 0; t < 9; ++t) Fm[t] = S.bestF[t];
-      const uint32_t c = residuals_sorted<MODEL, true>(pr, x1, x2, Fm, se, si, cap, &S.s_count);
+      double Fm[MS];
+      for (int t = 0; t < (int)MS; ++t) Fm[t] = S.bestF[t];
+      const uint32_t c = residuals_sorted<MODEL, true>(pr, x1, x2, Fm, se, si, cap, &S.s_count, x3);
       n_out = best_k < c ? best_k : c;
       for (uint32_t i = tid; i < n_out; i += kFThreads) out_matches[pr.pt_ofs + i] = matches[pr.pt_ofs + si[i]];
-      if (out_model && tid < 9) out_model[9 * (size_t)pair_id + tid] = S.bestF[tid];  // the best model (r3d_relative_poses)
+      if (out_model && tid < MS) out_model[MS * (size_t)pair_id + tid] = S.bestF[tid];  // the best model (r3d_relative_poses, r3d_resect_views)
     }
     if (tid == 0) {
       AcFusedOut o;
@@ -533,12 +563,12 @@ template <int MODEL, bool HUGE>
 static int launch_fused_t(r3d_ctx* ctx, DeviceWorker& w, const AcPair* pairs, const uint32_t* order, uint32_t n_order,
                           uint32_t* work_counter, const double2* x1, const double2* x2, const float* logc_n, const float* logc_k,
                           uint32_t cap, uint32_t max_iter, double* g_se, uint32_t* g_si, uint32_t* g_pool, const uint2* matches,
-                          uint2* out_matches, AcFusedOut* out, double* out_model, uint32_t grid) {
+                          uint2* out_matches, AcFusedOut* out, double* out_model, uint32_t grid, const double* x3) {
   const size_t smem = acransac_fused_smem_bytes(MODEL, cap, HUGE);
   R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(k_acransac_fused<MODEL, HUGE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   k_acransac_fused<MODEL, HUGE><<<grid, kFThreads, smem, w.stream>>>(pairs, order, n_order, work_counter, x1, x2, logc_n, logc_k,
                                                                       cap, max_iter, g_se, g_si, g_pool, matches, out_matches, out,
-                                                                      out_model);
+                                                                      out_model, x3);
   R3D_CUDA_TRY(ctx, cudaGetLastError());
   return R3D_OK;
 }
@@ -548,21 +578,23 @@ int acransac_fused_ctas_per_sm(int model, uint32_t cap, bool huge) {
   const size_t per_sm = 227 * 1024;
   int n = (int)(per_sm / (smem + 1024));
   if (n < 1) n = 1;
-  const int by_regs = model == 2 ? 1 : 2;  // __launch_bounds__ of the kernel
+  const int by_regs = model >= 2 ? 1 : 2;  // __launch_bounds__ of the kernel
   return n < by_regs ? n : by_regs;
 }
 
 int launch_acransac_fused(r3d_ctx* ctx, DeviceWorker& w, int model, bool huge, const AcPair* pairs, const uint32_t* order,
                           uint32_t n_order, uint32_t* work_counter, const double2* x1, const double2* x2, const float* logc_n,
                           const float* logc_k, uint32_t cap, uint32_t max_iter, double* g_se, uint32_t* g_si, uint32_t* g_pool,
-                          const uint2* matches, uint2* out_matches, AcFusedOut* out, double* out_model, uint32_t grid) {
+                          const uint2* matches, uint2* out_matches, AcFusedOut* out, double* out_model, uint32_t grid,
+                          const double* x3) {
   if (!n_order) return R3D_OK;
+  if ((model == 3) != (x3 != nullptr)) return fail(ctx, R3D_ERR_INVALID, "launch_acransac_fused: x3 belongs to the resection model");
 #define R3D_FUSED_CASE(MD, HG)                                                                                          \
   if (model == MD && huge == HG)                                                                                        \
     return launch_fused_t<MD, HG>(ctx, w, pairs, order, n_order, work_counter, x1, x2, logc_n, logc_k, cap, max_iter, \
-                                  g_se, g_si, g_pool, matches, out_matches, out, out_model, grid);
+                                  g_se, g_si, g_pool, matches, out_matches, out, out_model, grid, x3);
   R3D_FUSED_CASE(0, false) R3D_FUSED_CASE(0, true) R3D_FUSED_CASE(1, false) R3D_FUSED_CASE(1, true)
-  R3D_FUSED_CASE(2, false) R3D_FUSED_CASE(2, true)
+  R3D_FUSED_CASE(2, false) R3D_FUSED_CASE(2, true) R3D_FUSED_CASE(3, false) R3D_FUSED_CASE(3, true)
 #undef R3D_FUSED_CASE
   return fail(ctx, R3D_ERR_INVALID, "launch_acransac_fused: unknown model");
 }

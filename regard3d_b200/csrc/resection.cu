@@ -1,0 +1,761 @@
+// resection.cu -- absolute pose of views from 2D-3D correspondences (r3d_resect_views, r3d_sfm_resect_views).
+// COMPILED WITH --fmad=false (regard3d_b200/build.py): the undistorted pixels, the P3P models and every AC-RANSAC
+// decision must equal the CPU restatement's (oracle/oracle_resection.cpp) bit for bit; the pose refinement follows its
+// LM decisions.
+//
+// Replaces SfM_Localizer::Localize + SfM_Localizer::RefinePose (OpenMVG 1.4 sfm_localizer.cpp), the first step of the
+// loop both incremental engines run (src/threads/R3DTriangulationThread.cpp:416-512).  Three stages per device, one
+// stream, one synchronisation:
+//   1. k_resect_points, one thread per correspondence: the pixel undistorted once by the inverse of the view's camera
+//      model (p3p.cuh), the structure point split into the layout the AC-RANSAC kernel reads;
+//   2. k_acransac_fused<3>: the filters' persistent one-CTA-per-problem AC-RANSAC with the P3P solver and the pinhole
+//      reprojection error (acransac_fused.cu), one launch per size class; it hands back P = K [R | t] of the best model;
+//   3. k_resect_refine, one persistent CTA per view: Levenberg-Marquardt on the six pose parameters over the AC-RANSAC
+//      inliers, residuals on the original pixels through the full camera model (ba_model.cuh), Huber loss, the trust
+//      region of the bundle adjustment.  The 6 x 6 normal equations are reduced in a fixed order (no floating-point
+//      atomics), so a call is reproducible.  FP64 throughout; bound by FP64 latency, not by tensor cores or HBM.
+#include "acransac.cuh"
+#include "acransac_rng.cuh"
+#include "ba_model.cuh"
+#include "detmath.cuh"
+#include "p3p.cuh"
+#include "r3d_sfm.h"
+
+#include <algorithm>
+#include <chrono>
+#include <cmath>
+#include <cstring>
+#include <limits>
+#include <thread>
+
+namespace r3d {
+
+namespace {
+
+double now_ms() {
+  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
+}
+
+struct RsView {            // a view that reached the AC-RANSAC stage (device)
+  uint32_t ofs, M;         // its correspondences in the device arrays
+  int model;               // R3D_CAM_*
+  int pad_;
+  double intr[6], ext[2];  // f, ppx, ppy, the model's first three distortion coefficients | coefficients 4, 5
+};
+
+struct RsLm {              // refinement result
+  double pose[6];          // angle-axis | t
+  uint32_t iterations, successful;
+  int termination;         // -1: not refined
+  int pad_;
+  double initial_cost, final_cost;
+};
+
+struct RsLmParams {
+  uint32_t max_iterations;
+  double huber_a, function_tolerance, gradient_tolerance, parameter_tolerance, initial_radius;
+};
+
+// [R | t] of P = K [R | t], K = [f 0 ppx; 0 f ppy; 0 0 1]
+__host__ __device__ inline void pose_from_projective(const double* K, const double* P, double* R, double* t) {
+  for (int j = 0; j < 3; ++j) {
+    R[6 + j] = P[8 + j];
+    R[j] = (P[j] - K[1] * P[8 + j]) / K[0];
+    R[3 + j] = (P[4 + j] - K[2] * P[8 + j]) / K[0];
+  }
+  t[2] = P[11];
+  t[0] = (P[3] - K[1] * P[11]) / K[0];
+  t[1] = (P[7] - K[2] * P[11]) / K[0];
+}
+
+// ceres::RotationMatrixToAngleAxis (through the quaternion), R row-major
+__host__ __device__ inline void rotation_to_angle_axis(const double* R, double* aa) {
+  double q[4];
+  const double trace = R[0] + R[4] + R[8];
+  if (trace >= 0.0) {
+    double t = sqrt(trace + 1.0);
+    q[0] = 0.5 * t;
+    t = 0.5 / t;
+    q[1] = (R[7] - R[5]) * t;
+    q[2] = (R[2] - R[6]) * t;
+    q[3] = (R[3] - R[1]) * t;
+  } else {
+    int i = 0;
+    if (R[4] > R[0]) i = 1;
+    if (R[8] > R[4 * i]) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    double t = sqrt(R[4 * i] - R[4 * j] - R[4 * k] + 1.0);
+    q[i + 1] = 0.5 * t;
+    t = 0.5 / t;
+    q[0] = (R[3 * k + j] - R[3 * j + k]) * t;
+    q[j + 1] = (R[3 * j + i] + R[3 * i + j]) * t;
+    q[k + 1] = (R[3 * k + i] + R[3 * i + k]) * t;
+  }
+  const double s2 = q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+  double k = 2.0;
+  if (s2 > 0.0) {
+    const double st = sqrt(s2), ct = q[0];
+    const double two_theta = 2.0 * (ct < 0.0 ? atan2(-st, -ct) : atan2(st, ct));
+    k = two_theta / st;
+  }
+  for (int i = 0; i < 3; ++i) aa[i] = q[i + 1] * k;
+}
+
+// ---- 1. undistortion and the AC-RANSAC point layout ------------------------------------------------------------------
+// grid (8, views): X (3 per correspondence) -> x1 = (X, Y), x3 = Z; x (2 per correspondence) -> x2 = undistorted pixel;
+// idm = (i, i): the kernel lists a problem's inliers by copying entries of this array
+__global__ void __launch_bounds__(256) k_resect_points(const RsView* __restrict__ views, const double* __restrict__ X,
+                                                       const double2* __restrict__ x, double2* __restrict__ x1,
+                                                       double* __restrict__ x3, double2* __restrict__ x2, uint2* __restrict__ idm) {
+  const RsView& v = views[blockIdx.y];
+  const double disto[5] = {v.intr[3], v.intr[4], v.intr[5], v.ext[0], v.ext[1]};
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < v.M; i += gridDim.x * blockDim.x) {
+    const size_t g = (size_t)v.ofs + i;
+    x1[g] = make_double2(X[3 * g], X[3 * g + 1]);
+    x3[g] = X[3 * g + 2];
+    const double2 o = x[g];
+    double ux, uy;
+    p3p::undistort_pixel(v.model, v.intr[0], v.intr[1], v.intr[2], disto, o.x, o.y, &ux, &uy);
+    x2[g] = make_double2(ux, uy);
+    idm[g] = make_uint2(i, i);
+  }
+}
+
+// ---- 3. pose-only Levenberg-Marquardt ------------------------------------------------------------------------------------
+constexpr int kRThreads = 256;
+constexpr int kRWarps = kRThreads / 32;
+constexpr int kREntries = 27;            // 21 lower-triangle entries of J^T J + 6 of J^T r
+
+struct RefineSmem {
+  double pose[6], pose_new[6], scale[6], g[6], diag[6], D2[6], delta[6];
+  double H[36];
+  double part[kRWarps][kREntries + 1];
+  double sums[kREntries + 1];
+  RsView view;
+  int pd;
+  uint32_t work;
+};
+
+// sums[e] = sum over the threads of v[e], e < n: a fixed shuffle tree per warp, then the warps in order
+__device__ void block_sums(const double* v, int n, RefineSmem& S) {
+  for (int e = 0; e < n; ++e) {
+    double a = v[e];
+    for (int o = 16; o >= 1; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+    if ((threadIdx.x & 31u) == 0) S.part[threadIdx.x >> 5][e] = a;
+  }
+  __syncthreads();
+  if ((int)threadIdx.x < n) {
+    double s = 0.0;
+    for (int w = 0; w < kRWarps; ++w) s += S.part[w][threadIdx.x];
+    S.sums[threadIdx.x] = s;
+  }
+  __syncthreads();
+}
+
+// one persistent CTA per view; order: view slots, most correspondences first.  The inliers of slot a are
+// inl[views[a].ofs + 0 .. fo[a].n_inliers) (indices into the view's correspondences, AC-RANSAC's residual order).
+__global__ void __launch_bounds__(kRThreads) k_resect_refine(const RsView* __restrict__ views, const uint32_t* __restrict__ order,
+                                                             uint32_t n_order, uint32_t* __restrict__ work_counter,
+                                                             const AcFusedOut* __restrict__ fo, const double* __restrict__ models,
+                                                             const uint2* __restrict__ inl, const double2* __restrict__ x1,
+                                                             const double* __restrict__ x3, const double2* __restrict__ xo,
+                                                             RsLm* __restrict__ out, RsLmParams prm) {
+  __shared__ RefineSmem S;
+  const uint32_t tid = threadIdx.x;
+  for (;;) {
+    __syncthreads();
+    if (tid == 0) S.work = atomicAdd(work_counter, 1u);
+    __syncthreads();
+    const uint32_t wk = S.work;
+    if (wk >= n_order) break;
+    const uint32_t a = order[wk];
+    const AcFusedOut f = fo[a];
+    if (!(f.minNFA < 0.0) || !((double)f.n_inliers > 2.5 * 3)) continue;  // no model: nothing to refine
+    if (tid == 0) {
+      S.view = views[a];
+      double R[9], t[3];
+      pose_from_projective(S.view.intr, models + 12 * (size_t)a, R, t);
+      rotation_to_angle_axis(R, S.pose);
+      for (int i = 0; i < 3; ++i) S.pose[3 + i] = t[i];
+    }
+    __syncthreads();
+    const uint32_t N = f.n_inliers;
+    const size_t base = S.view.ofs;
+    const int model = S.view.model;
+
+    auto total_cost = [&](const double* pose) -> double {
+      double c = 0.0;
+      for (uint32_t p = tid; p < N; p += kRThreads) {
+        const size_t g = base + inl[base + p].x;
+        const double2 xy = x1[g], ob = xo[g];
+        const double X[3] = {xy.x, xy.y, x3[g]};
+        double r[2], rho1;
+        ba::residual_only(model, S.view.intr, S.view.ext, pose, X, ob.x, ob.y, r);
+        c += 0.5 * ba::huber_rho(r[0] * r[0] + r[1] * r[1], prm.huber_a, &rho1);
+      }
+      block_sums(&c, 1, S);
+      return S.sums[0];
+    };
+    // Corrector-scaled residuals and pose Jacobians at S.pose: the Jacobi scale on the first call, then g = J^T r and
+    // H = J^T J of the scaled columns
+    auto evaluate = [&](bool first) {
+      if (first) {
+        double n2[6] = {0, 0, 0, 0, 0, 0};
+        for (uint32_t p = tid; p < N; p += kRThreads) {
+          const size_t g = base + inl[base + p].x;
+          const double2 xy = x1[g], ob = xo[g];
+          const double X[3] = {xy.x, xy.y, x3[g]};
+          double r[2], Ji[12], Jc[12], Jp[6], rho1;
+          ba::residual_jacobian(model, S.view.intr, S.view.ext, S.pose, X, ob.x, ob.y, r, Ji, Jc, Jp);
+          ba::huber_rho(r[0] * r[0] + r[1] * r[1], prm.huber_a, &rho1);
+          const double sq = sqrt(rho1);
+          for (int k = 0; k < 6; ++k) {
+            const double j0 = Jc[k] * sq, j1 = Jc[6 + k] * sq;
+            n2[k] += j0 * j0 + j1 * j1;
+          }
+        }
+        block_sums(n2, 6, S);
+        if (tid < 6) S.scale[tid] = 1.0 / (1.0 + sqrt(S.sums[tid]));
+        __syncthreads();
+      }
+      double acc[kREntries];
+      for (int e = 0; e < kREntries; ++e) acc[e] = 0.0;
+      for (uint32_t p = tid; p < N; p += kRThreads) {
+        const size_t g = base + inl[base + p].x;
+        const double2 xy = x1[g], ob = xo[g];
+        const double X[3] = {xy.x, xy.y, x3[g]};
+        double r[2], Ji[12], Jc[12], Jp[6], rho1;
+        ba::residual_jacobian(model, S.view.intr, S.view.ext, S.pose, X, ob.x, ob.y, r, Ji, Jc, Jp);
+        ba::huber_rho(r[0] * r[0] + r[1] * r[1], prm.huber_a, &rho1);
+        const double sq = sqrt(rho1);
+        const double r0 = r[0] * sq, r1 = r[1] * sq;
+        double j0[6], j1[6];
+        for (int k = 0; k < 6; ++k) {
+          j0[k] = Jc[k] * sq * S.scale[k];
+          j1[k] = Jc[6 + k] * sq * S.scale[k];
+        }
+        int e = 0;
+        for (int i = 0; i < 6; ++i)
+          for (int j = 0; j <= i; ++j) acc[e++] += j0[i] * j0[j] + j1[i] * j1[j];
+        for (int k = 0; k < 6; ++k) acc[21 + k] += j0[k] * r0 + j1[k] * r1;
+      }
+      block_sums(acc, kREntries, S);
+      if (tid == 0) {
+        int e = 0;
+        for (int i = 0; i < 6; ++i)
+          for (int j = 0; j <= i; ++j) S.H[6 * i + j] = S.sums[e++];
+        for (int k = 0; k < 6; ++k) { S.g[k] = S.sums[21 + k]; S.diag[k] = S.H[7 * k]; }
+      }
+      __syncthreads();
+    };
+    auto grad_max = [&]() -> double {
+      double m = 0.0;
+      for (int j = 0; j < 6; ++j) m = fmax(m, fabs(S.g[j] / S.scale[j]));
+      return m;
+    };
+
+    double cost = total_cost(S.pose);
+    const double initial_cost = cost;
+    uint32_t iterations = 0, successful = 0;
+    int termination = 0;
+    double radius = prm.initial_radius, decrease_factor = 2.0;
+    evaluate(true);
+    if (grad_max() <= prm.gradient_tolerance) termination = 2;
+    else
+      for (uint32_t iter = 1; iter <= prm.max_iterations; ++iter) {
+        iterations = iter;
+        __syncthreads();
+        if (tid == 0) {  // LevenbergMarquardtStrategy: (H + D^2) delta = -g, D^2 = clamp(diag, 1e-6, 1e32) / radius
+          double A[36], b[6];
+          for (int j = 0; j < 6; ++j) S.D2[j] = fmin(fmax(S.diag[j], 1e-6), 1e32) / radius;
+          for (int i = 0; i < 6; ++i) {
+            for (int j = 0; j <= i; ++j) A[6 * i + j] = S.H[6 * i + j] + (i == j ? S.D2[i] : 0.0);
+            b[i] = -S.g[i];
+          }
+          int pd = 1;
+          for (int j = 0; j < 6 && pd; ++j) {
+            double d = A[6 * j + j];
+            for (int t = 0; t < j; ++t) d -= A[6 * j + t] * A[6 * j + t];
+            if (!(d > 0.0)) { pd = 0; break; }
+            d = sqrt(d);
+            A[6 * j + j] = d;
+            for (int i = j + 1; i < 6; ++i) {
+              double s = A[6 * i + j];
+              for (int t = 0; t < j; ++t) s -= A[6 * i + t] * A[6 * j + t];
+              A[6 * i + j] = s / d;
+            }
+          }
+          if (pd) {
+            for (int i = 0; i < 6; ++i) {
+              double s = b[i];
+              for (int t = 0; t < i; ++t) s -= A[6 * i + t] * b[t];
+              b[i] = s / A[6 * i + i];
+            }
+            for (int i = 5; i >= 0; --i) {
+              double s = b[i];
+              for (int t = i + 1; t < 6; ++t) s -= A[6 * t + i] * b[t];
+              b[i] = s / A[6 * i + i];
+            }
+            for (int j = 0; j < 6; ++j) S.delta[j] = b[j];
+          }
+          S.pd = pd;
+        }
+        __syncthreads();
+        bool step_ok = S.pd != 0;
+        double model_cost_change = 0.0;
+        if (step_ok) {
+          double m = 0.0;
+          for (int j = 0; j < 6; ++j) m += S.delta[j] * (S.D2[j] * S.delta[j] - S.g[j]);
+          model_cost_change = 0.5 * m;
+          step_ok = model_cost_change > 0.0;
+        }
+        bool accepted = false;
+        if (step_ok) {
+          double dn = 0.0, xn = 0.0;
+          for (int j = 0; j < 6; ++j) {
+            const double d = S.delta[j] * S.scale[j];
+            dn += d * d;
+            xn += S.pose[j] * S.pose[j];
+          }
+          if (tid < 6) S.pose_new[tid] = S.pose[tid] + S.delta[tid] * S.scale[tid];
+          __syncthreads();
+          if (sqrt(dn) <= prm.parameter_tolerance * (sqrt(xn) + prm.parameter_tolerance)) {
+            termination = 3;
+            break;
+          }
+          const double new_cost = total_cost(S.pose_new);
+          const double relative_decrease = (cost - new_cost) / model_cost_change;
+          if (relative_decrease > 1e-3) {
+            accepted = true;
+            if (tid < 6) S.pose[tid] = S.pose_new[tid];
+            const double cost_change = cost - new_cost;
+            const double t = 2.0 * relative_decrease - 1.0;
+            radius = radius / fmax(1.0 / 3.0, 1.0 - t * t * t);
+            radius = fmin(1e16, radius);
+            decrease_factor = 2.0;
+            ++successful;
+            const bool ftol = fabs(cost_change) < prm.function_tolerance * cost;
+            cost = new_cost;
+            __syncthreads();
+            evaluate(false);
+            if (ftol) { termination = 1; break; }
+            if (grad_max() <= prm.gradient_tolerance) { termination = 2; break; }
+          }
+        }
+        if (!accepted) {
+          radius = radius / decrease_factor;
+          decrease_factor *= 2.0;
+          if (radius < 1e-32) { termination = 4; break; }
+        }
+      }
+    __syncthreads();
+    if (tid == 0) {
+      RsLm o;
+      for (int k = 0; k < 6; ++k) o.pose[k] = S.pose[k];
+      o.iterations = iterations;
+      o.successful = successful;
+      o.termination = termination;
+      o.pad_ = 0;
+      o.initial_cost = initial_cost;
+      o.final_cost = cost;
+      out[a] = o;
+    }
+  }
+}
+
+template <typename T>
+struct DevArr {  // device scratch out of the worker's pool (context.cu)
+  DeviceWorker* w;
+  T* p = nullptr;
+  explicit DevArr(DeviceWorker& worker) : w(&worker) {}
+  DevArr(const DevArr&) = delete;
+  DevArr& operator=(const DevArr&) = delete;
+  ~DevArr() { if (p) pool_release(*w, p); }
+  bool alloc(size_t n) {
+    p = (T*)pool_alloc(*w, std::max<size_t>(n, 1) * sizeof(T));
+    return p != nullptr;
+  }
+};
+
+void angle_axis_to_rotation(const double* aa, double* R) { r3d_sfm::angle_axis_to_rotation(aa, R); }
+
+void set_pose(r3d_resection& o, const double* R, const double* t) {
+  std::memcpy(o.rotation, R, sizeof(o.rotation));
+  std::memcpy(o.translation, t, sizeof(o.translation));
+  for (int i = 0; i < 3; ++i) o.center[i] = -(R[i] * t[0] + R[3 + i] * t[1] + R[6 + i] * t[2]);  // C = -R^T t
+}
+
+// views [v0, v1) on worker w; inl[v]: the view's AC-RANSAC inliers (residual order)
+int resect_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_resection_view* views, uint32_t v0, uint32_t v1, const double* X,
+                 const double* x, const r3d_resection_options& opt, r3d_resection* out, std::vector<std::vector<uint32_t>>& inl,
+                 r3d_resection_timing& T) {
+  const double t0 = now_ms();
+  T = r3d_resection_timing{};
+  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
+  std::vector<uint32_t> cand;
+  for (uint32_t v = v0; v < v1; ++v) {
+    r3d_resection& o = out[v];
+    std::memset(&o, 0, sizeof(o));
+    o.view_id = views[v].view_id;
+    o.lm_termination = -1;
+    o.status = views[v].count <= 3 ? R3D_RESECT_TOO_FEW
+               : !(views[v].intrinsic.focal > 0.0) ? R3D_RESECT_NO_INTRINSIC
+                                                    : R3D_RESECT_NO_MODEL;
+    if (o.status == R3D_RESECT_NO_MODEL) cand.push_back(v);
+  }
+  if (cand.empty()) {
+    T.ms_host = now_ms() - t0;
+    return R3D_OK;
+  }
+  if (!rng_selftest())
+    return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: the device sample stream disagrees with this process's <random>");
+  const uint32_t n = (uint32_t)cand.size();
+  // ---- per view set-up: the a-contrario adaptor for resection with known K (point-to-point, pixel units) ----
+  std::vector<AcPair> hpairs(n);
+  std::vector<RsView> hviews(n);
+  uint64_t pt_total = 0, tbl_total = 0;
+  uint32_t maxM = 0;
+  for (uint32_t a = 0; a < n; ++a) {
+    const r3d_resection_view& v = views[cand[a]];
+    const uint32_t M = (uint32_t)v.count;
+    AcPair& ap = hpairs[a];
+    std::memset(&ap, 0, sizeof(ap));
+    ap.pt_ofs = (uint32_t)pt_total; ap.M = M; ap.tbl_ofs = (uint32_t)tbl_total;
+    ap.max_thr = opt.precision_px * opt.precision_px;  // upper_bound_precision = Square(error_max)
+    ap.logalpha0 = dm::log10_det(R3D_PI / ((double)v.width * (double)v.height));
+    ap.loge0 = dm::log10_det((double)ac_max_models(3) * (double)(M - ac_min_samples(3)));
+    ap.K[0] = v.intrinsic.focal; ap.K[1] = v.intrinsic.ppx; ap.K[2] = v.intrinsic.ppy;
+    ap.K[3] = (double)v.width * (double)v.width + (double)v.height * (double)v.height;
+    RsView& rv = hviews[a];
+    std::memset(&rv, 0, sizeof(rv));
+    rv.ofs = ap.pt_ofs; rv.M = M; rv.model = v.intrinsic.model;
+    rv.intr[0] = v.intrinsic.focal; rv.intr[1] = v.intrinsic.ppx; rv.intr[2] = v.intrinsic.ppy;
+    for (int i = 0; i < 3; ++i) rv.intr[3 + i] = v.intrinsic.disto[i];
+    rv.ext[0] = v.intrinsic.disto[3]; rv.ext[1] = v.intrinsic.disto[4];
+    pt_total += M;
+    tbl_total += M + 2;
+    maxM = std::max(maxM, M);
+  }
+  if (pt_total > 0xfffffff0ull) return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: too many correspondences in one call");
+  std::vector<double> hX(3 * pt_total), hx(2 * pt_total);
+  parallel_for(ctx->host_threads, n, [&](size_t a) {
+    const r3d_resection_view& v = views[cand[a]];
+    std::memcpy(&hX[3 * (size_t)hpairs[a].pt_ofs], X + 3 * v.first, 3 * v.count * sizeof(double));
+    std::memcpy(&hx[2 * (size_t)hpairs[a].pt_ofs], x + 2 * v.first, 2 * v.count * sizeof(double));
+  });
+  std::vector<float> vlog10(maxM + 2);
+  for (uint32_t k = 0; k <= maxM + 1; ++k) vlog10[k] = std::log10((float)k);
+  std::vector<float> hlogc_k(maxM + 1, 0.f);  // makelogcombi_k: log10 C(n, 3) as the running float sum upstream builds
+  for (uint32_t m = 0; m <= maxM; ++m) {
+    uint32_t k = ac_min_samples(3);
+    if (k >= m) continue;
+    if (m - k < k) k = m - k;
+    float r = 0.f;
+    for (uint32_t i = 1; i <= k; ++i) r += vlog10[m - i + 1] - vlog10[i];
+    hlogc_k[m] = r;
+  }
+  // ---- size classes of the persistent kernel (shared-memory sort capacity 1024 ... 16384, beyond: global scratch) ----
+  constexpr int kClasses = 6;
+  std::vector<uint32_t> order[kClasses], horder;
+  uint32_t class_ofs[kClasses + 1] = {0}, caps[kClasses] = {0}, grids[kClasses] = {0}, huge_maxM = 0;
+  for (uint32_t a = 0; a < n; ++a) {
+    const uint32_t M = hpairs[a].M;
+    int c = 0;
+    while (c < 5 && (1024u << c) < M) ++c;
+    if (M > 16384u) { c = 5; huge_maxM = std::max(huge_maxM, M); }
+    order[c].push_back(a);
+  }
+  size_t si_need = 0, huge_need = 0;
+  for (int c = 0; c < kClasses; ++c) {
+    std::stable_sort(order[c].begin(), order[c].end(), [&](uint32_t p, uint32_t q) { return hpairs[p].M > hpairs[q].M; });
+    class_ofs[c] = (uint32_t)horder.size();
+    horder.insert(horder.end(), order[c].begin(), order[c].end());
+    const uint32_t cnt = (uint32_t)order[c].size();
+    if (!cnt) continue;
+    const bool huge = c == 5;
+    uint32_t cap = 1024u << c;
+    if (huge) {
+      cap = 32768;
+      while (cap < huge_maxM) cap <<= 1;
+    }
+    uint32_t grid = std::min<uint32_t>(cnt, (uint32_t)w.sm_count * (uint32_t)acransac_fused_ctas_per_sm(3, cap, huge));
+    if (huge) grid = std::min<uint32_t>(grid, (uint32_t)w.sm_count);
+    caps[c] = cap;
+    grids[c] = grid;
+    si_need = std::max(si_need, (size_t)grid * cap);
+    if (huge) huge_need = (size_t)grid * cap;
+  }
+  class_ofs[kClasses] = (uint32_t)horder.size();
+  std::vector<uint32_t> lm_order(n);  // refinement: most correspondences first
+  for (uint32_t a = 0; a < n; ++a) lm_order[a] = a;
+  std::stable_sort(lm_order.begin(), lm_order.end(), [&](uint32_t p, uint32_t q) { return hpairs[p].M > hpairs[q].M; });
+
+  DevArr<AcPair> d_pairs(w);
+  DevArr<RsView> d_views(w);
+  DevArr<double> d_X(w), d_x3(w), d_se(w), d_model(w);
+  DevArr<double2> d_xo(w), d_x1(w), d_x2(w);
+  DevArr<uint2> d_idm(w), d_outm(w);
+  DevArr<float> d_vlog10(w), d_logc_n(w), d_logc_k(w);
+  DevArr<uint32_t> d_order(w), d_lm_order(w), d_work(w), d_si(w), d_pool(w);
+  DevArr<AcFusedOut> d_out(w);
+  DevArr<RsLm> d_lm(w);
+  if (!d_pairs.alloc(n) || !d_views.alloc(n) || !d_X.alloc(3 * pt_total) || !d_x3.alloc(pt_total) || !d_xo.alloc(pt_total) ||
+      !d_x1.alloc(pt_total) || !d_x2.alloc(pt_total) || !d_idm.alloc(pt_total) || !d_outm.alloc(pt_total) ||
+      !d_vlog10.alloc(vlog10.size()) || !d_logc_n.alloc(tbl_total) || !d_logc_k.alloc(hlogc_k.size()) || !d_order.alloc(n) ||
+      !d_lm_order.alloc(n) || !d_work.alloc(kClasses + 1) || !d_si.alloc(si_need) || !d_se.alloc(huge_need) ||
+      !d_pool.alloc(huge_need) || !d_model.alloc(12 * (size_t)n) || !d_out.alloc(n) || !d_lm.alloc(n))
+    return fail(ctx, R3D_ERR_NOMEM, "r3d_resect_views: device scratch");
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_pairs.p, hpairs.data(), n * sizeof(AcPair), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_views.p, hviews.data(), n * sizeof(RsView), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_X.p, hX.data(), hX.size() * sizeof(double), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_xo.p, hx.data(), hx.size() * sizeof(double), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_vlog10.p, vlog10.data(), vlog10.size() * sizeof(float), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_logc_k.p, hlogc_k.data(), hlogc_k.size() * sizeof(float), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_order.p, horder.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_lm_order.p, lm_order.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_work.p, 0, (kClasses + 1) * sizeof(uint32_t), w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_lm.p, 0xff, n * sizeof(RsLm), w.stream));  // termination -1: not refined
+  cudaEvent_t ev[3];
+  for (auto& e : ev) R3D_CUDA_TRY(ctx, cudaEventCreate(&e));
+  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 3; ++i) cudaEventDestroy(e[i]); } } evg{ev};
+  R3D_CUDA_TRY(ctx, cudaEventRecord(ev[0], w.stream));
+  for (uint32_t a0 = 0; a0 < n; a0 += 65535u) {  // gridDim.y limit
+    const uint32_t na = std::min(65535u, n - a0);
+    k_resect_points<<<dim3(8, na), 256, 0, w.stream>>>(d_views.p + a0, d_X.p, d_xo.p, d_x1.p, d_x3.p, d_x2.p, d_idm.p);
+    T.kernel_launches += 1;
+  }
+  R3D_CUDA_TRY(ctx, cudaGetLastError());
+  {
+    const int rc = launch_ac_tables(ctx, w, d_pairs.p, n, d_vlog10.p, d_logc_n.p);
+    if (rc) return rc;
+    T.kernel_launches += 1;
+  }
+  for (int c = kClasses - 1; c >= 0; --c) {  // the long-running classes first
+    const uint32_t cnt = class_ofs[c + 1] - class_ofs[c];
+    if (!cnt) continue;
+    const int rc = launch_acransac_fused(ctx, w, 3, c == 5, d_pairs.p, d_order.p + class_ofs[c], cnt, d_work.p + c, d_x1.p, d_x2.p,
+                                         d_logc_n.p, d_logc_k.p, caps[c], opt.max_iter, d_se.p, d_si.p, d_pool.p, d_idm.p, d_outm.p,
+                                         d_out.p, d_model.p, grids[c], d_x3.p);
+    if (rc) return rc;
+    T.kernel_launches += 1;
+  }
+  R3D_CUDA_TRY(ctx, cudaEventRecord(ev[1], w.stream));
+  if (opt.refine) {
+    RsLmParams prm;
+    prm.max_iterations = opt.ba.max_iterations;
+    prm.huber_a = opt.ba.huber_a;
+    prm.function_tolerance = opt.ba.function_tolerance;
+    prm.gradient_tolerance = opt.ba.gradient_tolerance;
+    prm.parameter_tolerance = opt.ba.parameter_tolerance;
+    prm.initial_radius = opt.ba.initial_radius;
+    const uint32_t grid = std::min<uint32_t>(n, (uint32_t)w.sm_count);
+    k_resect_refine<<<grid, kRThreads, 0, w.stream>>>(d_views.p, d_lm_order.p, n, d_work.p + kClasses, d_out.p, d_model.p, d_outm.p,
+                                                      d_x1.p, d_x3.p, d_xo.p, d_lm.p, prm);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    T.kernel_launches += 1;
+  }
+  R3D_CUDA_TRY(ctx, cudaEventRecord(ev[2], w.stream));
+  std::vector<AcFusedOut> hout(n);
+  std::vector<double> hmodel(12 * (size_t)n);
+  std::vector<RsLm> hlm(n);
+  std::vector<uint2> houtm(pt_total);
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(hout.data(), d_out.p, n * sizeof(AcFusedOut), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(hmodel.data(), d_model.p, hmodel.size() * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(hlm.data(), d_lm.p, n * sizeof(RsLm), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(houtm.data(), d_outm.p, pt_total * sizeof(uint2), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+  float ms = 0.f;
+  cudaEventElapsedTime(&ms, ev[0], ev[1]);
+  T.ms_ransac = ms;
+  cudaEventElapsedTime(&ms, ev[1], ev[2]);
+  T.ms_refine = ms;
+  T.ms_device_total = T.ms_ransac + T.ms_refine;
+  for (uint32_t a = 0; a < n; ++a) {
+    const AcFusedOut& f = hout[a];
+    if (!(f.minNFA < 0.0) || !((double)f.n_inliers > 2.5 * 3)) continue;  // R3D_RESECT_NO_MODEL stays
+    r3d_resection& o = out[cand[a]];
+    o.status = R3D_RESECT_OK;
+    o.n_inliers = f.n_inliers;
+    o.found_residual_precision = std::sqrt(f.errorMax);
+    pose_from_projective(hpairs[a].K, &hmodel[12 * (size_t)a], o.rotation_ransac, o.translation_ransac);
+    set_pose(o, o.rotation_ransac, o.translation_ransac);
+    std::vector<uint32_t>& il = inl[cand[a]];
+    il.resize(f.n_inliers);
+    for (uint32_t k = 0; k < f.n_inliers; ++k) il[k] = houtm[(size_t)hpairs[a].pt_ofs + k].x;
+    if (!opt.refine) continue;
+    const RsLm& l = hlm[a];
+    o.lm_iterations = l.iterations;
+    o.lm_successful_steps = l.successful;
+    o.lm_termination = l.termination;
+    o.lm_initial_cost = l.initial_cost;
+    o.lm_final_cost = l.final_cost;
+    T.lm_iterations += l.iterations;
+    if (l.termination == 4) continue;  // the solve failed: the AC-RANSAC pose stays
+    double R[9];
+    angle_axis_to_rotation(l.pose, R);
+    set_pose(o, R, l.pose + 3);
+  }
+  T.ms_host = now_ms() - t0 - T.ms_device_total;
+  return R3D_OK;
+}
+
+bool finite_all(const double* p, size_t n) {
+  for (size_t i = 0; i < n; ++i)
+    if (!std::isfinite(p[i])) return false;
+  return true;
+}
+
+}  // namespace
+
+}  // namespace r3d
+
+using namespace r3d;
+
+extern "C" void r3d_resection_default_options(r3d_resection_options* o) {
+  if (!o) return;
+  o->precision_px = std::numeric_limits<double>::infinity();  // SfM_Localizer: error_max = infinity, pure a-contrario
+  o->max_iter = 4096;
+  o->refine = 1;
+  r3d_ba_default_options(&o->ba);
+  o->ba.refine_intrinsics = 0;  // RefinePose(b_refine_pose = true, b_refine_intrinsic = false)
+}
+
+extern "C" int r3d_resect_views(r3d_ctx* ctx, const r3d_resection_view* views, uint32_t n_views, const double* X, const double* x,
+                                const r3d_resection_options* opt, r3d_resection* out, uint32_t* inliers, uint64_t* inlier_ofs) {
+  if (!ctx || !opt || (n_views && (!views || !out))) return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: bad arguments");
+  if (inliers && !inlier_ofs) return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: inliers without inlier_ofs");
+  if (!(opt->precision_px > 0.0) || opt->max_iter == 0) return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: bad AC-RANSAC options");
+  if (opt->refine && opt->ba.refine_intrinsics)
+    return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: the pose refinement keeps the intrinsics fixed");
+  for (uint32_t v = 0; v < n_views; ++v) {
+    const r3d_resection_view& rv = views[v];
+    if (rv.count > 0xfffffff0ull) return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: too many correspondences in one view");
+    if (rv.count && (!X || !x)) return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: bad arguments");
+    if (rv.width == 0 || rv.height == 0) return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: a view without a size");
+    if (rv.intrinsic.focal > 0.0) {
+      const int m = rv.intrinsic.model;
+      if (m < R3D_CAM_PINHOLE || m > R3D_CAM_PINHOLE_FISHEYE) return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: unknown camera model");
+      if (!std::isfinite(rv.intrinsic.focal) || !std::isfinite(rv.intrinsic.ppx) || !std::isfinite(rv.intrinsic.ppy) ||
+          !finite_all(rv.intrinsic.disto, 5))
+        return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: non-finite intrinsic");
+    }
+    if (!finite_all(X + 3 * rv.first, 3 * rv.count) || !finite_all(x + 2 * rv.first, 2 * rv.count))
+      return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: non-finite correspondence");
+  }
+  std::vector<std::vector<uint32_t>> inl(n_views);
+  // the views are independent: contiguous ranges of equal correspondence counts, one per device (the rule of
+  // r3d_relative_poses)
+  const size_t nw = ctx->workers.size();
+  std::vector<uint32_t> cut(nw + 1, 0);
+  {
+    std::vector<double> cost(n_views + 1, 0.0);
+    for (uint32_t v = 0; v < n_views; ++v) cost[v + 1] = cost[v] + (double)views[v].count + 1.0;
+    for (size_t k = 1; k < nw; ++k)
+      cut[k] = std::min<uint32_t>(n_views, (uint32_t)(std::lower_bound(cost.begin(), cost.end(), cost[n_views] * (double)k / (double)nw) - cost.begin()));
+    cut[nw] = n_views;
+  }
+  std::vector<int> rcs(nw, R3D_OK);
+  std::vector<r3d_resection_timing> tms(nw);
+  if (nw == 1) {
+    rcs[0] = resect_range(ctx, ctx->workers[0], views, 0, n_views, X, x, *opt, out, inl, tms[0]);
+  } else {
+    std::vector<std::thread> th;
+    for (size_t k = 0; k < nw; ++k)
+      th.emplace_back([&, k]() { rcs[k] = resect_range(ctx, ctx->workers[k], views, cut[k], cut[k + 1], X, x, *opt, out, inl, tms[k]); });
+    for (auto& t : th) t.join();
+  }
+  for (int rc : rcs)
+    if (rc) return rc;
+  r3d_resection_timing sum{};
+  for (const r3d_resection_timing& t : tms) {
+    sum.ms_ransac = std::max(sum.ms_ransac, t.ms_ransac);
+    sum.ms_refine = std::max(sum.ms_refine, t.ms_refine);
+    sum.ms_device_total = std::max(sum.ms_device_total, t.ms_device_total);
+    sum.ms_host = std::max(sum.ms_host, t.ms_host);
+    sum.kernel_launches += t.kernel_launches;
+    sum.lm_iterations += t.lm_iterations;
+  }
+  ctx->resection_timing = sum;
+  if (inlier_ofs) {
+    uint64_t ofs = 0;
+    for (uint32_t v = 0; v < n_views; ++v) {
+      inlier_ofs[v] = ofs;
+      if (inliers) std::memcpy(inliers + ofs, inl[v].data(), inl[v].size() * sizeof(uint32_t));
+      ofs += inl[v].size();
+    }
+    inlier_ofs[n_views] = ofs;
+  }
+  return R3D_OK;
+}
+
+extern "C" int r3d_sfm_resect_views(r3d_ctx* ctx, r3d_sfm_data* sd, const uint32_t* view_ids, uint32_t n,
+                                    const r3d_resection_options* opt, r3d_resection* out, uint32_t* n_out) {
+  if (!ctx || !sd || !opt || (n && !view_ids)) return fail(ctx, R3D_ERR_INVALID, "r3d_sfm_resect_views: bad arguments");
+  if (n_out) *n_out = 0;
+  std::vector<uint32_t> ids;
+  if (n) {
+    ids.assign(view_ids, view_ids + n);
+  } else {
+    for (const auto& kv : sd->views)
+      if (!sd->poses.count(kv.second.id_pose)) ids.push_back(kv.first);
+  }
+  if (ids.size() && !out) return fail(ctx, R3D_ERR_INVALID, "r3d_sfm_resect_views: bad arguments");
+  std::vector<r3d_resection_view> rv(ids.size());
+  std::map<uint32_t, uint32_t> slot;  // view id -> index in rv
+  for (size_t k = 0; k < ids.size(); ++k) {
+    const auto vit = sd->views.find(ids[k]);
+    if (vit == sd->views.end()) return fail(ctx, R3D_ERR_INVALID, "r3d_sfm_resect_views: unknown view id");
+    if (sd->poses.count(vit->second.id_pose)) return fail(ctx, R3D_ERR_INVALID, "r3d_sfm_resect_views: the view already has a pose");
+    if (!slot.emplace(ids[k], (uint32_t)k).second) return fail(ctx, R3D_ERR_INVALID, "r3d_sfm_resect_views: a view id given twice");
+    const auto iit = sd->intrinsics.find(vit->second.id_intrinsic);
+    if (iit == sd->intrinsics.end()) return fail(ctx, R3D_ERR_INVALID, "r3d_sfm_resect_views: unknown intrinsic id");
+    r3d_resection_view& r = rv[k];
+    std::memset(&r, 0, sizeof(r));
+    r.view_id = ids[k];
+    r.width = vit->second.width;
+    r.height = vit->second.height;
+    r.intrinsic.id = iit->first;
+    r.intrinsic.model = iit->second.model;
+    r.intrinsic.width = iit->second.width;
+    r.intrinsic.height = iit->second.height;
+    r.intrinsic.focal = iit->second.focal;
+    r.intrinsic.ppx = iit->second.ppx;
+    r.intrinsic.ppy = iit->second.ppy;
+    for (size_t i = 0; i < iit->second.disto.size() && i < 5; ++i) r.intrinsic.disto[i] = iit->second.disto[i];
+  }
+  // the 2D-3D correspondences of a view: every landmark that holds an observation of it, in landmark-id order
+  std::vector<std::vector<double>> Xs(ids.size()), xs(ids.size());
+  for (const auto& lm : sd->structure)
+    for (const auto& ob : lm.second.obs) {
+      const auto s = slot.find(ob.first);
+      if (s == slot.end()) continue;
+      Xs[s->second].insert(Xs[s->second].end(), lm.second.X, lm.second.X + 3);
+      xs[s->second].insert(xs[s->second].end(), ob.second.x, ob.second.x + 2);
+    }
+  std::vector<double> X, x;
+  for (size_t k = 0; k < ids.size(); ++k) {
+    rv[k].first = x.size() / 2;
+    rv[k].count = xs[k].size() / 2;
+    X.insert(X.end(), Xs[k].begin(), Xs[k].end());
+    x.insert(x.end(), xs[k].begin(), xs[k].end());
+  }
+  X.resize(std::max<size_t>(X.size(), 3));
+  x.resize(std::max<size_t>(x.size(), 2));
+  const int rc = r3d_resect_views(ctx, rv.data(), (uint32_t)rv.size(), X.data(), x.data(), opt, out, nullptr, nullptr);
+  if (rc) return rc;
+  for (size_t k = 0; k < ids.size(); ++k) {
+    if (out[k].status != R3D_RESECT_OK) continue;
+    r3d_sfm_data::Pose p;
+    std::memcpy(p.R, out[k].rotation, sizeof(p.R));
+    std::memcpy(p.C, out[k].center, sizeof(p.C));
+    sd->poses[sd->views[ids[k]].id_pose] = p;
+  }
+  if (n_out) *n_out = (uint32_t)ids.size();
+  return R3D_OK;
+}
+
+extern "C" int r3d_get_resection_timing(const r3d_ctx* ctx, r3d_resection_timing* out) {
+  if (!ctx || !out) return R3D_ERR_INVALID;
+  *out = ctx->resection_timing;
+  return R3D_OK;
+}
