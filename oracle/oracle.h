@@ -160,7 +160,7 @@ int64_t orc_tracks_build(const uint32_t* pairs, uint64_t P, const uint64_t* pair
                          uint64_t cap_nodes);
 void orc_triangulate_landmarks(uint32_t n_lm, const uint64_t* obs_ofs, const uint32_t* obs_cam, const double* obs_xy,
                                const double* poses, const uint32_t* cam_intr, const double* intrinsics, const uint8_t* intr_model,
-                               double* X, uint8_t* ok);
+                               const double* intrinsics_ext, double* X, uint8_t* ok);
 void orc_landmark_checks(uint32_t n_lm, const uint64_t* obs_ofs, const uint32_t* obs_cam, const double* obs_xy, const double* poses,
                          const uint32_t* cam_intr, const double* intrinsics, const uint8_t* intr_model, const double* intrinsics_ext,
                          const double* X, double thr_px, uint8_t* keep_obs, double* max_angle);

@@ -22,6 +22,7 @@
 #include "oracle_resection.h"
 
 #include "oracle_detmath.hpp"
+#include "oracle_undistort.hpp"
 
 #include <algorithm>
 #include <cfloat>
@@ -37,7 +38,6 @@
 namespace orc {
 namespace rs {
 
-constexpr int kUndistortIters = 10;
 
 // numeric/poly.h SolveCubicPolynomial, as oracle_acransac.cpp
 static int solve_cubic_monic(double a, double b, double c, double* x0, double* x1, double* x2) {
@@ -92,48 +92,6 @@ static void bearing(const double* K, double x, double y, double* b) {
   const double bx = kinv00 * x + kinv02, by = kinv00 * y + kinv12, bz = 1.0;
   const double n = std::sqrt((bx * bx + by * by) + bz * bz);
   b[0] = bx / n; b[1] = by / n; b[2] = bz / n;
-}
-
-static void undistort_pixel(int model, double f, double ppx, double ppy, const double* disto, double x, double y, double* xo,
-                            double* yo) {
-  const double xd = (x - ppx) / f, yd = (y - ppy) / f;
-  double xu = xd, yu = yd;
-  if (model == 5) {
-    const double rd = std::sqrt(xd * xd + yd * yd);
-    if (rd > 1e-8) {
-      double th = rd;
-      for (int it = 0; it < kUndistortIters; ++it) {
-        const double t2 = th * th, t4 = t2 * t2, t6 = t4 * t2, t8 = t4 * t4;
-        const double g = th * (1.0 + disto[0] * t2 + disto[1] * t4 + disto[2] * t6 + disto[3] * t8) - rd;
-        const double dg = 1.0 + 3.0 * disto[0] * t2 + 5.0 * disto[1] * t4 + 7.0 * disto[2] * t6 + 9.0 * disto[3] * t8;
-        th = th - g / dg;
-      }
-      const double ru = det::cos(0.5 * det::kPi - th) / det::cos(th);  // tan(theta)
-      const double s = ru / rd;
-      xu = xd * s;
-      yu = yd * s;
-    }
-  } else if (model >= 2) {
-    const double k1 = disto[0], k2 = model >= 3 ? disto[1] : 0.0, k3 = model >= 3 ? disto[2] : 0.0;
-    const double t1 = model == 4 ? disto[3] : 0.0, t2 = model == 4 ? disto[4] : 0.0;
-    for (int it = 0; it < kUndistortIters; ++it) {
-      const double r2 = xu * xu + yu * yu, r4 = r2 * r2, r6 = r4 * r2;
-      const double c = 1.0 + k1 * r2 + k2 * r4 + k3 * r6;
-      const double dc = k1 + 2.0 * k2 * r2 + 3.0 * k3 * r4;
-      const double fx = xu * c + t2 * (r2 + 2.0 * xu * xu) + 2.0 * t1 * xu * yu - xd;
-      const double fy = yu * c + t1 * (r2 + 2.0 * yu * yu) + 2.0 * t2 * xu * yu - yd;
-      const double a00 = c + 2.0 * xu * xu * dc + 6.0 * t2 * xu + 2.0 * t1 * yu;
-      const double a01 = 2.0 * xu * yu * dc + 2.0 * t2 * yu + 2.0 * t1 * xu;
-      const double a11 = c + 2.0 * yu * yu * dc + 6.0 * t1 * yu + 2.0 * t2 * xu;
-      const double dt = a00 * a11 - a01 * a01;
-      if (dt == 0.0) break;
-      const double dx = (a11 * fx - a01 * fy) / dt, dy = (a00 * fy - a01 * fx) / dt;
-      xu = xu - dx;
-      yu = yu - dy;
-    }
-  }
-  *xo = f * xu + ppx;
-  *yo = f * yu + ppy;
 }
 
 static int quadratic_roots(double b, double c, double* r) {
@@ -654,8 +612,8 @@ int orc_p3p(const double* K, const double* X, const double* x, double* P) { retu
 
 void orc_undistort(int model, const double* intr8, const double* xy, uint32_t n, double* out) {
   for (uint32_t i = 0; i < n; ++i)
-    undistort_pixel(model, intr8[0], intr8[1], intr8[2], intr8 + 3, xy[2 * (size_t)i], xy[2 * (size_t)i + 1], out + 2 * (size_t)i,
-                    out + 2 * (size_t)i + 1);
+    orc::undistort_newton(model, intr8[0], intr8[1], intr8[2], intr8 + 3, xy[2 * (size_t)i], xy[2 * (size_t)i + 1],
+                          out + 2 * (size_t)i, out + 2 * (size_t)i + 1);
 }
 
 int orc_resect_refine(int model, const double* intr8, const double* X, const double* x, uint32_t N, const orc_ba_options* o,

@@ -8,6 +8,7 @@
 // published sources (tracks/tracks.hpp + union_find.hpp, multiview/triangulation_nview.hpp `Triangulation`,
 // sfm/sfm_data_triangulation.cpp SfM_Data_Structure_Computation_Blind, sfm/sfm_data_filters.hpp).  PARITY UNPINNED.
 #include "oracle.h"
+#include "oracle_undistort.hpp"
 
 #include <algorithm>
 #include <cmath>
@@ -100,9 +101,15 @@ double undistort_radius_factor(int model, const double* k, double r2d) {
 }
 }  // namespace
 
-// cam->get_ud_pixel(x): pixel without distortion (models 1-3; Brown / fisheye: not restated, identity for zero coefficients)
-void undistort_pixel(int model, const double* intr, const double* x, double* out) {
+// cam->get_ud_pixel(x): pixel without distortion.  Radial K1 / K3 by upstream's bisection; Brown T2 and fisheye by the
+// resection oracle's Newton inverse (oracle_undistort.hpp).  intr: f ppx ppy k1 k2 k3; ext: t1 t2 (Brown) or k4 (fisheye)
+void undistort_pixel(int model, const double* intr, const double* ext, const double* x, double* out) {
   const double f = intr[0], ppx = intr[1], ppy = intr[2];
+  if (model == 4 || model == 5) {
+    const double disto[5] = {intr[3], intr[4], intr[5], ext ? ext[0] : 0.0, ext ? ext[1] : 0.0};
+    undistort_newton(model, f, ppx, ppy, disto, x[0], x[1], out, out + 1);
+    return;
+  }
   if (model < 2 || model > 3 || (intr[3] == 0.0 && intr[4] == 0.0 && intr[5] == 0.0)) { out[0] = x[0]; out[1] = x[1]; return; }
   const double xd = (x[0] - ppx) / f, yd = (x[1] - ppy) / f;
   const double s = undistort_radius_factor(model, intr + 3, xd * xd + yd * yd);
@@ -177,11 +184,11 @@ int64_t orc_tracks_build(const uint32_t* pairs, uint64_t P, const uint64_t* pair
 }
 
 // SfM_Data_Structure_Computation_Blind::triangulate on flat arrays: landmark l has observations obs_ofs[l]..obs_ofs[l+1]
-// (camera index, pixel); cameras: pose (angle-axis | t) and intrinsic group (model, intr[6]).  ok[l] = 1 and X[l] set when
-// >= 2 observations and the smallest depth is positive.
+// (camera index, pixel); cameras: pose (angle-axis | t) and intrinsic group (model, intr[6], ext[2] = t1 t2 | k4 0, or
+// null for zeros).  ok[l] = 1 and X[l] set when >= 2 observations and the smallest depth is positive.
 void orc_triangulate_landmarks(uint32_t n_lm, const uint64_t* obs_ofs, const uint32_t* obs_cam, const double* obs_xy,
                                const double* poses, const uint32_t* cam_intr, const double* intrinsics, const uint8_t* intr_model,
-                               double* X, uint8_t* ok);
+                               const double* intrinsics_ext, double* X, uint8_t* ok);
 }
 
 namespace {
@@ -201,7 +208,7 @@ extern "C" {
 
 void orc_triangulate_landmarks(uint32_t n_lm, const uint64_t* obs_ofs, const uint32_t* obs_cam, const double* obs_xy,
                                const double* poses, const uint32_t* cam_intr, const double* intrinsics, const uint8_t* intr_model,
-                               double* X, uint8_t* ok) {
+                               const double* intrinsics_ext, double* X, uint8_t* ok) {
 #pragma omp parallel for schedule(dynamic, 256)
   for (int64_t l = 0; l < (int64_t)n_lm; ++l) {
     const int n = (int)(obs_ofs[l + 1] - obs_ofs[l]);
@@ -226,7 +233,8 @@ void orc_triangulate_landmarks(uint32_t n_lm, const uint64_t* obs_ofs, const uin
       PM[3] = Kf * tr[0] + kx * tr[2];
       PM[7] = Kf * tr[1] + ky * tr[2];
       PM[11] = tr[2];
-      orc::undistort_pixel(intr_model ? intr_model[g] : 3, in, obs_xy + 2 * o, &x[2 * (size_t)t]);
+      orc::undistort_pixel(intr_model ? intr_model[g] : 3, in, intrinsics_ext ? intrinsics_ext + 2 * (size_t)g : nullptr, obs_xy + 2 * o,
+                           &x[2 * (size_t)t]);
     }
     double zmin;
     orc::triangulate_nview(P.data(), x.data(), n, X + 3 * l, &zmin);

@@ -546,7 +546,12 @@ def tracks_build(pairs, pair_ofs, m, min_length=2):
             for k in range(T)}
 
 
-def triangulate_landmarks(obs_ofs, obs_cam, obs_xy, poses, cam_intr, intrinsics, intr_model=None):
+def _ext(intr_ext, n_intr):
+    """intrinsics_ext per intrinsic group (t1 t2 for Brown, k4 0 for the fisheye); None: zeros."""
+    return None if intr_ext is None else np.ascontiguousarray(np.asarray(intr_ext, np.float64).reshape(n_intr, 2))
+
+
+def triangulate_landmarks(obs_ofs, obs_cam, obs_xy, poses, cam_intr, intrinsics, intr_model=None, intr_ext=None):
     obs_ofs = np.ascontiguousarray(obs_ofs, np.uint64)
     obs_cam = np.ascontiguousarray(obs_cam, np.uint32)
     obs_xy = np.ascontiguousarray(obs_xy, np.float64)
@@ -557,12 +562,13 @@ def triangulate_landmarks(obs_ofs, obs_cam, obs_xy, poses, cam_intr, intrinsics,
     X = np.zeros((n, 3))
     ok = np.zeros(n, np.uint8)
     im = None if intr_model is None else np.ascontiguousarray(intr_model, np.uint8)
+    ext = _ext(intr_ext, len(intrinsics))
     lib().orc_triangulate_landmarks(C.c_uint32(n), _p(obs_ofs), _p(obs_cam), _p(obs_xy), _p(poses), _p(cam_intr), _p(intrinsics),
-                                    None if im is None else _p(im), _p(X), _p(ok))
+                                    None if im is None else _p(im), None if ext is None else _p(ext), _p(X), _p(ok))
     return X, ok.astype(bool)
 
 
-def landmark_checks(obs_ofs, obs_cam, obs_xy, poses, cam_intr, intrinsics, X, thr_px, intr_model=None):
+def landmark_checks(obs_ofs, obs_cam, obs_xy, poses, cam_intr, intrinsics, X, thr_px, intr_model=None, intr_ext=None):
     obs_ofs = np.ascontiguousarray(obs_ofs, np.uint64)
     obs_cam = np.ascontiguousarray(obs_cam, np.uint32)
     obs_xy = np.ascontiguousarray(obs_xy, np.float64)
@@ -574,6 +580,8 @@ def landmark_checks(obs_ofs, obs_cam, obs_xy, poses, cam_intr, intrinsics, X, th
     keep = np.zeros(len(obs_cam), np.uint8)
     ang = np.zeros(n)
     im = None if intr_model is None else np.ascontiguousarray(intr_model, np.uint8)
+    ext = _ext(intr_ext, len(intrinsics))
     lib().orc_landmark_checks(C.c_uint32(n), _p(obs_ofs), _p(obs_cam), _p(obs_xy), _p(poses), _p(cam_intr), _p(intrinsics),
-                              None if im is None else _p(im), None, _p(X), C.c_double(thr_px), _p(keep), _p(ang))
+                              None if im is None else _p(im), None if ext is None else _p(ext), _p(X), C.c_double(thr_px),
+                              _p(keep), _p(ang))
     return keep.astype(bool), ang

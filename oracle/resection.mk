@@ -10,7 +10,7 @@ all: $(OUT)
 _build/liboracle.so: FORCE
 	$(MAKE) -f Makefile
 
-$(OUT): oracle_resection.cpp oracle_resection.h oracle.h oracle_detmath.hpp _build/liboracle.so
+$(OUT): oracle_resection.cpp oracle_resection.h oracle.h oracle_detmath.hpp oracle_undistort.hpp _build/liboracle.so
 	$(CXX) $(CXXFLAGS) -shared -o $@ oracle_resection.cpp -L_build -loracle -Wl,-rpath,'$$ORIGIN'
 
 FORCE:

@@ -22,7 +22,9 @@ namespace p3p {
 constexpr int kUndistortIters = 10;
 
 // get_ud_pixel: inverse of the camera model's distortion by a fixed number of Newton steps (model: R3D_CAM_* 1..5;
-// disto: k1 k2 k3 t1 t2 for the polynomial models, k1 k2 k3 k4 for the fisheye)
+// disto: k1 k2 k3 t1 t2 for the polynomial models, k1 k2 k3 k4 for the fisheye).  sfm_structure.cu also calls it for
+// the Brown and fisheye observations it triangulates; that unit keeps FMA contraction, and its tests hold it to a
+// tolerance rather than to the oracle's bits.
 __device__ inline void undistort_pixel(int model, double f, double ppx, double ppy, const double* disto, double x, double y,
                                        double* xo, double* yo) {
   const double xd = (x - ppx) / f, yd = (y - ppy) / f;

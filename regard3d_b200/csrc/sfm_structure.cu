@@ -11,6 +11,7 @@
 #include "r3d_internal.cuh"
 #include "r3d_sfm.h"
 #include "ba_model.cuh"
+#include "p3p.cuh"
 
 #include <cstring>
 #include <map>
@@ -45,8 +46,15 @@ __global__ void k_camera_matrices(const double* __restrict__ poses, const uint32
   PM[11] = t[2];
 }
 
-// cam->get_ud_pixel(x) for the radial models (bisection on the radius, as Pinhole_Intrinsic_Radial_K*::remove_disto)
-__device__ void undistort_pixel(int model, const double* in, double x, double y, double* ox, double* oy) {
+// cam->get_ud_pixel(x): radial K1 / K3 by bisection on the radius (as Pinhole_Intrinsic_Radial_K*::remove_disto), Brown
+// T2 and fisheye by the resection step's Newton inverse (p3p::undistort_pixel), pinhole unchanged.
+// in: f ppx ppy k1 k2 k3; ext: t1 t2 (Brown) or k4 (fisheye)
+__device__ void undistort_pixel(int model, const double* in, const double* ext, double x, double y, double* ox, double* oy) {
+  if (model == 4 || model == 5) {
+    const double disto[5] = {in[3], in[4], in[5], ext[0], ext[1]};
+    p3p::undistort_pixel(model, in[0], in[1], in[2], disto, x, y, ox, oy);
+    return;
+  }
   if (model < 2 || model > 3 || (in[3] == 0.0 && in[4] == 0.0 && in[5] == 0.0)) { *ox = x; *oy = y; return; }
   const double f = in[0], xd = (x - in[1]) / f, yd = (y - in[2]) / f;
   const double r2d = xd * xd + yd * yd;
@@ -72,7 +80,8 @@ __global__ void __launch_bounds__(128) k_triangulate(uint32_t n_lm, const uint64
                                                      const uint32_t* __restrict__ obs_cam, const double2* __restrict__ obs_xy,
                                                      const double* __restrict__ P, const uint32_t* __restrict__ cam_intr,
                                                      const double* __restrict__ intr, const uint8_t* __restrict__ intr_model,
-                                                     double* __restrict__ X, uint8_t* __restrict__ ok) {
+                                                     const double* __restrict__ intr_ext, double* __restrict__ X,
+                                                     uint8_t* __restrict__ ok) {
   const uint32_t l = blockIdx.x * blockDim.x + threadIdx.x;
   if (l >= n_lm) return;
   const uint64_t b = obs_ofs[l], e = obs_ofs[l + 1];
@@ -85,7 +94,8 @@ __global__ void __launch_bounds__(128) k_triangulate(uint32_t n_lm, const uint64
       const uint32_t c = obs_cam[o], g = cam_intr[c];
       const double* PM = P + 12 * (size_t)c;
       double px, py;
-      undistort_pixel(intr_model ? (int)intr_model[g] : 3, intr + 6 * (size_t)g, obs_xy[o].x, obs_xy[o].y, &px, &py);
+      undistort_pixel(intr_model ? (int)intr_model[g] : 3, intr + 6 * (size_t)g, intr_ext + 2 * (size_t)g, obs_xy[o].x, obs_xy[o].y,
+                      &px, &py);
       double w = 1.0;
       if (it > 0) w = 1.0 / (PM[8] * Xl[0] + PM[9] * Xl[1] + PM[10] * Xl[2] + PM[11]);
       double v1[3], v2[3];
@@ -284,7 +294,8 @@ extern "C" int r3d_sfm_structure_from_tracks(r3d_ctx* ctx, r3d_sfm_data* sd, con
     if ((rc = upload(ctx, F, D))) return rc;
     const uint32_t n_cams = (uint32_t)F.pose_index.size();
     sfmk::k_camera_matrices<<<(n_cams + 127) / 128, 128, 0, w.stream>>>(D.poses, D.cam_intr, D.intr, n_cams, D.P);
-    sfmk::k_triangulate<<<(n_lm + 127) / 128, 128, 0, w.stream>>>(n_lm, D.obs_ofs, D.obs_cam, D.obs_xy, D.P, D.cam_intr, D.intr, D.model, D.X, D.ok);
+    sfmk::k_triangulate<<<(n_lm + 127) / 128, 128, 0, w.stream>>>(n_lm, D.obs_ofs, D.obs_cam, D.obs_xy, D.P, D.cam_intr, D.intr, D.model, D.ext,
+                                                                  D.X, D.ok);
     R3D_CUDA_TRY(ctx, cudaGetLastError());
     std::vector<uint8_t> hok(n_lm);
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(F.X.data(), D.X, F.X.size() * 8, cudaMemcpyDeviceToHost, w.stream));

@@ -64,13 +64,24 @@ def test_matches_to_tracks_to_structure_to_ba(gpu_ctx, oracle, r3dlib):
         if len(tids) == 1 and -1 not in tids:
             err.append(np.linalg.norm(np.array(lm["X"]) - sc["points"][tids.pop()]))
     assert len(err) > 250 and np.median(err) < 0.05
-    # outlier rejection: flags equal the oracle's, then BA on what is left
+    # outlier rejection: the observations kept and the angle decisions equal the oracle's, then BA on what is left
     keep_o, ang_o = oracle.landmark_checks(ofs, cam, xy, poses, np.zeros(6, np.uint32), intr, X, 4.0)
+    # the angle test runs on what the residual test left: the oracle's largest angle over the kept observations
+    kofs = np.r_[0, np.cumsum(np.add.reduceat(keep_o.astype(np.int64), ofs[:-1].astype(np.int64)))].astype(np.uint64)
+    _, ang_kept = oracle.landmark_checks(kofs, cam[keep_o], xy[keep_o], poses, np.zeros(6, np.uint32), intr, X, np.inf)
     n_obs_before = sum(len(lm["obs"]) for lm in lms)
     rm_obs, rm_lm = gpu_ctx.remove_outliers(sd, 4.0, 2, 2.0)
     assert rm_obs == int((~keep_o).sum())
+    expected = {}
+    for l, lm in enumerate(lms):
+        k = keep_o[int(ofs[l]):int(ofs[l + 1])]
+        kept = sorted((v, f) for (v, f, _, _), kk in zip(lm["obs"], k) if kk)
+        assert ang_kept[l] <= ang_o[l] + 1e-12
+        if len(kept) >= 2 and ang_kept[l] >= 2.0:
+            expected[lm["id"]] = kept
     after = sd.landmarks()
-    assert sum(len(lm["obs"]) for lm in after) <= n_obs_before - rm_obs and len(after) == len(lms) - rm_lm
+    assert {lm["id"]: sorted((v, f) for (v, f, _, _) in lm["obs"]) for lm in after} == expected
+    assert sum(len(lm["obs"]) for lm in after) == n_obs_before - rm_obs and len(after) == len(lms) - rm_lm
     s = gpu_ctx.sfm_bundle_adjust(sd, max_iterations=25)
     assert s["final_cost"] <= s["initial_cost"] and s["iterations"] >= 1
     res = np.sqrt(2.0 * s["final_cost"] / max(1, sum(len(lm["obs"]) for lm in after)))
