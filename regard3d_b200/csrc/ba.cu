@@ -19,6 +19,7 @@
 // the path is bound by the observation stream, not by arithmetic.
 #include "r3d_internal.cuh"
 #include "ba_model.cuh"
+#include "lm_trust_region.cuh"
 
 #include <cooperative_groups.h>
 
@@ -1557,20 +1558,15 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
   double cost = 0;
   if ((rc = eval_cost(d.poses, d.intr, d.pts, &cost))) return rc;
   sum->initial_cost = cost;
-  sum->iterations = 0;
-  sum->successful_steps = 0;
-  sum->termination = 0;
   sum->seconds_linear = 0;
   if (cost_trace) cost_trace[0] = cost;
-  double radius = opt->initial_radius, decrease_factor = 2.0;
+  r3d::LmTrustRegion lm(r3d::lm_params(*opt));
   if ((rc = evaluate())) return rc;
-  bool stop = gmax <= opt->gradient_tolerance;
-  if (stop) sum->termination = 2;
-
+  const bool stop = lm.start(gmax);
   for (uint32_t iter = 1; !stop && iter <= opt->max_iterations; ++iter) {
-    sum->iterations = iter;
+    lm.iterations = iter;
     const auto t_lin = std::chrono::steady_clock::now();
-    const double inv_radius = 1.0 / radius;
+    const double inv_radius = 1.0 / lm.radius;
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.S, 0, ((size_t)nB * nB + nB) * 8, w.stream));
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.scal, 0, 5 * sizeof(double), w.stream));
     if (plan.n_batches)
@@ -1596,44 +1592,33 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
     if ((rc = comm_allreduce(ctx, w.stream, d.scal + 1, 3, kCommSum))) return rc;
     if ((rc = read_scal())) return rc;
     sum->seconds_linear += std::chrono::duration<double>(std::chrono::steady_clock::now() - t_lin).count();
-    const bool pd = h_scal[4] == 0.0;
     const double model_cost_change = 0.5 * h_scal[1];
     bool accepted = false;
-    if (pd && model_cost_change > 0.0 && std::isfinite(model_cost_change)) {
-      if (std::sqrt(h_scal[2]) <= opt->parameter_tolerance * (std::sqrt(h_scal[3]) + opt->parameter_tolerance)) {
-        sum->termination = 3;
+    if (lm.step_usable(h_scal[4] == 0.0, model_cost_change)) {
+      if (lm.step_too_small(h_scal[2], h_scal[3])) {
         if (cost_trace) cost_trace[iter] = cost;
         break;
       }
       double new_cost = 0;
       if ((rc = eval_cost(d.poses_new, d.intr_new, d.pts_new, &new_cost))) return rc;
-      const double relative_decrease = (cost - new_cost) / model_cost_change;
-      if (relative_decrease > 1e-3) {
-        accepted = true;
+      if ((accepted = lm.accept(cost, new_cost, model_cost_change))) {
         std::swap(d.poses, d.poses_new);
         std::swap(d.intr, d.intr_new);
         std::swap(d.pts, d.pts_new);
-        const double cost_change = cost - new_cost;
-        const double t = 2.0 * relative_decrease - 1.0;
-        radius = radius / std::max(1.0 / 3.0, 1.0 - t * t * t);
-        radius = std::min(1e16, radius);
-        decrease_factor = 2.0;
-        sum->successful_steps++;
-        const bool ftol = std::fabs(cost_change) < opt->function_tolerance * cost;
         cost = new_cost;
         if (cost_trace) cost_trace[iter] = cost;
         if ((rc = evaluate())) return rc;
-        if (ftol) { sum->termination = 1; break; }
-        if (gmax <= opt->gradient_tolerance) { sum->termination = 2; break; }
+        if (lm.converged(gmax)) break;
       }
     }
     if (!accepted) {
-      radius = radius / decrease_factor;
-      decrease_factor *= 2.0;
       if (cost_trace) cost_trace[iter] = cost;
-      if (radius < 1e-32) { sum->termination = 4; break; }
+      if (lm.reject()) break;
     }
   }
+  sum->iterations = lm.iterations;
+  sum->successful_steps = lm.successful;
+  sum->termination = lm.termination;
   sum->final_cost = cost;
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(p->poses, d.poses, 6 * (size_t)p->n_cams * 8, cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(p->intrinsics, d.intr, 6 * (size_t)p->n_intr * 8, cudaMemcpyDeviceToHost, w.stream));

@@ -17,6 +17,7 @@
 //      is reproducible.  FP64 throughout; the kernel is bound by FP64 latency, not by tensor cores or HBM.
 #include "acransac.cuh"
 #include "ba_model.cuh"
+#include "lm_trust_region.cuh"
 #include "relpose_math.cuh"
 
 #include <chrono>
@@ -53,11 +54,6 @@ struct RpBa {              // bundle adjustment: initial state in, solution out
   int termination;
   int pad_;
   double initial_cost, final_cost;
-};
-
-struct RpBaParams {
-  uint32_t max_iterations;
-  double huber_a, function_tolerance, gradient_tolerance, parameter_tolerance, initial_radius;
 };
 
 constexpr int kCThreads = 128;
@@ -136,26 +132,6 @@ struct BaSmem {
   uint32_t work;
 };
 
-__device__ double block_sum(double v, double* red) {
-  for (int o = 16; o >= 1; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  __syncthreads();
-  if ((threadIdx.x & 31u) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < kBWarps; ++w) s += red[w];
-  return s;
-}
-
-__device__ double block_max(double v, double* red) {
-  for (int o = 16; o >= 1; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
-  __syncthreads();
-  if ((threadIdx.x & 31u) == 0) red[threadIdx.x >> 5] = v;
-  __syncthreads();
-  double s = 0.0;
-  for (int w = 0; w < kBWarps; ++w) s = fmax(s, red[w]);
-  return s;
-}
-
 // sums[e] = sum over the points of fn(e, p), e < n: the points are cut into fixed ranges, one thread per (range,
 // entry) walks its range in order, the ranges are added in order -- the same bits on every call
 template <class Fn>
@@ -183,7 +159,7 @@ __device__ void entry_sums(int n, uint32_t N, BaSmem& S, Fn fn) {
 __global__ void __launch_bounds__(kBThreads) k_relpose_ba(const RpPair* __restrict__ pairs, const uint32_t* __restrict__ order,
                                                           uint32_t n_order, uint32_t* __restrict__ work_counter,
                                                           const double2* __restrict__ xa1, const double2* __restrict__ xa2,
-                                                          RpBa* __restrict__ io, RpBaParams prm, double* __restrict__ scratch,
+                                                          RpBa* __restrict__ io, LmParams prm, double* __restrict__ scratch,
                                                           uint32_t cap) {
   __shared__ BaSmem S;
   const uint32_t tid = threadIdx.x;
@@ -231,7 +207,7 @@ __global__ void __launch_bounds__(kBThreads) k_relpose_ba(const RpPair* __restri
           c += 0.5 * ba::huber_rho(r[0] * r[0] + r[1] * r[1], prm.huber_a, &rho1);
         }
       }
-      return block_sum(c, S.red);
+      return block_sum_fixed<kBThreads>(c, S.red);
     };
     // residuals, Jacobians (Corrector-scaled), the Jacobi scale on the first call, then g and diag(J^T J)
     auto evaluate = [&](bool first) {
@@ -295,30 +271,27 @@ __global__ void __launch_bounds__(kBThreads) k_relpose_ba(const RpPair* __restri
       double m = 0.0;
       for (uint32_t p = tid; p < N; p += kBThreads)
         for (int k = 0; k < 3; ++k) m = fmax(m, fabs(F(fG + k, p) / F(fS + k, p)));
-      m = block_max(m, S.red);
+      m = block_max_fixed<kBThreads>(m, S.red);
       for (int j = 0; j < 12; ++j) m = fmax(m, fabs(S.g[j] / S.scale[j]));
       return m;
     };
 
     double cost = total_cost(S.pose, cur);
     const double initial_cost = cost;
-    uint32_t iterations = 0, successful = 0;
-    int termination = 0;
-    double radius = prm.initial_radius, decrease_factor = 2.0;
+    LmTrustRegion lm(prm);  // every thread keeps its own: the inputs are block-wide, so are the decisions
     evaluate(true);
-    if (grad_max() <= prm.gradient_tolerance) termination = 2;
-    else
+    if (!lm.start(grad_max()))
       for (uint32_t iter = 1; iter <= prm.max_iterations; ++iter) {
-        iterations = iter;
+        lm.iterations = iter;
         // LevenbergMarquardtStrategy: D^2 = clamp(diag(J^T J), 1e-6, 1e32) / radius
-        if (tid < 12) S.D2[tid] = fmin(fmax(S.diag[tid], 1e-6), 1e32) / radius;
+        if (tid < 12) S.D2[tid] = fmin(fmax(S.diag[tid], 1e-6), 1e32) / lm.radius;
         for (uint32_t p = tid; p < N; p += kBThreads) {  // point blocks: (V + D^2)^-1, W (V + D^2)^-1, (V + D^2)^-1 g
           double V[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
           for (int v = 0; v < 2; ++v)
             for (int a = 0; a < 2; ++a)
               for (int i = 0; i < 3; ++i)
                 for (int j = 0; j < 3; ++j) V[3 * i + j] += F(fJp + 6 * v + 3 * a + i, p) * F(fJp + 6 * v + 3 * a + j, p);
-          for (int i = 0; i < 3; ++i) V[4 * i] += fmin(fmax(F(fD + i, p), 1e-6), 1e32) / radius;
+          for (int i = 0; i < 3; ++i) V[4 * i] += fmin(fmax(F(fD + i, p), 1e-6), 1e32) / lm.radius;
           const double c00 = V[4] * V[8] - V[5] * V[7], c01 = V[5] * V[6] - V[3] * V[8], c02 = V[3] * V[7] - V[4] * V[6];
           const double det = V[0] * c00 + V[1] * c01 + V[2] * c02;
           double Vi[9];
@@ -368,38 +341,14 @@ __global__ void __launch_bounds__(kBThreads) k_relpose_ba(const RpPair* __restri
           }
           double* bb = S.rhs;
           for (int j = 0; j < 12; ++j) bb[j] = -S.g[j] + S.sums[78 + j];
-          int pd = 1;
-          for (int j = 0; j < 12 && pd; ++j) {
-            double d = A[12 * j + j];
-            for (int t = 0; t < j; ++t) d -= A[12 * j + t] * A[12 * j + t];
-            if (!(d > 0.0)) { pd = 0; break; }
-            d = sqrt(d);
-            A[12 * j + j] = d;
-            for (int i = j + 1; i < 12; ++i) {
-              double s = A[12 * i + j];
-              for (int t = 0; t < j; ++t) s -= A[12 * i + t] * A[12 * j + t];
-              A[12 * i + j] = s / d;
-            }
-          }
-          if (pd) {
-            for (int i = 0; i < 12; ++i) {
-              double s = bb[i];
-              for (int t = 0; t < i; ++t) s -= A[12 * i + t] * bb[t];
-              bb[i] = s / A[12 * i + i];
-            }
-            for (int i = 11; i >= 0; --i) {
-              double s = bb[i];
-              for (int t = i + 1; t < 12; ++t) s -= A[12 * t + i] * bb[t];
-              bb[i] = s / A[12 * i + i];
-            }
+          S.pd = chol_solve_small<12>(A, bb);
+          if (S.pd)
             for (int j = 0; j < 12; ++j) S.delta[j] = bb[j];
-          }
-          S.pd = pd;
         }
         __syncthreads();
-        bool step_ok = S.pd != 0;
+        const bool pd = S.pd != 0;
         double model_cost_change = 0.0;
-        if (step_ok) {
+        if (pd) {
           // back substitution delta_p = V^-1 (-g_p - W^T delta_B) and the model cost change 1/2 delta^T (D^2 delta - g)
           double acc = 0.0;
           for (uint32_t p = tid; p < N; p += kBThreads) {
@@ -413,17 +362,16 @@ __global__ void __launch_bounds__(kBThreads) k_relpose_ba(const RpPair* __restri
             for (int i = 0; i < 3; ++i) {
               const double d = F(fVi + 3 * i, p) * t3[0] + F(fVi + 3 * i + 1, p) * t3[1] + F(fVi + 3 * i + 2, p) * t3[2];
               F(fDel + i, p) = d;
-              acc += d * ((fmin(fmax(F(fD + i, p), 1e-6), 1e32) / radius) * d - F(fG + i, p));
+              acc += d * ((fmin(fmax(F(fD + i, p), 1e-6), 1e32) / lm.radius) * d - F(fG + i, p));
             }
           }
-          acc = block_sum(acc, S.red);
+          acc = block_sum_fixed<kBThreads>(acc, S.red);
           double cam = 0.0;
           for (int j = 0; j < 12; ++j) cam += S.delta[j] * (S.D2[j] * S.delta[j] - S.g[j]);
           model_cost_change = 0.5 * (cam + acc);
-          step_ok = model_cost_change > 0.0;
         }
         bool accepted = false;
-        if (step_ok) {
+        if (lm.step_usable(pd, model_cost_change)) {
           // trial point and the parameter tolerance on the unscaled step
           double dn = 0.0, xn = 0.0;
           for (uint32_t p = tid; p < N; p += kBThreads)
@@ -433,8 +381,8 @@ __global__ void __launch_bounds__(kBThreads) k_relpose_ba(const RpPair* __restri
               dn += d * d;
               xn += x * x;
             }
-          dn = block_sum(dn, S.red);
-          xn = block_sum(xn, S.red);
+          dn = block_sum_fixed<kBThreads>(dn, S.red);
+          xn = block_sum_fixed<kBThreads>(xn, S.red);
           for (int j = 0; j < 12; ++j) {
             const double d = S.delta[j] * S.scale[j];
             dn += d * d;
@@ -442,44 +390,27 @@ __global__ void __launch_bounds__(kBThreads) k_relpose_ba(const RpPair* __restri
           }
           if (tid < 12) S.pose_new[tid] = S.pose[tid] + S.delta[tid] * S.scale[tid];
           __syncthreads();
-          if (sqrt(dn) <= prm.parameter_tolerance * (sqrt(xn) + prm.parameter_tolerance)) {
-            termination = 3;
-            break;
-          }
+          if (lm.step_too_small(dn, xn)) break;
           const double new_cost = total_cost(S.pose_new, cur ^ 1);
-          const double relative_decrease = (cost - new_cost) / model_cost_change;
-          if (relative_decrease > 1e-3) {
-            accepted = true;
+          if ((accepted = lm.accept(cost, new_cost, model_cost_change))) {
             cur ^= 1;
             __syncthreads();
             if (tid < 12) S.pose[tid] = S.pose_new[tid];
-            const double cost_change = cost - new_cost;
-            const double t = 2.0 * relative_decrease - 1.0;
-            radius = radius / fmax(1.0 / 3.0, 1.0 - t * t * t);
-            radius = fmin(1e16, radius);
-            decrease_factor = 2.0;
-            ++successful;
-            const bool ftol = fabs(cost_change) < prm.function_tolerance * cost;
             cost = new_cost;
             __syncthreads();
             evaluate(false);
-            if (ftol) { termination = 1; break; }
-            if (grad_max() <= prm.gradient_tolerance) { termination = 2; break; }
+            if (lm.converged(grad_max())) break;
           }
         }
-        if (!accepted) {
-          radius = radius / decrease_factor;
-          decrease_factor *= 2.0;
-          if (radius < 1e-32) { termination = 4; break; }
-        }
+        if (!accepted && lm.reject()) break;
         __syncthreads();
       }
     __syncthreads();
     if (tid < 12) io[pid].pose[tid] = S.pose[tid];
     if (tid == 0) {
-      io[pid].iterations = iterations;
-      io[pid].successful = successful;
-      io[pid].termination = termination;
+      io[pid].iterations = lm.iterations;
+      io[pid].successful = lm.successful;
+      io[pid].termination = lm.termination;
       io[pid].initial_cost = initial_cost;
       io[pid].final_cost = cost;
     }
@@ -621,7 +552,7 @@ int relpose_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_matches* m, const r3d
     }
     std::vector<uint32_t> order(ok);
     std::stable_sort(order.begin(), order.end(), [&](uint32_t x, uint32_t y) { return hp[x].M > hp[y].M; });
-    // grid: one CTA per SM (the kernel needs ~250 registers per thread), fewer when the per-CTA scratch slots would pass
+    // grid: one CTA per SM (the kernel needs ~170 registers per thread), fewer when the per-CTA scratch slots would pass
     // 4 GB
     const size_t slot = (size_t)kFields * cap * sizeof(double);
     uint32_t grid = std::min<uint32_t>((uint32_t)order.size(), (uint32_t)w.sm_count);
@@ -637,15 +568,8 @@ int relpose_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_matches* m, const r3d
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_ba.p, hba.data(), nc * sizeof(RpBa), cudaMemcpyHostToDevice, w.stream));
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_order.p, order.data(), order.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, w.stream));
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_work.p, 0, sizeof(uint32_t), w.stream));
-    RpBaParams prm;
-    prm.max_iterations = opt.ba.max_iterations;
-    prm.huber_a = opt.ba.huber_a;
-    prm.function_tolerance = opt.ba.function_tolerance;
-    prm.gradient_tolerance = opt.ba.gradient_tolerance;
-    prm.parameter_tolerance = opt.ba.parameter_tolerance;
-    prm.initial_radius = opt.ba.initial_radius;
     R3D_CUDA_TRY(ctx, cudaEventRecord(ev[2], w.stream));
-    k_relpose_ba<<<grid, kBThreads, 0, w.stream>>>(d_pairs.p, d_order.p, (uint32_t)order.size(), d_work.p, d_a1.p, d_a2.p, d_ba.p, prm,
+    k_relpose_ba<<<grid, kBThreads, 0, w.stream>>>(d_pairs.p, d_order.p, (uint32_t)order.size(), d_work.p, d_a1.p, d_a2.p, d_ba.p, lm_params(opt.ba),
                                                    d_scr.p, cap);
     R3D_CUDA_TRY(ctx, cudaGetLastError());
     R3D_CUDA_TRY(ctx, cudaEventRecord(ev[3], w.stream));

@@ -176,9 +176,10 @@ R3D_RP_HD void projective(const double* K, const double* R, const double* t, dou
   P[11] = t[2];
 }
 
-// ceres::RotationMatrixToAngleAxis (RotationMatrixToQuaternion + QuaternionToAngleAxis), R row-major.  Host only in
-// the library: the BA's initial pose is converted where the oracle converts it, with the same libm.
-inline void rotation_to_angle_axis(const double* R, double* aa) {
+// ceres::RotationMatrixToAngleAxis (RotationMatrixToQuaternion + QuaternionToAngleAxis), R row-major.  The two-view
+// BA's initial pose is converted on the host, where the oracle converts it, with the same libm; the pose refinement
+// of resection.cu converts on the device.
+R3D_RP_HD void rotation_to_angle_axis(const double* R, double* aa) {
   double q[4];
   const double trace = R[0] + R[4] + R[8];
   if (trace >= 0.0) {

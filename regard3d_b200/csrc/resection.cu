@@ -18,7 +18,9 @@
 #include "acransac_rng.cuh"
 #include "ba_model.cuh"
 #include "detmath.cuh"
+#include "lm_trust_region.cuh"
 #include "p3p.cuh"
+#include "relpose_math.cuh"
 #include "r3d_sfm.h"
 
 #include <algorithm>
@@ -51,11 +53,6 @@ struct RsLm {              // refinement result
   double initial_cost, final_cost;
 };
 
-struct RsLmParams {
-  uint32_t max_iterations;
-  double huber_a, function_tolerance, gradient_tolerance, parameter_tolerance, initial_radius;
-};
-
 // [R | t] of P = K [R | t], K = [f 0 ppx; 0 f ppy; 0 0 1]
 __host__ __device__ inline void pose_from_projective(const double* K, const double* P, double* R, double* t) {
   for (int j = 0; j < 3; ++j) {
@@ -66,39 +63,6 @@ __host__ __device__ inline void pose_from_projective(const double* K, const doub
   t[2] = P[11];
   t[0] = (P[3] - K[1] * P[11]) / K[0];
   t[1] = (P[7] - K[2] * P[11]) / K[0];
-}
-
-// ceres::RotationMatrixToAngleAxis (through the quaternion), R row-major
-__host__ __device__ inline void rotation_to_angle_axis(const double* R, double* aa) {
-  double q[4];
-  const double trace = R[0] + R[4] + R[8];
-  if (trace >= 0.0) {
-    double t = sqrt(trace + 1.0);
-    q[0] = 0.5 * t;
-    t = 0.5 / t;
-    q[1] = (R[7] - R[5]) * t;
-    q[2] = (R[2] - R[6]) * t;
-    q[3] = (R[3] - R[1]) * t;
-  } else {
-    int i = 0;
-    if (R[4] > R[0]) i = 1;
-    if (R[8] > R[4 * i]) i = 2;
-    const int j = (i + 1) % 3, k = (j + 1) % 3;
-    double t = sqrt(R[4 * i] - R[4 * j] - R[4 * k] + 1.0);
-    q[i + 1] = 0.5 * t;
-    t = 0.5 / t;
-    q[0] = (R[3 * k + j] - R[3 * j + k]) * t;
-    q[j + 1] = (R[3 * j + i] + R[3 * i + j]) * t;
-    q[k + 1] = (R[3 * k + i] + R[3 * i + k]) * t;
-  }
-  const double s2 = q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
-  double k = 2.0;
-  if (s2 > 0.0) {
-    const double st = sqrt(s2), ct = q[0];
-    const double two_theta = 2.0 * (ct < 0.0 ? atan2(-st, -ct) : atan2(st, ct));
-    k = two_theta / st;
-  }
-  for (int i = 0; i < 3; ++i) aa[i] = q[i + 1] * k;
 }
 
 // ---- 1. undistortion and the AC-RANSAC point layout ------------------------------------------------------------------
@@ -159,7 +123,7 @@ __global__ void __launch_bounds__(kRThreads) k_resect_refine(const RsView* __res
                                                              const AcFusedOut* __restrict__ fo, const double* __restrict__ models,
                                                              const uint2* __restrict__ inl, const double2* __restrict__ x1,
                                                              const double* __restrict__ x3, const double2* __restrict__ xo,
-                                                             RsLm* __restrict__ out, RsLmParams prm) {
+                                                             RsLm* __restrict__ out, LmParams prm) {
   __shared__ RefineSmem S;
   const uint32_t tid = threadIdx.x;
   for (;;) {
@@ -175,7 +139,7 @@ __global__ void __launch_bounds__(kRThreads) k_resect_refine(const RsView* __res
       S.view = views[a];
       double R[9], t[3];
       pose_from_projective(S.view.intr, models + 12 * (size_t)a, R, t);
-      rotation_to_angle_axis(R, S.pose);
+      rp::rotation_to_angle_axis(R, S.pose);
       for (int i = 0; i < 3; ++i) S.pose[3 + i] = t[i];
     }
     __syncthreads();
@@ -256,61 +220,33 @@ __global__ void __launch_bounds__(kRThreads) k_resect_refine(const RsView* __res
 
     double cost = total_cost(S.pose);
     const double initial_cost = cost;
-    uint32_t iterations = 0, successful = 0;
-    int termination = 0;
-    double radius = prm.initial_radius, decrease_factor = 2.0;
+    LmTrustRegion lm(prm);  // every thread keeps its own: the inputs are block-wide, so are the decisions
     evaluate(true);
-    if (grad_max() <= prm.gradient_tolerance) termination = 2;
-    else
+    if (!lm.start(grad_max()))
       for (uint32_t iter = 1; iter <= prm.max_iterations; ++iter) {
-        iterations = iter;
+        lm.iterations = iter;
         __syncthreads();
         if (tid == 0) {  // LevenbergMarquardtStrategy: (H + D^2) delta = -g, D^2 = clamp(diag, 1e-6, 1e32) / radius
           double A[36], b[6];
-          for (int j = 0; j < 6; ++j) S.D2[j] = fmin(fmax(S.diag[j], 1e-6), 1e32) / radius;
+          for (int j = 0; j < 6; ++j) S.D2[j] = fmin(fmax(S.diag[j], 1e-6), 1e32) / lm.radius;
           for (int i = 0; i < 6; ++i) {
             for (int j = 0; j <= i; ++j) A[6 * i + j] = S.H[6 * i + j] + (i == j ? S.D2[i] : 0.0);
             b[i] = -S.g[i];
           }
-          int pd = 1;
-          for (int j = 0; j < 6 && pd; ++j) {
-            double d = A[6 * j + j];
-            for (int t = 0; t < j; ++t) d -= A[6 * j + t] * A[6 * j + t];
-            if (!(d > 0.0)) { pd = 0; break; }
-            d = sqrt(d);
-            A[6 * j + j] = d;
-            for (int i = j + 1; i < 6; ++i) {
-              double s = A[6 * i + j];
-              for (int t = 0; t < j; ++t) s -= A[6 * i + t] * A[6 * j + t];
-              A[6 * i + j] = s / d;
-            }
-          }
-          if (pd) {
-            for (int i = 0; i < 6; ++i) {
-              double s = b[i];
-              for (int t = 0; t < i; ++t) s -= A[6 * i + t] * b[t];
-              b[i] = s / A[6 * i + i];
-            }
-            for (int i = 5; i >= 0; --i) {
-              double s = b[i];
-              for (int t = i + 1; t < 6; ++t) s -= A[6 * t + i] * b[t];
-              b[i] = s / A[6 * i + i];
-            }
+          S.pd = chol_solve_small<6>(A, b);
+          if (S.pd)
             for (int j = 0; j < 6; ++j) S.delta[j] = b[j];
-          }
-          S.pd = pd;
         }
         __syncthreads();
-        bool step_ok = S.pd != 0;
+        const bool pd = S.pd != 0;
         double model_cost_change = 0.0;
-        if (step_ok) {
+        if (pd) {
           double m = 0.0;
           for (int j = 0; j < 6; ++j) m += S.delta[j] * (S.D2[j] * S.delta[j] - S.g[j]);
           model_cost_change = 0.5 * m;
-          step_ok = model_cost_change > 0.0;
         }
         bool accepted = false;
-        if (step_ok) {
+        if (lm.step_usable(pd, model_cost_change)) {
           double dn = 0.0, xn = 0.0;
           for (int j = 0; j < 6; ++j) {
             const double d = S.delta[j] * S.scale[j];
@@ -319,42 +255,25 @@ __global__ void __launch_bounds__(kRThreads) k_resect_refine(const RsView* __res
           }
           if (tid < 6) S.pose_new[tid] = S.pose[tid] + S.delta[tid] * S.scale[tid];
           __syncthreads();
-          if (sqrt(dn) <= prm.parameter_tolerance * (sqrt(xn) + prm.parameter_tolerance)) {
-            termination = 3;
-            break;
-          }
+          if (lm.step_too_small(dn, xn)) break;
           const double new_cost = total_cost(S.pose_new);
-          const double relative_decrease = (cost - new_cost) / model_cost_change;
-          if (relative_decrease > 1e-3) {
-            accepted = true;
+          if ((accepted = lm.accept(cost, new_cost, model_cost_change))) {
             if (tid < 6) S.pose[tid] = S.pose_new[tid];
-            const double cost_change = cost - new_cost;
-            const double t = 2.0 * relative_decrease - 1.0;
-            radius = radius / fmax(1.0 / 3.0, 1.0 - t * t * t);
-            radius = fmin(1e16, radius);
-            decrease_factor = 2.0;
-            ++successful;
-            const bool ftol = fabs(cost_change) < prm.function_tolerance * cost;
             cost = new_cost;
             __syncthreads();
             evaluate(false);
-            if (ftol) { termination = 1; break; }
-            if (grad_max() <= prm.gradient_tolerance) { termination = 2; break; }
+            if (lm.converged(grad_max())) break;
           }
         }
-        if (!accepted) {
-          radius = radius / decrease_factor;
-          decrease_factor *= 2.0;
-          if (radius < 1e-32) { termination = 4; break; }
-        }
+        if (!accepted && lm.reject()) break;
       }
     __syncthreads();
     if (tid == 0) {
       RsLm o;
       for (int k = 0; k < 6; ++k) o.pose[k] = S.pose[k];
-      o.iterations = iterations;
-      o.successful = successful;
-      o.termination = termination;
+      o.iterations = lm.iterations;
+      o.successful = lm.successful;
+      o.termination = lm.termination;
       o.pad_ = 0;
       o.initial_cost = initial_cost;
       o.final_cost = cost;
@@ -541,16 +460,9 @@ int resect_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_resection_view* views,
   }
   R3D_CUDA_TRY(ctx, cudaEventRecord(ev[1], w.stream));
   if (opt.refine) {
-    RsLmParams prm;
-    prm.max_iterations = opt.ba.max_iterations;
-    prm.huber_a = opt.ba.huber_a;
-    prm.function_tolerance = opt.ba.function_tolerance;
-    prm.gradient_tolerance = opt.ba.gradient_tolerance;
-    prm.parameter_tolerance = opt.ba.parameter_tolerance;
-    prm.initial_radius = opt.ba.initial_radius;
     const uint32_t grid = std::min<uint32_t>(n, (uint32_t)w.sm_count);
     k_resect_refine<<<grid, kRThreads, 0, w.stream>>>(d_views.p, d_lm_order.p, n, d_work.p + kClasses, d_out.p, d_model.p, d_outm.p,
-                                                      d_x1.p, d_x3.p, d_xo.p, d_lm.p, prm);
+                                                      d_x1.p, d_x3.p, d_xo.p, d_lm.p, lm_params(opt.ba));
     R3D_CUDA_TRY(ctx, cudaGetLastError());
     T.kernel_launches += 1;
   }

@@ -15,7 +15,7 @@
 //      (ba.cu), block inverse iteration with 3 right-hand sides (k_rotavg_trsm3: blocked forward / backward
 //      substitution, one cooperative launch) and a 3 x 3 Cholesky-QR (k_rotavg_orth), then the sign, the SO(3)
 //      projection of every 3 x 3 block (relpose_math.cuh's Jacobi SVD) and the gauge (k_rotavg_project).
-//   4. refinement: the Levenberg-Marquardt state machine of r3d_bundle_adjust on the angle-axis of every kept view,
+//   4. refinement: Levenberg-Marquardt (lm_trust_region.cuh's trust region) on the angle-axis of every kept view,
 //      residual log(R_ij^T R_j R_i^T) with forward-mode duals, dense normal equations by one owner per block row (no
 //      floating-point atomics), k_chol_fused, fixed-order reductions: repeated calls are bit-identical.
 #include "r3d_internal.cuh"
@@ -540,35 +540,6 @@ __global__ void __launch_bounds__(128) k_rotavg_normal(int mode, const uint32_t*
   }
 }
 
-// the LM step: out[0] = 1/2 delta^T (D^2 delta - g), out[1] = |scaled-back step|^2, out[2] = |x|^2, aa_new = aa + step;
-// out[3] = max |g / scale| (the unscaled gradient), computed from the current g
-__global__ void __launch_bounds__(kOThreads) k_rotavg_step(const double* __restrict__ delta, const double* __restrict__ g,
-                                                           const double* __restrict__ diag, const double* __restrict__ scale,
-                                                           const double* __restrict__ aa, uint32_t N, double inv_radius,
-                                                           double* __restrict__ aa_new, double* __restrict__ out) {
-  __shared__ double red[kOThreads / 32];
-  double mcc = 0.0, dn = 0.0, xn = 0.0, gm = 0.0;
-  for (uint32_t j = threadIdx.x; j < N; j += kOThreads) {
-    const double d2 = fmin(fmax(diag[j], 1e-6), 1e32) * inv_radius;
-    mcc += delta[j] * (d2 * delta[j] - g[j]);
-    const double d = delta[j] * scale[j];
-    aa_new[j] = aa[j] + d;
-    dn += d * d;
-    xn += aa[j] * aa[j];
-    gm = fmax(gm, fabs(g[j] / scale[j]));
-  }
-  mcc = block_sum_fixed<kOThreads>(mcc, red);
-  dn = block_sum_fixed<kOThreads>(dn, red);
-  xn = block_sum_fixed<kOThreads>(xn, red);
-  gm = block_max_fixed<kOThreads>(gm, red);
-  if (threadIdx.x == 0) {
-    out[0] = 0.5 * mcc;
-    out[1] = dn;
-    out[2] = xn;
-    out[3] = gm;
-  }
-}
-
 // ---- host ---------------------------------------------------------------------------------------------------------
 // cooperative grid of k_rotavg_trsm3: grid 0 = up to 4 CTAs per SM as occupancy allows (what the inverse iteration
 // runs), otherwise the caller's, R3D_ERR_INVALID when that many CTAs cannot be co-resident
@@ -877,8 +848,7 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
       return fail(ctx, R3D_ERR_NOMEM, "r3d_rotation_averaging: device scratch");
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_aa.p, aa.data(), N * sizeof(double), cudaMemcpyHostToDevice, w.stream));
     R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[4], w.stream));
-    const r3d_ba_options& lm = opt.lm;
-    const double ha = lm.huber_a;
+    const double ha = opt.lm.huber_a;
     const uint32_t eg = (ne + 127) / 128;
     double* cur = d_aa.p;
     double* trial = d_aan.p;
@@ -904,7 +874,8 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
                                                nullptr);
       // the step kernel with a zero step and radius reports max |g / scale| in scal[3]
       R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_x.p, 0, N * sizeof(double), w.stream));
-      k_rotavg_step<<<1, kOThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, (uint32_t)N, 0.0, trial, d_scal.p);
+      k_avg_step<kOThreads><<<1, kOThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, (uint32_t)N, (uint32_t)N, 0.0, trial,
+                                                           d_scal.p);
       R3D_CUDA_TRY(ctx, cudaGetLastError());
       int r2;
       if ((r2 = read_scal())) return r2;
@@ -917,55 +888,40 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
     S.lm_iterations = 0;
     S.lm_successful_steps = 0;
     S.lm_termination = 0;
-    double radius = lm.initial_radius, decrease_factor = 2.0;
+    LmTrustRegion lm(lm_params(opt.lm));
     if ((rc = evaluate())) return rc;
-    bool stop = gmax <= lm.gradient_tolerance;
-    if (stop) S.lm_termination = 2;
-    for (uint32_t iter = 1; !stop && iter <= lm.max_iterations; ++iter) {
-      S.lm_iterations = iter;
-      const double inv_radius = 1.0 / radius;
+    const bool stop = lm.start(gmax);
+    for (uint32_t iter = 1; !stop && iter <= lm.p.max_iterations; ++iter) {
+      lm.iterations = iter;
+      const double inv_radius = 1.0 / lm.radius;
       R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_A.p, 0, (size_t)(N + 1) * N * sizeof(double), w.stream));
       R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_scal.p + 7, 0, sizeof(double), w.stream));
       k_rotavg_normal<<<m, 128, 0, w.stream>>>(2, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_res.p, d_jac.p, m, d_scale.p, d_g.p, d_diag.p,
                                                inv_radius, d_A.p);
       R3D_CUDA_TRY(ctx, cudaGetLastError());
       if ((rc = dense_cholesky(ctx, w, d_A.p, d_L.p, d_Linv.p, N, d_scal.p + 7, d_x.p))) return rc;
-      k_rotavg_step<<<1, kOThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, (uint32_t)N, inv_radius, trial, d_scal.p);
+      k_avg_step<kOThreads><<<1, kOThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, (uint32_t)N, (uint32_t)N, inv_radius,
+                                                           trial, d_scal.p);
       R3D_CUDA_TRY(ctx, cudaGetLastError());
       if ((rc = read_scal())) return rc;
-      const bool pd = scal[7] == 0.0;
       const double model_cost_change = scal[0];
       bool accepted = false;
-      if (pd && model_cost_change > 0.0 && std::isfinite(model_cost_change)) {
-        if (std::sqrt(scal[1]) <= lm.parameter_tolerance * (std::sqrt(scal[2]) + lm.parameter_tolerance)) {
-          S.lm_termination = 3;
-          break;
-        }
+      if (lm.step_usable(scal[7] == 0.0, model_cost_change)) {
+        if (lm.step_too_small(scal[1], scal[2])) break;
         double new_cost = 0.0;
         if ((rc = eval_cost(trial, &new_cost))) return rc;
-        const double relative_decrease = (cost - new_cost) / model_cost_change;
-        if (relative_decrease > 1e-3) {
-          accepted = true;
+        if ((accepted = lm.accept(cost, new_cost, model_cost_change))) {
           std::swap(cur, trial);
-          const double cost_change = cost - new_cost;
-          const double t = 2.0 * relative_decrease - 1.0;
-          radius = radius / std::max(1.0 / 3.0, 1.0 - t * t * t);
-          radius = std::min(1e16, radius);
-          decrease_factor = 2.0;
-          S.lm_successful_steps++;
-          const bool ftol = std::fabs(cost_change) < lm.function_tolerance * cost;
           cost = new_cost;
           if ((rc = evaluate())) return rc;
-          if (ftol) { S.lm_termination = 1; break; }
-          if (gmax <= lm.gradient_tolerance) { S.lm_termination = 2; break; }
+          if (lm.converged(gmax)) break;
         }
       }
-      if (!accepted) {
-        radius = radius / decrease_factor;
-        decrease_factor *= 2.0;
-        if (radius < 1e-32) { S.lm_termination = 4; break; }
-      }
+      if (!accepted && lm.reject()) break;
     }
+    S.lm_iterations = lm.iterations;
+    S.lm_successful_steps = lm.successful;
+    S.lm_termination = lm.termination;
     S.lm_final_cost = cost;
     R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[5], w.stream));
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(aa.data(), cur, N * sizeof(double), cudaMemcpyDeviceToHost, w.stream));

@@ -6,12 +6,12 @@
 // Replaces GlobalSfM_Translation_AveragingSolver::Translation_averaging (OpenMVG 1.4, SURVEY.md A.11) for
 // TRANSLATION_AVERAGING_L2_DISTANCE_CHORDAL and TRANSLATION_AVERAGING_SOFTL1, on the pairwise relative translations:
 //   1. host: the usable edges, the largest bi-edge-connected component (rotavg.cu's Tarjan), reindexing by view id.
-//   2. Levenberg-Marquardt (the state machine of r3d_bundle_adjust / rotation averaging), the lowest kept view held:
+//   2. Levenberg-Marquardt (lm_trust_region.cuh's trust region), the lowest kept view held:
 //      k_ta_eval (one thread per edge, forward-mode duals: residual, 3 x 7 Jacobian, soft-L1 corrector),
 //      k_ta_view (one owner CTA per view block row: Jacobi scale, gradient, J^T J + D^2 with each edge's scale
 //      eliminated in the same pass -- no floating-point atomics), k_chol_fused (ba.cu) on the 3(m-1) reduced system,
-//      k_ta_back (the scale steps; a scale on its bound pushed outwards is held), k_ta_step (clamp s >= 1, model cost change, norms, projected gradient; fixed-order
-//      reductions).  Repeated calls are bit-identical.
+//      k_ta_back (the scale steps; a scale on its bound pushed outwards is held), k_avg_step (averaging.cuh; clamp
+//      s >= 1, model cost change, norms, projected gradient; fixed-order reductions).  Repeated calls are bit-identical.
 #include "r3d_internal.cuh"
 #include "averaging.cuh"
 #include "relpose_math.cuh"
@@ -23,8 +23,6 @@
 namespace r3d {
 namespace ta {
 
-using ra::block_max_fixed;
-using ra::block_sum_fixed;
 using ra::DevArr;
 
 constexpr int kChordal = 2;  // R3D_TRANSAVG_L2_CHORDAL
@@ -313,45 +311,6 @@ __global__ void k_ta_back(const uint2* __restrict__ ab, const double* __restrict
   delta[N + e] = -acc / V;
 }
 
-// the LM step over the Nv variables (views, then scales from index nb on, bounded below by 1): out[0] = 1/2 delta^T
-// (D^2 delta - g) with the unclamped delta, out[1] = |x_new - x|^2 with x_new = Plus(x, scaled-back delta) (clamped),
-// out[2] = |x|^2, out[3] = max |x - Plus(x, -g / scale)| (the projected unscaled gradient, from the current g)
-__global__ void __launch_bounds__(kRThreads) k_ta_step(const double* __restrict__ delta, const double* __restrict__ g,
-                                                       const double* __restrict__ diag, const double* __restrict__ scale,
-                                                       const double* __restrict__ x, uint32_t Nv, uint32_t nb, double inv_radius,
-                                                       double* __restrict__ x_new, double* __restrict__ out) {
-  __shared__ double red[kRThreads / 32];
-  double mcc = 0.0, dn = 0.0, xn = 0.0, gm = 0.0;
-  for (uint32_t j = threadIdx.x; j < Nv; j += kRThreads) {
-    const double d2 = fmin(fmax(diag[j], 1e-6), 1e32) * inv_radius;
-    mcc += delta[j] * (d2 * delta[j] - g[j]);
-    const double d = delta[j] * scale[j];
-    const double xj = x[j];
-    const double gt = g[j] / scale[j];
-    if (j < nb) {
-      x_new[j] = xj + d;
-      dn += d * d;
-      gm = fmax(gm, fabs(gt));
-    } else {
-      const double xc = fmax(xj + d, 1.0);
-      x_new[j] = xc;
-      dn += (xc - xj) * (xc - xj);
-      gm = fmax(gm, fabs(xj - fmax(xj - gt, 1.0)));
-    }
-    xn += xj * xj;
-  }
-  mcc = block_sum_fixed<kRThreads>(mcc, red);
-  dn = block_sum_fixed<kRThreads>(dn, red);
-  xn = block_sum_fixed<kRThreads>(xn, red);
-  gm = block_max_fixed<kRThreads>(gm, red);
-  if (threadIdx.x == 0) {
-    out[0] = 0.5 * mcc;
-    out[1] = dn;
-    out[2] = xn;
-    out[3] = gm;
-  }
-}
-
 // the chordal start (the oracle draws the same numbers): a splitmix64 stream of its own, uniform in [0, 1)
 double start_value(uint64_t k) {
   uint64_t z = k * 0x9E3779B97F4A7C15ull + 0x6A09E667F3BCC909ull;
@@ -485,11 +444,11 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
     R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
     return R3D_OK;
   };
-  const r3d_ba_options& lm = opt.lm;
+  LmParams prm = lm_params(opt.lm);
+  if (prm.max_iterations == 0) prm.max_iterations = softl1 ? std::max<uint32_t>(50, 2 * ne) : 500u;
+  if (!(prm.function_tolerance > 0.0)) prm.function_tolerance = softl1 ? 1e-6 : 1e-7;
   const double la = opt.softl1_loss;
   const uint32_t eg = (ne + 127) / 128;
-  const uint32_t max_iterations = lm.max_iterations > 0 ? lm.max_iterations : (softl1 ? std::max<uint32_t>(50, 2 * ne) : 500u);
-  const double function_tolerance = lm.function_tolerance > 0.0 ? lm.function_tolerance : (softl1 ? 1e-6 : 1e-7);
   double* cur = d_cur.p;
   double* trial = d_trial.p;
   auto eval_cost = [&](const double* xx, double* out) -> int {
@@ -518,7 +477,8 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
     if (softl1) k_ta_edge<<<eg, 128, 0, w.stream>>>(1, d_res.p, d_jac.p, ne, (uint32_t)N, d_scale.p, d_g.p, d_diag.p);
     // the step kernel with a zero step and radius reports the projected gradient in scal[3]
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_x.p, 0, Nv * sizeof(double), w.stream));
-    k_ta_step<<<1, kRThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, Nv, (uint32_t)N, 0.0, trial, d_scal.p);
+    ra::k_avg_step<kRThreads><<<1, kRThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, Nv, (uint32_t)N, 0.0, trial,
+                                                            d_scal.p);
     R3D_CUDA_TRY(ctx, cudaGetLastError());
     int r2;
     if ((r2 = read_scal())) return r2;
@@ -529,16 +489,12 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
   double cost = 0.0;
   if ((rc = eval_cost(cur, &cost))) return rc;
   S.lm_initial_cost = cost;
-  S.lm_iterations = 0;
-  S.lm_successful_steps = 0;
-  S.lm_termination = 0;
-  double radius = lm.initial_radius, decrease_factor = 2.0;
+  LmTrustRegion lm(prm);
   if ((rc = evaluate())) return rc;
-  bool stop = gmax <= lm.gradient_tolerance;
-  if (stop) S.lm_termination = 2;
-  for (uint32_t iter = 1; !stop && iter <= max_iterations; ++iter) {
-    S.lm_iterations = iter;
-    const double inv_radius = 1.0 / radius;
+  const bool stop = lm.start(gmax);
+  for (uint32_t iter = 1; !stop && iter <= prm.max_iterations; ++iter) {
+    lm.iterations = iter;
+    const double inv_radius = 1.0 / lm.radius;
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_A.p, 0, (size_t)(N + 1) * N * sizeof(double), w.stream));
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_scal.p + 7, 0, sizeof(double), w.stream));
     k_ta_view<<<m - 1, 128, 0, w.stream>>>(2, softl1, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_res.p, d_jac.p, cur, (uint32_t)N, d_scale.p,
@@ -546,42 +502,28 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
     R3D_CUDA_TRY(ctx, cudaGetLastError());
     if ((rc = dense_cholesky(ctx, w, d_A.p, d_L.p, d_Linv.p, N, d_scal.p + 7, d_x.p))) return rc;
     if (softl1) k_ta_back<<<eg, 128, 0, w.stream>>>(d_ab.p, d_jac.p, cur, d_scale.p, d_g.p, ne, (uint32_t)N, inv_radius, d_x.p);
-    k_ta_step<<<1, kRThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, Nv, (uint32_t)N, inv_radius, trial, d_scal.p);
+    ra::k_avg_step<kRThreads><<<1, kRThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, Nv, (uint32_t)N, inv_radius, trial,
+                                                            d_scal.p);
     R3D_CUDA_TRY(ctx, cudaGetLastError());
     if ((rc = read_scal())) return rc;
-    const bool pd = scal[7] == 0.0;
     const double model_cost_change = scal[0];
     bool accepted = false;
-    if (pd && model_cost_change > 0.0 && std::isfinite(model_cost_change)) {
-      if (std::sqrt(scal[1]) <= lm.parameter_tolerance * (std::sqrt(scal[2]) + lm.parameter_tolerance)) {
-        S.lm_termination = 3;
-        break;
-      }
+    if (lm.step_usable(scal[7] == 0.0, model_cost_change)) {
+      if (lm.step_too_small(scal[1], scal[2])) break;
       double new_cost = 0.0;
       if ((rc = eval_cost(trial, &new_cost))) return rc;
-      const double relative_decrease = (cost - new_cost) / model_cost_change;
-      if (relative_decrease > 1e-3) {
-        accepted = true;
+      if ((accepted = lm.accept(cost, new_cost, model_cost_change))) {
         std::swap(cur, trial);
-        const double cost_change = cost - new_cost;
-        const double t = 2.0 * relative_decrease - 1.0;
-        radius = radius / std::max(1.0 / 3.0, 1.0 - t * t * t);
-        radius = std::min(1e16, radius);
-        decrease_factor = 2.0;
-        S.lm_successful_steps++;
-        const bool ftol = std::fabs(cost_change) < function_tolerance * cost;
         cost = new_cost;
         if ((rc = evaluate())) return rc;
-        if (ftol) { S.lm_termination = 1; break; }
-        if (gmax <= lm.gradient_tolerance) { S.lm_termination = 2; break; }
+        if (lm.converged(gmax)) break;
       }
     }
-    if (!accepted) {
-      radius = radius / decrease_factor;
-      decrease_factor *= 2.0;
-      if (radius < 1e-32) { S.lm_termination = 4; break; }
-    }
+    if (!accepted && lm.reject()) break;
   }
+  S.lm_iterations = lm.iterations;
+  S.lm_successful_steps = lm.successful;
+  S.lm_termination = lm.termination;
   S.lm_final_cost = cost;
   R3D_CUDA_TRY(ctx, cudaEventRecord(evt.e[1], w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(x.data(), cur, Nv * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
