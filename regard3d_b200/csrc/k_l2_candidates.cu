@@ -18,11 +18,12 @@
 //           then the epilogue.
 //     u8:   4 consumers, so every database tile in shared memory feeds 256 query rows; per 128-row half tile,
 //           m64n128k32 (the K extent fixed at compile time: back-to-back MMAs, no branch) into one 64-register s32
-//           accumulator, then the epilogue of that half.  While one consumer reduces, the other three keep MMAs in the
-//           tensor pipe.  The database map loads every 32-row group with its row pairs transposed (context.cu), so
-//           each lane of a quad holds whole chunks: the chunk minima take no shuffle.  An integer bound taken once per
-//           half from each set's largest key rejects nearly every chunk before its key is formed; the rest are
-//           inserted in warp-uniform rounds.
+//           accumulator.  The chunk minima of a half are taken from the accumulator as soon as its MMAs are done; the
+//           next half's MMAs are issued, and the half's key insertion runs behind them.  The other three consumers
+//           keep MMAs in the tensor pipe too.  The database map loads every 32-row group with its row pairs
+//           transposed (context.cu), so each lane of a quad holds whole chunks: the chunk minima take no shuffle.  An
+//           integer bound taken once per half from each set's largest key rejects nearly every chunk before its key
+//           is formed; the rest are inserted in warp-uniform rounds.
 // Barriers: full[s] (TMA bytes landed), empty[s] (every consumer warp is done with the stage), qfull / qempty the same
 // for the query buffers.
 #include "r3d_internal.cuh"
@@ -242,13 +243,15 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       // and lane per round (FLT_MAX, a no-op of the network, where a lane has none left); a key that passed the bound
       // but is not below the set's largest is a no-op too.  The keys of a set differ in their chunk bits, so the order
       // of the insertions does not change the set.
-      auto reduce = [&](uint32_t t, uint32_t h, uint32_t s0) {
+      // take_minima reads the accumulator and the half's norms; insert reads neither, so it runs while the MMAs of the
+      // next half write the accumulator.
+      int32_t m0[4], m1[4];
+      uint32_t p0, p1;  // bit g: m0[g] / m1[g] is still to be inserted
+      auto take_minima = [&](uint32_t h, uint32_t s0) {
         const int32_t* nrm = (const int32_t*)(smem_raw + (n_base + s0 * kNormBytes - smem_u32(smem_raw))) + h * 128u + 8u * q;
-        const uint32_t chunk0 = t * (kTileN / kChunk) + h * (kTileN / 2 / kChunk) + q;
         const int32_t b0 = bracket_bound(key0[kNumKeys - 1], keep_mask, qn0);
         const int32_t b1 = bracket_bound(key1[kNumKeys - 1], keep_mask, qn1);
-        int32_t m0[4], m1[4];
-        uint32_t p0 = 0, p1 = 0;  // bit g: m0[g] / m1[g] is still to be inserted
+        p0 = p1 = 0;
 #pragma unroll
         for (uint32_t g = 0; g < 4; ++g) {
           const int4 na = *(const int4*)(nrm + kGroupRows * g);
@@ -263,6 +266,9 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
           p0 |= (m0[g] <= b0 ? 1u : 0u) << g;
           p1 |= (m1[g] <= b1 ? 1u : 0u) << g;
         }
+      };
+      auto insert = [&](uint32_t t, uint32_t h) {
+        const uint32_t chunk0 = t * (kTileN / kChunk) + h * (kTileN / 2 / kChunk) + q;
         while (__any_sync(0xffffffffu, (p0 | p1) != 0u)) {
           int32_t y0 = 0, y1 = 0;
           uint32_t g0 = 0, g1 = 0;
@@ -279,26 +285,36 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
           key_insert_packed(x1, key1);
         }
       };
-      // One accumulator: the MMAs of a half, then its epilogue.  The MMAs of the other consumers fill the tensor pipe
-      // meanwhile (a second accumulator would not fit the register budget of four consumers).
-      mbar_wait(bar_qfull + 8 * qb, qf);
-      for (uint32_t t = 0; t < ntiles; ++t) {
-        const uint32_t s_t = stage;
+      // the first stage of the next tile, once all of its K-blocks have landed
+      auto wait_tile = [&]() {
+        const uint32_t s0 = stage;
 #pragma unroll
         for (uint32_t kb = 0; kb < kNkb; ++kb) {
           mbar_wait(bar_full + 8 * stage, phase);
           if (++stage == n_stages) { stage = 0; phase ^= 1u; }
         }
-#pragma unroll
-        for (uint32_t h = 0; h < 2; ++h) {
-          issue(h, s_t);
-          wgmma_wait<0>();
-          wgmma_fence_operand(acc);
-          // every MMA of the item has read the query block
-          if (h == 1 && t + 1 == ntiles && lane == 0) mbar_arrive(bar_qempty + 8 * qb);
-          reduce(t, h, s_t);
-        }
-        // the epilogue has read the tile's norms and the MMAs its operands: hand its stages back to the producer
+        return s0;
+      };
+      auto mma_done = [&]() {
+        wgmma_wait<0>();
+        wgmma_fence_operand(acc);
+      };
+      // One accumulator, and the insertions of each half behind the MMAs of the next: per half, wait for its MMAs, take
+      // its minima, issue the next half's MMAs, then insert.  The halves are unrolled, so each has its own wait.  The
+      // item's last half is inserted with nothing in flight.  take_minima of a half runs after the previous half's
+      // insert, so every bound is taken from the same keys as with no overlap.  Views are padded to whole tiles
+      // (n_pad >= 256), so an item has at least one tile.
+      mbar_wait(bar_qfull + 8 * qb, qf);
+      uint32_t s_t = wait_tile();
+      issue(0, s_t);
+      mma_done();
+      take_minima(0, s_t);
+      for (uint32_t t = 0;; ++t) {
+        issue(1, s_t);
+        insert(t, 0);
+        mma_done();
+        take_minima(1, s_t);
+        // the tile's norms and operands are read: hand its stages back to the producer
         __syncwarp();
         if (lane == 0)
 #pragma unroll
@@ -306,6 +322,17 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
             mbar_arrive(bar_empty + 8 * s);
             if (++s == n_stages) s = 0;
           }
+        if (t + 1 == ntiles) {
+          // every MMA of the item has read the query block
+          if (lane == 0) mbar_arrive(bar_qempty + 8 * qb);
+          insert(t, 1);
+          break;
+        }
+        s_t = wait_tile();
+        issue(0, s_t);
+        insert(t, 1);
+        mma_done();
+        take_minima(0, s_t);
       }
     } else {
       float acc[128];
