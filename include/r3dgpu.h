@@ -580,6 +580,29 @@ int64_t r3d_debug_post_process_ranked(r3d_indmatch* m, int64_t n, const float* x
  * std::uniform_int_distribution<uint32_t> (the ACRANSAC sample stream) reproduces this process's <random>; the
  * filters then run entirely on the device, otherwise samples are drawn on the host, round by round. */
 int r3d_debug_rng_selftest(void);
+/* Diagnostics (device): the AC-RANSAC kernel's scoring of caller-supplied models on one pair, through the device code
+ * the F / H / E filters, r3d_relative_poses and r3d_resect_views run.  model: internal id 0 = F (symmetric epipolar
+ * error, 9 doubles), 1 = H (asymmetric transfer error, 9), 2 = E as F = K2^-T E K1^-1 (one-sided epipolar distance in
+ * pixels, 9), 3 = resection (reprojection error of P = K [R | t], 12 doubles, row-major 3 x 4).  x1, x2: M x 2
+ * (model 3: x1 = X.xy, x2 = the pixel), x3: X.z (model 3 only, NULL otherwise), M >= the model's minimal sample.
+ * max_thr: the squared precision bound (+inf only for model 3); K[6]: the pair's AcPair.K (model 3: K[3] > 0 is where
+ * the tier-1 histogram's top bin starts).  loge0 and the float log-combination tables are built as the filters build
+ * them; the size class (shared-memory or global sort) is the one the filters would pick for M.
+ * Per model, out[m]: lb = the tier-1 lower bound of the best NFA, cnt_hi / cnt_lo = the tier-1 upper / lower count of
+ * the residuals <= max_thr, count = their exact number, nfa / k / err = the tier-2 best NFA, its number of inliers and
+ * the k-th smallest residual.  Optional (may be NULL): lo / hi / e, n_models x M, the tier-1 interval and the tier-2
+ * residual of every (model, point); logc_n (M + 2: log10 C(M, k) for k = 0 .. M, then the table's error bound) and
+ * logc_k (M + 1). */
+typedef struct {
+  double lb, nfa, err;
+  uint32_t cnt_hi, cnt_lo, count, k;
+} r3d_ac_score;
+int r3d_debug_acransac_score(r3d_ctx* ctx, int model, uint32_t M, const double* x1, const double* x2, const double* x3,
+                             double max_thr, double logalpha0, const double* K, const double* models, uint32_t n_models,
+                             r3d_ac_score* out, double* lo, double* hi, double* e, float* logc_n, float* logc_k);
+/* Diagnostics: the library's deterministic transcendental functions (detmath.cuh) on n inputs, on the current CUDA
+ * device (on_device != 0) or in the library's host code.  fn: 0 = log10, 1 = cbrt, 2 = cos, 3 = acos. */
+int r3d_debug_detmath(int fn, int on_device, const double* x, uint64_t n, double* y);
 /* test hook: hash tables of a prepared view (code n x ceil(dim/32), bucket n x 6, bk_ofs 6 x 1025, bk_ids 6 x n) */
 int r3d_debug_cascade_view(r3d_ctx* ctx, uint32_t view_id, uint32_t* code, uint16_t* bucket, uint32_t* bk_ofs, uint32_t* bk_ids);
 

@@ -38,9 +38,14 @@ EXPORTS = [
     "r3d_resection_default_options", "r3d_resect_views", "r3d_sfm_resect_views", "r3d_get_resection_timing",
     "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_matches_keep_largest_biedge_component",
     "r3d_transavg_default_options", "r3d_translation_averaging", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
+    "r3d_debug_acransac_score", "r3d_debug_detmath",
 ]
 
 CHOL_DENSE, CHOL_ENVELOPE = 0, 1
+# r3d_ac_score: one model's scores from r3d_debug_acransac_score
+ac_score_dtype = np.dtype([("lb", np.float64), ("nfa", np.float64), ("err", np.float64), ("cnt_hi", np.uint32),
+                           ("cnt_lo", np.uint32), ("count", np.uint32), ("k", np.uint32)])
+DETMATH_LOG10, DETMATH_CBRT, DETMATH_COS, DETMATH_ACOS = 0, 1, 2, 3
 
 
 class R3DError(RuntimeError):
@@ -617,6 +622,17 @@ def debug_ba_jacobian_model(model, intr, ext, pose, X, obs):
     return r, J
 
 
+def debug_detmath(fn, x, on_device):
+    """r3d_debug_detmath: detmath.cuh's log10 / cbrt / cos / acos (DETMATH_*) of every entry of x, on the current CUDA
+    device or in the library's host code."""
+    x = np.ascontiguousarray(x, np.float64).ravel()
+    y = np.empty_like(x)
+    rc = lib().r3d_debug_detmath(C.c_int(fn), C.c_int(int(on_device)), _p(x), C.c_uint64(len(x)), _p(y))
+    if rc:
+        raise R3DError(rc, lib().r3d_last_error(None).decode())
+    return y
+
+
 def debug_ba_prior(pose, center, weight):
     pose, center, weight = [np.ascontiguousarray(a, np.float64) for a in (pose, center, weight)]
     r = np.zeros(3)
@@ -760,6 +776,40 @@ class Context:
         X = np.empty((n, 3))
         self._check(lib().r3d_debug_chol_solve3(self._h, C.c_int(n), _p(A), _p(Y), C.c_int(grid), _p(X)))
         return X
+
+    def debug_acransac_score(self, model, x1, x2, models, max_thr, logalpha0, K, x3=None, per_point=False):
+        """r3d_debug_acransac_score: the AC-RANSAC kernel's tier-1 bounds and tier-2 NFA scan of `models` (n x 9, or n x 12
+        for the internal resection model 3) on one pair.  Returns a dict: "score" (ac_score_dtype per model), "logc_n"
+        (M + 2 floats: log10 C(M, k), then the table's error bound), "logc_k" (M + 1) and, with per_point, "lo", "hi",
+        "e" (n x M: the tier-1 interval and the tier-2 residual of every point)."""
+        x1 = np.ascontiguousarray(x1, np.float64).reshape(-1, 2)
+        x2 = np.ascontiguousarray(x2, np.float64).reshape(-1, 2)
+        M = len(x1)
+        if x2.shape != (M, 2):
+            raise ValueError("x1 and x2 must both be M x 2")
+        ms = 12 if model == 3 else 9
+        models = np.ascontiguousarray(models, np.float64).reshape(-1, ms)
+        n = len(models)
+        K = np.ascontiguousarray(np.broadcast_to(np.asarray(K, np.float64).ravel(), (6,)), np.float64)
+        x3p = None
+        if x3 is not None:
+            x3 = np.ascontiguousarray(x3, np.float64).ravel()
+            if len(x3) != M:
+                raise ValueError("x3 must hold M entries")
+            x3p = _p(x3)
+        out = np.zeros(max(n, 1), ac_score_dtype)
+        logc_n = np.zeros(M + 2, np.float32)
+        logc_k = np.zeros(M + 1, np.float32)
+        lo = hi = e = None
+        if per_point:
+            lo, hi, e = (np.zeros((n, M)) for _ in range(3))
+        self._check(lib().r3d_debug_acransac_score(
+            self._h, C.c_int(model), C.c_uint32(M), _p(x1), _p(x2), x3p, C.c_double(max_thr), C.c_double(logalpha0), _p(K),
+            _p(models), C.c_uint32(n), _p(out), *(None if a is None else _p(a) for a in (lo, hi, e)), _p(logc_n), _p(logc_k)))
+        r = {"score": out[:n], "logc_n": logc_n, "logc_k": logc_k}
+        if per_point:
+            r.update(lo=lo, hi=hi, e=e)
+        return r
 
     def filter_pairs(self, putative, widths, heights, model=MODEL_F, precision_px=4.0, max_iter=2048, Ks=None):
         n = len(widths)

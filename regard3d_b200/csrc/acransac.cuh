@@ -76,6 +76,18 @@ int launch_acransac_fused(r3d_ctx* ctx, DeviceWorker& w, int model, bool huge, c
                           const uint2* matches, uint2* out_matches, AcFusedOut* out, double* out_model, uint32_t grid,
                           const double* x3 = nullptr);
 
+// r3d_debug_acransac_score on one pair already on the device (acransac_fused.cu): d_pair->pt_ofs = tbl_ofs = 0,
+// d_se / d_si: debug_acransac_cap(M) entries, d_lo / d_hi / d_e: n_models x M or null
+uint32_t debug_acransac_cap(uint32_t M);
+int debug_acransac_score(r3d_ctx* ctx, DeviceWorker& w, int model, const AcPair* d_pair, const double2* d_x1, const double2* d_x2,
+                         const double* d_x3, const float* d_logc_n, const float* d_logc_k, const double* d_models, uint32_t n_models,
+                         uint32_t M, double* d_se, uint32_t* d_si, r3d_ac_score* d_out, double* d_lo, double* d_hi, double* d_e);
+
+// the host's log10 table k = 0 .. maxM + 1 (single precision, as upstream's makelogcombi builds it) that k_ac_tables
+// sums, and makelogcombi_k: log10 C(n, ns) for n = 0 .. maxM as the running float sum upstream builds (acransac_host.cu)
+std::vector<float> ac_vlog10(uint32_t maxM);
+std::vector<float> ac_logc_k(uint32_t ns, const std::vector<float>& vlog10, uint32_t maxM);
+
 struct AcBestModel {      // per pair of the putative map (r3d_relative_poses): the kept pair's best model, errorMax
   double model[9];       // row-major; F = K2^-T E K1^-1 for the essential model
   double errorMax;       // squared residual of the last inlier

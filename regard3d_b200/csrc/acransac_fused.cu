@@ -114,12 +114,16 @@ __device__ __forceinline__ void approx_bounds(const double* F, double eta, const
     }
     const double iw = rcp_fast(hw, &ok);
     const double ex = fabs(__fma_rn(-hx, iw, b.x)), ey = fabs(__fma_rn(-hy, iw, b.y));
-    // eta bounds the absolute error of hx, hy, hw; propagated through the quotient (|hw| >> eta or the point is flagged)
+    // eta bounds the absolute error of hx, hy, hw; propagated through the quotient (|hw| >> eta or the point is flagged).
+    // The reciprocal's own relative error (<= kApproxRel) enters the cancelling difference b - h / hw too: as an
+    // absolute error |h / hw| kApproxRel of it, which a relative factor on the result cannot cover (an exact fit, where
+    // b - h / hw is 0, would get a lower bound above the true residual).
     const double aiw = fabs(iw);
     const double q = eta * aiw;                                  // relative error of hw
     if (!(q < 1e-3)) ok = false;
-    const double dx = eta * aiw + fabs(hx * iw) * q * 1.01 + 4e-16 * (fabs(b.x) + fabs(hx * iw));
-    const double dy = eta * aiw + fabs(hy * iw) * q * 1.01 + 4e-16 * (fabs(b.y) + fabs(hy * iw));
+    const double rq = q * 1.01 + kApproxRel;
+    const double dx = eta * aiw + fabs(hx * iw) * rq + 4e-16 * (fabs(b.x) + fabs(hx * iw));
+    const double dy = eta * aiw + fabs(hy * iw) * rq + 4e-16 * (fabs(b.y) + fabs(hy * iw));
     const double lx = fmax(ex - dx, 0.0), ly = fmax(ey - dy, 0.0), ux = ex + dx, uy = ey + dy;
     l = __fma_rn(lx, lx, ly * ly) * (1.0 - kApproxRel);
     h = __fma_rn(ux, ux, uy * uy) * (1.0 + kApproxRel);
@@ -148,6 +152,177 @@ __device__ __forceinline__ void approx_bounds(const double* F, double eta, const
   }
   *lo = l;
   *hi = h;
+}
+
+// ---- per-pair set-up, shared by k_acransac_fused and k_acransac_debug ------------------------------------------
+// This thread's share of R = the pair's largest |coordinate| (reduced over its warp, the warp's value stored at
+// s_rmax[warp]), and the histogram's bin_base and la[] table.  per_point(i) runs once for every point this thread reads.
+// bin(e) = clamp((bits(e) >> kBinShift) - bin_base, 0, kBins - 1): the precision bound falls in the top bin (the
+// resection model's bound may be infinite: its top bin starts at pr.K[3]; larger residuals are clamped into it,
+// whose lower edge still bounds them from below)
+template <int MODEL, typename PerPoint>
+__device__ __forceinline__ long long pair_setup(const AcPair& pr, const double2* p1, const double2* p2, const double* pz,
+                                                double* la, double* s_rmax, double* rmax_out, PerPoint per_point) {
+  const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u;
+  const double mult_error = (MODEL == 1 || MODEL == 3) ? 1.0 : 0.5;
+  double rmax = 0.0;
+  for (uint32_t i = tid; i < pr.M; i += kFThreads) {
+    per_point(i);
+    const double2 a = p1[i], b = p2[i];
+    rmax = fmax(rmax, fmax(fmax(fabs(a.x), fabs(a.y)), fmax(fabs(b.x), fabs(b.y))));
+    if (MODEL == 3) rmax = fmax(rmax, fabs(pz[i]));
+  }
+  for (int o = 16; o >= 1; o >>= 1) rmax = fmax(rmax, __shfl_xor_sync(0xffffffffu, rmax, o));
+  if (lane == 0) s_rmax[warp] = rmax;
+  const long long thr_key = __double_as_longlong(MODEL == 3 ? fmin(pr.max_thr, pr.K[3]) : pr.max_thr) >> kBinShift;
+  const long long bin_base = thr_key - (kBins - 1);
+  for (uint32_t b = tid; b < (uint32_t)kBins; b += kFThreads) {
+    const long long kb = bin_base + (long long)b;
+    const double lo = (b == 0 || kb <= 0) ? 0.0 : __longlong_as_double(kb << kBinShift);
+    la[bin_slot(b)] = pr.logalpha0 + mult_error * dm::log10_det(lo + (double)FLT_EPSILON);
+  }
+  *rmax_out = rmax;
+  return bin_base;
+}
+
+// (2 R + 1)^2 from the per-warp maxima of pair_setup (call after the barrier that publishes them)
+__device__ __forceinline__ double pair_coord_span(const double* s_rmax, double rmax) {
+  for (uint32_t wv = 0; wv < (uint32_t)kFWarps; ++wv) rmax = fmax(rmax, s_rmax[wv]);
+  return (2.0 * rmax + 1.0) * (2.0 * rmax + 1.0);
+}
+
+// absolute error bound of the cancelling term of approx_bounds for model Fm
+template <int MODEL>
+__device__ __forceinline__ double model_eta(const double* Fm, double coord_span) {
+  double fmax_abs = 0.0;
+  for (int t = 0; t < (int)ac_model_size(MODEL); ++t) fmax_abs = fmax(fmax_abs, fabs(Fm[t]));
+  return 7.2e-15 * fmax_abs * coord_span;            // 64 ulp x the largest term of x2^T F x1 (or H x1)
+}
+
+// Tier 1 of one batch, run by the consumer warps 1 .. kFWarps - 1 only (they sync on named barrier 1): for every model
+// of Q, Q.cnt / Q.cnt_lo (upper / lower count of the residuals <= pr.max_thr) and Q.lb (lower bound of its best NFA).
+// Points outer / models inner: the consumer warps split the pair's points, each point is loaded ONCE and scored against
+// a group of kGroup models (their matrices are broadcast reads from shared memory), so the loop is bound by the fp64
+// pipe instead of by the latency of re-streaming the points for every model.
+template <int MODEL>
+__device__ __forceinline__ void tier1_score(FusedSmem<MODEL>& S, BatchBuf<MODEL>& Q, uint32_t B, uint32_t* hist_all,
+                                           const AcPair& pr, const double2* p1, const double2* p2, const double* pz,
+                                           const float* lcn, const float* logc_k, double coord_span, long long bin_base) {
+  constexpr uint32_t NS = ac_min_samples(MODEL);
+  const uint32_t M = pr.M;
+  const uint32_t tid = threadIdx.x, warp = tid >> 5, lane = tid & 31u;
+  constexpr uint32_t kGroup = kFWarps - 1;                 // models per group = consumer warps (one LB scan each)
+  constexpr uint32_t kConsumers = (kFWarps - 1) * 32;
+  const uint32_t cw = warp - 1, ctid = tid - 32;
+  // the batch's models as a flat list (iteration b, model mi) -- every consumer thread walks it identically
+  uint32_t n_models_batch = 0;
+  for (uint32_t b = 0; b < B; ++b) n_models_batch += Q.nm[b];
+  // the histograms alias the tier-2 sort buffer: clear them once per batch, every scan clears its own afterwards
+  for (uint32_t i = ctid; i < kGroup * (uint32_t)kHistStride; i += kConsumers) hist_all[i] = 0;
+  if (ctid < 2 * kGroup) S.gcnt[ctid] = 0;
+  asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
+  for (uint32_t g0 = 0; g0 < n_models_batch; g0 += kGroup) {
+    const uint32_t gn = min(kGroup, n_models_batch - g0);
+    // locate the group's models
+    uint32_t gb[kGroup], gm[kGroup];
+    {
+      uint32_t seen = 0, k = 0;
+      for (uint32_t b = 0; b < B && k < gn; ++b) {
+        const uint32_t nmb = Q.nm[b];
+        if (seen + nmb <= g0) { seen += nmb; continue; }
+        for (uint32_t mi = (g0 > seen ? g0 - seen : 0u); mi < nmb && k < gn; ++mi) { gb[k] = b; gm[k] = mi; ++k; }
+        seen += nmb;
+      }
+    }
+    double eta[kGroup];
+    for (uint32_t k = 0; k < gn; ++k) eta[k] = model_eta<MODEL>(&Q.models[gb[k]][gm[k]][0], coord_span);
+    uint32_t c_hi[kGroup], c_lo[kGroup];
+    for (uint32_t k = 0; k < kGroup; ++k) { c_hi[k] = 0; c_lo[k] = 0; }
+    for (uint32_t i = ctid; i < M; i += kConsumers) {
+      const double2 a = p1[i], b2 = p2[i];
+      const double z = MODEL == 3 ? pz[i] : 0.0;
+#pragma unroll
+      for (uint32_t k = 0; k < kGroup; ++k) {
+        if (k >= gn) break;
+        double elo, ehi;
+        approx_bounds<MODEL>(&Q.models[gb[k]][gm[k]][0], eta[k], a, b2, z, &elo, &ehi);
+        if (elo <= pr.max_thr) {  // may be an inlier of the precision bound
+          long long bin = (__double_as_longlong(elo) >> kBinShift) - bin_base;
+          bin = bin < 0 ? 0 : (bin > kBins - 1 ? kBins - 1 : bin);
+          atomicAdd(&hist_all[k * kHistStride + bin_slot((uint32_t)bin)], 1u);
+          ++c_hi[k];
+          if (ehi <= pr.max_thr) ++c_lo[k];
+        }
+      }
+    }
+#pragma unroll
+    for (uint32_t k = 0; k < kGroup; ++k) {
+      if (k >= gn) break;
+      uint32_t h = c_hi[k], l = c_lo[k];
+      for (int o = 16; o >= 1; o >>= 1) {
+        h += __shfl_xor_sync(0xffffffffu, h, o);
+        l += __shfl_xor_sync(0xffffffffu, l, o);
+      }
+      if (lane == 0) { atomicAdd(&S.gcnt[2 * k], h); atomicAdd(&S.gcnt[2 * k + 1], l); }
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
+    if (cw < gn) {  // one warp per model of the group: lower bound of its best NFA from its histogram
+      uint32_t* hist = hist_all + (size_t)cw * kHistStride + lane * 33u;  // this lane's 32 consecutive bins
+      const double* lab = S.la + lane * 33u;
+      const uint32_t ch = S.gcnt[2 * cw], cl = S.gcnt[2 * cw + 1];
+      double lbv = DBL_MAX * 2.0;
+      if (ch > NS) {
+        uint32_t tot = 0;
+#pragma unroll 8
+        for (uint32_t j = 0; j < 32; ++j) tot += hist[j];
+        uint32_t incl = tot;
+        for (int o = 1; o < 32; o <<= 1) {
+          const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
+          if ((int)lane >= o) incl += u;
+        }
+        uint32_t run = incl - tot;  // lower bounds in the bins before this lane's
+        // Ranks (run, run + v] live in a bin with lower edge e_b.  With e_(k) the true k-th smallest residual: at
+        // least k of the lower bounds are <= e_(k), so the k-th smallest LOWER BOUND is <= e_(k), hence
+        //   NFA_k >= g_b(k) = loge0 + la[b] (k - NS) + logc_n[k] + logc_k[k];
+        // extra ranks (c_hi >= c) only lower the minimum.  log10 C(n, k) and log10 C(k, NS) are concave in k and
+        // the rest of g_b is linear, so over the ranks of one bin g_b is smallest at one of the two end ranks --
+        // for the exact binomials.  The float tables differ from them by at most tbl_err (accumulated by
+        // k_ac_tables while it sums), which the bound gives back twice over.
+        for (uint32_t j = 0; j < 32; ++j) {
+          const uint32_t v = hist[j];
+          if (v) {
+            const uint32_t ka = max(run + 1, NS + 1), kb = run + v;
+            if (ka <= kb) {
+              const double la = lab[j];
+              const double ga = la * (double)(ka - NS) + ((double)lcn[ka] + (double)logc_k[ka]);
+              const double gb2 = la * (double)(kb - NS) + ((double)lcn[kb] + (double)logc_k[kb]);
+              lbv = fmin(lbv, fmin(ga, gb2));
+            }
+            run += v;
+            hist[j] = 0;
+          }
+        }
+        for (int o = 16; o >= 1; o >>= 1) {
+          const double ov = __shfl_xor_sync(0xffffffffu, lbv, o);
+          lbv = ov < lbv ? ov : lbv;
+        }
+        lbv += pr.loge0;
+        // table error (see above), then a few ulp for the monotonicity of log10_det at its range-reduction seams
+        // (tests/test_detmath.py measures its largest drop: ~1e-15 absolute, far inside this slack)
+        lbv -= 2.0 * (double)lcn[M + 1] + 1e-4;
+        lbv = lbv - 1e-9 * (1.0 + fabs(lbv));
+      } else {
+#pragma unroll 8
+        for (uint32_t j = 0; j < 32; ++j) hist[j] = 0;
+      }
+      __syncwarp();  // every lane has read the group counters before lane 0 clears them (racecheck: intra-warp hazard)
+      if (lane == 0) {
+        Q.cnt[gb[cw]][gm[cw]] = ch; Q.cnt_lo[gb[cw]][gm[cw]] = cl; Q.lb[gb[cw]][gm[cw]] = lbv;
+        S.gcnt[2 * cw] = 0; S.gcnt[2 * cw + 1] = 0;
+      }
+    }
+    asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");  // cleared histograms and counters: next group
+  }
 }
 
 }  // namespace
@@ -195,7 +370,6 @@ __global__ void __launch_bounds__(kFThreads, MODEL >= 2 ? 1 : 2) k_acransac_fuse
   extern __shared__ __align__(16) unsigned char smem_raw[];
   constexpr uint32_t NS = ac_min_samples(MODEL), MAXM = ac_max_models(MODEL), MS = ac_model_size(MODEL);
   typedef typename std::conditional<HUGE, uint32_t, uint16_t>::type PoolT;
-  const double mult_error = (MODEL == 1 || MODEL == 3) ? 1.0 : 0.5;
   FusedSmem<MODEL>& S = *reinterpret_cast<FusedSmem<MODEL>*>(smem_raw);
   unsigned char* region = smem_raw + ((sizeof(FusedSmem<MODEL>) + 15) & ~(size_t)15);
   uint32_t* hist_all = reinterpret_cast<uint32_t*>(region);                 // tier 1: kFWarps x kBins
@@ -221,29 +395,11 @@ __global__ void __launch_bounds__(kFThreads, MODEL >= 2 ? 1 : 2) k_acransac_fuse
     const double* pz = MODEL == 3 ? x3 + pr.pt_ofs : nullptr;
 
     // ---- per-pair set-up: sampling pool, generator, bin edges, coordinate bound --------------------------------
-    double rmax = 0.0;
-    for (uint32_t i = tid; i < M; i += kFThreads) {
-      pool[i] = (PoolT)i;
-      const double2 a = p1[i], b = p2[i];
-      rmax = fmax(rmax, fmax(fmax(fabs(a.x), fabs(a.y)), fmax(fabs(b.x), fabs(b.y))));
-      if (MODEL == 3) rmax = fmax(rmax, fabs(pz[i]));
-    }
-    for (int o = 16; o >= 1; o >>= 1) rmax = fmax(rmax, __shfl_xor_sync(0xffffffffu, rmax, o));
-    if (lane == 0) S.s_nfa[warp] = rmax;
-    // bin(e) = clamp((bits(e) >> kBinShift) - bin_base, 0, kBins - 1): the precision bound falls in the top bin (the
-    // resection model's bound may be infinite: its top bin starts at pr.K[3]; larger residuals are clamped into it,
-    // whose lower edge still bounds them from below)
-    const long long thr_key = __double_as_longlong(MODEL == 3 ? fmin(pr.max_thr, pr.K[3]) : pr.max_thr) >> kBinShift;
-    const long long bin_base = thr_key - (kBins - 1);
-    for (uint32_t b = tid; b < (uint32_t)kBins; b += kFThreads) {
-      const long long kb = bin_base + (long long)b;
-      const double lo = (b == 0 || kb <= 0) ? 0.0 : __longlong_as_double(kb << kBinShift);
-      S.la[bin_slot(b)] = pr.logalpha0 + mult_error * dm::log10_det(lo + (double)FLT_EPSILON);
-    }
+    double rmax;
+    const long long bin_base = pair_setup<MODEL>(pr, p1, p2, pz, S.la, S.s_nfa, &rmax, [&](uint32_t i) { pool[i] = (PoolT)i; });
     if (tid == 0) mt_seed(S.rng);
     __syncthreads();
-    for (uint32_t wv = 0; wv < (uint32_t)kFWarps; ++wv) rmax = fmax(rmax, S.s_nfa[wv]);
-    const double coord_span = (2.0 * rmax + 1.0) * (2.0 * rmax + 1.0);
+    const double coord_span = pair_coord_span(S.s_nfa, rmax);
     // ACRANSAC state, replicated in the registers of every thread (updated identically from shared data)
     uint32_t iter = 0, nIterReserve = max_iter / 10, nIter = max_iter - nIterReserve;
     bool ac_mode = !(pr.max_thr < DBL_MAX);  // bACRansacMode = (precision == infinity)
@@ -334,126 +490,7 @@ __global__ void __launch_bounds__(kFThreads, MODEL >= 2 ? 1 : 2) k_acransac_fuse
       if (warp == 0) {
         if (ahead) produce(S.q[cur ^ 1u], ahead, pool_size);
       } else {
-        // Tier 1, points outer / models inner: the consumer warps split the pair's points, each point is loaded ONCE
-        // and scored against a group of kGroup models (their matrices are broadcast reads from shared memory), so the
-        // loop is bound by the fp64 pipe instead of by the latency of re-streaming the points for every model.
-        constexpr uint32_t kGroup = kFWarps - 1;                 // models per group = consumer warps (one LB scan each)
-        constexpr uint32_t kConsumers = (kFWarps - 1) * 32;
-        const uint32_t cw = warp - 1, ctid = tid - 32;
-        // the batch's models as a flat list (iteration b, model mi) -- every consumer thread walks it identically
-        uint32_t n_models_batch = 0;
-        for (uint32_t b = 0; b < B; ++b) n_models_batch += Q.nm[b];
-        // the histograms alias the tier-2 sort buffer: clear them once per batch, every scan clears its own afterwards
-        for (uint32_t i = ctid; i < kGroup * (uint32_t)kHistStride; i += kConsumers) hist_all[i] = 0;
-        if (ctid < 2 * kGroup) S.gcnt[ctid] = 0;
-        asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
-        for (uint32_t g0 = 0; g0 < n_models_batch; g0 += kGroup) {
-          const uint32_t gn = min(kGroup, n_models_batch - g0);
-          // locate the group's models
-          uint32_t gb[kGroup], gm[kGroup];
-          {
-            uint32_t seen = 0, k = 0;
-            for (uint32_t b = 0; b < B && k < gn; ++b) {
-              const uint32_t nmb = Q.nm[b];
-              if (seen + nmb <= g0) { seen += nmb; continue; }
-              for (uint32_t mi = (g0 > seen ? g0 - seen : 0u); mi < nmb && k < gn; ++mi) { gb[k] = b; gm[k] = mi; ++k; }
-              seen += nmb;
-            }
-          }
-          double eta[kGroup];
-          for (uint32_t k = 0; k < gn; ++k) {
-            const double* Fm = &Q.models[gb[k]][gm[k]][0];
-            double fmax_abs = 0.0;
-            for (int t = 0; t < (int)MS; ++t) fmax_abs = fmax(fmax_abs, fabs(Fm[t]));
-            eta[k] = 7.2e-15 * fmax_abs * coord_span;            // 64 ulp x the largest term of x2^T F x1 (or H x1)
-          }
-          uint32_t c_hi[kGroup], c_lo[kGroup];
-          for (uint32_t k = 0; k < kGroup; ++k) { c_hi[k] = 0; c_lo[k] = 0; }
-          for (uint32_t i = ctid; i < M; i += kConsumers) {
-            const double2 a = p1[i], b2 = p2[i];
-            const double z = MODEL == 3 ? pz[i] : 0.0;
-#pragma unroll
-            for (uint32_t k = 0; k < kGroup; ++k) {
-              if (k >= gn) break;
-              double elo, ehi;
-              approx_bounds<MODEL>(&Q.models[gb[k]][gm[k]][0], eta[k], a, b2, z, &elo, &ehi);
-              if (elo <= pr.max_thr) {  // may be an inlier of the precision bound
-                long long bin = (__double_as_longlong(elo) >> kBinShift) - bin_base;
-                bin = bin < 0 ? 0 : (bin > kBins - 1 ? kBins - 1 : bin);
-                atomicAdd(&hist_all[k * kHistStride + bin_slot((uint32_t)bin)], 1u);
-                ++c_hi[k];
-                if (ehi <= pr.max_thr) ++c_lo[k];
-              }
-            }
-          }
-#pragma unroll
-          for (uint32_t k = 0; k < kGroup; ++k) {
-            if (k >= gn) break;
-            uint32_t h = c_hi[k], l = c_lo[k];
-            for (int o = 16; o >= 1; o >>= 1) {
-              h += __shfl_xor_sync(0xffffffffu, h, o);
-              l += __shfl_xor_sync(0xffffffffu, l, o);
-            }
-            if (lane == 0) { atomicAdd(&S.gcnt[2 * k], h); atomicAdd(&S.gcnt[2 * k + 1], l); }
-          }
-          asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");
-          if (cw < gn) {  // one warp per model of the group: lower bound of its best NFA from its histogram
-            uint32_t* hist = hist_all + (size_t)cw * kHistStride + lane * 33u;  // this lane's 32 consecutive bins
-            const double* lab = S.la + lane * 33u;
-            const uint32_t ch = S.gcnt[2 * cw], cl = S.gcnt[2 * cw + 1];
-            double lbv = DBL_MAX * 2.0;
-            if (ch > NS) {
-              uint32_t tot = 0;
-#pragma unroll 8
-              for (uint32_t j = 0; j < 32; ++j) tot += hist[j];
-              uint32_t incl = tot;
-              for (int o = 1; o < 32; o <<= 1) {
-                const uint32_t u = __shfl_up_sync(0xffffffffu, incl, o);
-                if ((int)lane >= o) incl += u;
-              }
-              uint32_t run = incl - tot;  // lower bounds in the bins before this lane's
-              // Ranks (run, run + v] live in a bin with lower edge e_b.  With e_(k) the true k-th smallest residual: at
-              // least k of the lower bounds are <= e_(k), so the k-th smallest LOWER BOUND is <= e_(k), hence
-              //   NFA_k >= g_b(k) = loge0 + la[b] (k - NS) + logc_n[k] + logc_k[k];
-              // extra ranks (c_hi >= c) only lower the minimum.  log10 C(n, k) and log10 C(k, NS) are concave in k and
-              // the rest of g_b is linear, so over the ranks of one bin g_b is smallest at one of the two end ranks --
-              // for the exact binomials.  The float tables differ from them by at most tbl_err (accumulated by
-              // k_ac_tables while it sums), which the bound gives back twice over.
-              for (uint32_t j = 0; j < 32; ++j) {
-                const uint32_t v = hist[j];
-                if (v) {
-                  const uint32_t ka = max(run + 1, NS + 1), kb = run + v;
-                  if (ka <= kb) {
-                    const double la = lab[j];
-                    const double ga = la * (double)(ka - NS) + ((double)lcn[ka] + (double)logc_k[ka]);
-                    const double gb2 = la * (double)(kb - NS) + ((double)lcn[kb] + (double)logc_k[kb]);
-                    lbv = fmin(lbv, fmin(ga, gb2));
-                  }
-                  run += v;
-                  hist[j] = 0;
-                }
-              }
-              for (int o = 16; o >= 1; o >>= 1) {
-                const double ov = __shfl_xor_sync(0xffffffffu, lbv, o);
-                lbv = ov < lbv ? ov : lbv;
-              }
-              lbv += pr.loge0;
-              // table error (see above), then a few ulp for the (unproven) monotonicity of log10_det at its
-              // range-reduction seams
-              lbv -= 2.0 * (double)lcn[M + 1] + 1e-4;
-              lbv = lbv - 1e-9 * (1.0 + fabs(lbv));
-            } else {
-#pragma unroll 8
-              for (uint32_t j = 0; j < 32; ++j) hist[j] = 0;
-            }
-            __syncwarp();  // every lane has read the group counters before lane 0 clears them (racecheck: intra-warp hazard)
-            if (lane == 0) {
-              Q.cnt[gb[cw]][gm[cw]] = ch; Q.cnt_lo[gb[cw]][gm[cw]] = cl; Q.lb[gb[cw]][gm[cw]] = lbv;
-              S.gcnt[2 * cw] = 0; S.gcnt[2 * cw + 1] = 0;
-            }
-          }
-          asm volatile("bar.sync 1, %0;" ::"n"(kConsumers) : "memory");  // cleared histograms and counters: next group
-        }
+        tier1_score<MODEL>(S, Q, B, hist_all, pr, p1, p2, pz, lcn, logc_k, coord_span, bin_base);
       }
       __syncthreads();
       // ---- phase B: replay the ACRANSAC state machine over the batch (uniform control flow) ---------------------
@@ -597,6 +634,99 @@ int launch_acransac_fused(r3d_ctx* ctx, DeviceWorker& w, int model, bool huge, c
   R3D_FUSED_CASE(2, false) R3D_FUSED_CASE(2, true) R3D_FUSED_CASE(3, false) R3D_FUSED_CASE(3, true)
 #undef R3D_FUSED_CASE
   return fail(ctx, R3D_ERR_INVALID, "launch_acransac_fused: unknown model");
+}
+
+// ---- r3d_debug_acransac_score: the fused kernel's set-up, tier 1 and tier 2 on a caller's models ---------------
+// One CTA, one pair.  The caller's models are laid out as RANSAC iterations of ac_max_models(MODEL) models each
+// (the last one partial), kBatch iterations per pass, and scored by the very tier1_score() of k_acransac_fused (warp 0
+// idle, warps 1.. on named barrier 1); then every model goes through exact_count and the tier-2 sort + NFA scan.
+// lo / hi / e (may be null): per (model, point) the tier-1 interval and the tier-2 residual.
+template <int MODEL, bool HUGE>
+__global__ void __launch_bounds__(kFThreads, 1) k_acransac_debug(const AcPair* __restrict__ pair, const double2* __restrict__ x1,
+                                                                 const double2* __restrict__ x2, const double* __restrict__ x3,
+                                                                 const float* __restrict__ logc_n, const float* __restrict__ logc_k,
+                                                                 const double* __restrict__ models, uint32_t n_models, uint32_t cap,
+                                                                 double* __restrict__ g_se, uint32_t* __restrict__ g_si,
+                                                                 r3d_ac_score* __restrict__ out, double* __restrict__ out_lo,
+                                                                 double* __restrict__ out_hi, double* __restrict__ out_e) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  constexpr uint32_t MAXM = ac_max_models(MODEL), MS = ac_model_size(MODEL), kPass = kBatch * MAXM;
+  FusedSmem<MODEL>& S = *reinterpret_cast<FusedSmem<MODEL>*>(smem_raw);
+  unsigned char* region = smem_raw + ((sizeof(FusedSmem<MODEL>) + 15) & ~(size_t)15);
+  uint32_t* hist_all = reinterpret_cast<uint32_t*>(region);
+  double* se = HUGE ? g_se : reinterpret_cast<double*>(region);
+  const uint32_t tid = threadIdx.x, warp = tid >> 5;
+  const AcPair pr = *pair;
+  const uint32_t M = pr.M;
+  double rmax;
+  const long long bin_base = pair_setup<MODEL>(pr, x1, x2, x3, S.la, S.s_nfa, &rmax, [](uint32_t) {});
+  __syncthreads();
+  const double coord_span = pair_coord_span(S.s_nfa, rmax);
+  BatchBuf<MODEL>& Q = S.q[0];
+  for (uint32_t m0 = 0; m0 < n_models; m0 += kPass) {
+    const uint32_t nq = min(kPass, n_models - m0), B = (nq + MAXM - 1) / MAXM;
+    __syncthreads();  // the previous pass's tier 2 is done with Q and the shared scratch
+    for (uint32_t t = tid; t < nq * MS; t += kFThreads) {
+      const uint32_t j = t / MS;
+      Q.models[j / MAXM][j % MAXM][t % MS] = models[(size_t)(m0 + j) * MS + t % MS];
+    }
+    if (tid < B) Q.nm[tid] = min(MAXM, nq - tid * MAXM);
+    __syncthreads();
+    if (warp != 0) tier1_score<MODEL>(S, Q, B, hist_all, pr, x1, x2, x3, logc_n, logc_k, coord_span, bin_base);
+    __syncthreads();
+    for (uint32_t j = 0; j < nq; ++j) {
+      const uint32_t b = j / MAXM, mi = j % MAXM, m = m0 + j;
+      double Fm[MS];
+      for (int t = 0; t < (int)MS; ++t) Fm[t] = Q.models[b][mi][t];
+      const uint32_t count = exact_count<MODEL>(pr, x1, x2, x3, Fm, &S.s_count);
+      const uint32_t c = residuals_sorted<MODEL, false>(pr, x1, x2, Fm, se, g_si, cap, &S.s_count, x3);
+      const NfaBest r = nfa_scan_sorted<MODEL>(pr, se, c, logc_n, logc_k, S.s_nfa, S.s_k);
+      if (tid == 0) {
+        r3d_ac_score o;
+        o.lb = Q.lb[b][mi]; o.nfa = r.nfa; o.err = r.err;
+        o.cnt_hi = Q.cnt[b][mi]; o.cnt_lo = Q.cnt_lo[b][mi]; o.count = count; o.k = r.k;
+        out[m] = o;
+      }
+      if (out_lo) {
+        const double eta = model_eta<MODEL>(Fm, coord_span);
+        for (uint32_t i = tid; i < M; i += kFThreads) {
+          const double z = MODEL == 3 ? x3[i] : 0.0;
+          double lo, hi;
+          approx_bounds<MODEL>(Fm, eta, x1[i], x2[i], z, &lo, &hi);
+          out_lo[(size_t)m * M + i] = lo;
+          out_hi[(size_t)m * M + i] = hi;
+          out_e[(size_t)m * M + i] = model_error<MODEL>(Fm, x1[i], x2[i], z);
+        }
+      }
+    }
+  }
+}
+
+// the sort capacity of the size class run_fused / resect_range put a pair of M matches in
+uint32_t debug_acransac_cap(uint32_t M) {
+  uint32_t cap = 1024;
+  while (cap < M) cap <<= 1;
+  return M > 16384u ? std::max(cap, 32768u) : cap;
+}
+
+int debug_acransac_score(r3d_ctx* ctx, DeviceWorker& w, int model, const AcPair* d_pair, const double2* d_x1, const double2* d_x2,
+                         const double* d_x3, const float* d_logc_n, const float* d_logc_k, const double* d_models, uint32_t n_models,
+                         uint32_t M, double* d_se, uint32_t* d_si, r3d_ac_score* d_out, double* d_lo, double* d_hi, double* d_e) {
+  const bool huge = M > 16384u;
+  const uint32_t cap = debug_acransac_cap(M);
+  const size_t smem = acransac_fused_smem_bytes(model, cap, huge);
+#define R3D_DEBUG_CASE(MD, HG)                                                                                            \
+  if (model == MD && huge == HG) {                                                                                        \
+    R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(k_acransac_debug<MD, HG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+    k_acransac_debug<MD, HG><<<1, kFThreads, smem, w.stream>>>(d_pair, d_x1, d_x2, d_x3, d_logc_n, d_logc_k, d_models, n_models, \
+                                                              cap, d_se, d_si, d_out, d_lo, d_hi, d_e);                     \
+    R3D_CUDA_TRY(ctx, cudaGetLastError());                                                                                \
+    return R3D_OK;                                                                                                        \
+  }
+  R3D_DEBUG_CASE(0, false) R3D_DEBUG_CASE(0, true) R3D_DEBUG_CASE(1, false) R3D_DEBUG_CASE(1, true)
+  R3D_DEBUG_CASE(2, false) R3D_DEBUG_CASE(2, true) R3D_DEBUG_CASE(3, false) R3D_DEBUG_CASE(3, true)
+#undef R3D_DEBUG_CASE
+  return fail(ctx, R3D_ERR_INVALID, "debug_acransac_score: unknown model");
 }
 
 // ---- the restated sample stream against this process's <random> -------------------------------------------------

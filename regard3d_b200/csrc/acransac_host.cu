@@ -280,6 +280,28 @@ int run_fused(r3d_ctx* ctx, DeviceWorker& w, int model, uint32_t max_iter, const
 
 }  // namespace
 
+// log-combinatorial tables (float, upstream makelogcombi_n / makelogcombi_k).  logcombi(k,n) is a running float sum over
+// i = 1..min(k,n-k): its partial sums ARE the entries for smaller k, so one O(n) pass reproduces the upstream O(n^2)
+// table bit for bit.
+std::vector<float> ac_vlog10(uint32_t maxM) {
+  std::vector<float> vlog10(maxM + 2);
+  for (uint32_t k = 0; k <= maxM + 1; ++k) vlog10[k] = std::log10((float)k);
+  return vlog10;
+}
+
+std::vector<float> ac_logc_k(uint32_t ns, const std::vector<float>& vlog10, uint32_t maxM) {
+  std::vector<float> logc_k(maxM + 1, 0.f);
+  for (uint32_t n = 0; n <= maxM; ++n) {
+    uint32_t k = ns;
+    if (k >= n) continue;
+    if (n - k < k) k = n - k;
+    float r = 0.f;
+    for (uint32_t i = 1; i <= k; ++i) r += vlog10[n - i + 1] - vlog10[i];
+    logc_k[n] = r;
+  }
+  return logc_k;
+}
+
 // pairs [p0, p1) of the putative map on worker w; result (sized by the caller to the whole map) is indexed by pair
 int filter_pairs_model(r3d_ctx* ctx, DeviceWorker& w, int model, double precision_px, uint32_t max_iter, const r3d_matches* put,
                    const r3d_view_info* views, uint32_t n_views, uint64_t p0, uint64_t p1, r3d_filter_timing& T,
@@ -329,20 +351,8 @@ int filter_pairs_model(r3d_ctx* ctx, DeviceWorker& w, int model, double precisio
   if (best && !use_fused)
     return fail(ctx, R3D_ERR_UNSUPPORTED, "AC-RANSAC model output needs the device-resident path (the device sample stream "
                                           "disagrees with this process's <random>)");
-  // log-combinatorial tables (float, upstream makelogcombi_n / makelogcombi_k).  logcombi(k,n) is a
-  // running float sum over i = 1..min(k,n-k): its partial sums ARE the entries for smaller k, so one
-  // O(n) pass reproduces the upstream O(n^2) table bit for bit.
-  std::vector<float> vlog10(maxM + 2);
-  for (uint32_t k = 0; k <= maxM + 1; ++k) vlog10[k] = std::log10((float)k);
-  std::vector<float> hlogc_k(maxM + 1, 0.f);
-  for (uint32_t n = 0; n <= maxM; ++n) {
-    uint32_t k = sizeSample;
-    if (k >= n) { hlogc_k[n] = 0.f; continue; }
-    if (n - k < k) k = n - k;
-    float r = 0.f;
-    for (uint32_t i = 1; i <= k; ++i) r += vlog10[n - i + 1] - vlog10[i];
-    hlogc_k[n] = r;
-  }
+  const std::vector<float> vlog10 = ac_vlog10(maxM);
+  const std::vector<float> hlogc_k = ac_logc_k(sizeSample, vlog10, maxM);
   std::atomic<int> bad{0};
   const double t_pairs0 = now_ms();
   parallel_for(ctx->host_threads, st.size(), [&](size_t a) {
@@ -673,6 +683,86 @@ using namespace r3d;
 // Diagnostics (host only): 1 when the device-side restatement of std::mt19937 + std::uniform_int_distribution
 // (acransac_rng.cuh) reproduces this process's <random>, i.e. when the filter runs fully on the device.
 extern "C" int r3d_debug_rng_selftest(void) { return rng_selftest() ? 1 : 0; }
+
+extern "C" int r3d_debug_acransac_score(r3d_ctx* ctx, int model, uint32_t M, const double* x1, const double* x2, const double* x3,
+                                        double max_thr, double logalpha0, const double* K, const double* models, uint32_t n_models,
+                                        r3d_ac_score* out, double* lo, double* hi, double* e, float* logc_n, float* logc_k) {
+  if (!ctx || model < 0 || model > 3 || !x1 || !x2 || !K || !models || !out || n_models < 1)
+    return fail(ctx, R3D_ERR_INVALID, "r3d_debug_acransac_score: bad arguments");
+  const uint32_t NS = ac_min_samples(model), MS = ac_model_size(model);
+  if ((model == 3) != (x3 != nullptr)) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_acransac_score: x3 belongs to model 3");
+  if (M < NS || M > (1u << 24)) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_acransac_score: M outside [minimal sample, 2^24]");
+  if (!(max_thr >= 0.0) || (model != 3 && !(max_thr < INFINITY)) || !std::isfinite(logalpha0))
+    return fail(ctx, R3D_ERR_INVALID, "r3d_debug_acransac_score: bad max_thr / logalpha0");
+  if (model == 3 && !(K[3] > 0.0 && K[3] < INFINITY)) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_acransac_score: K[3] must be > 0");
+  if ((lo != nullptr) != (hi != nullptr) || (lo != nullptr) != (e != nullptr))
+    return fail(ctx, R3D_ERR_INVALID, "r3d_debug_acransac_score: lo, hi and e go together");
+  if (n_models > (1u << 20) || (lo && (uint64_t)n_models * M > (1ull << 28)))
+    return fail(ctx, R3D_ERR_INVALID, "r3d_debug_acransac_score: too many models");
+  DeviceWorker& w = ctx->workers[0];
+  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
+  AcPair ap;
+  std::memset(&ap, 0, sizeof(ap));
+  ap.M = M;
+  ap.max_thr = max_thr;
+  ap.logalpha0 = logalpha0;
+  ap.loge0 = dm::log10_det((double)ac_max_models(model) * (double)(M - NS));
+  std::memcpy(ap.K, K, sizeof(ap.K));
+  const std::vector<float> vlog10 = ac_vlog10(M);
+  const std::vector<float> hlogc_k = ac_logc_k(NS, vlog10, M);
+  std::vector<double2> h1(M), h2(M);
+  for (uint32_t i = 0; i < M; ++i) {
+    h1[i] = make_double2(x1[2 * i], x1[2 * i + 1]);
+    h2[i] = make_double2(x2[2 * i], x2[2 * i + 1]);
+  }
+  const uint32_t cap = debug_acransac_cap(M);
+  const size_t nper = lo ? (size_t)n_models * M : 0;
+  DevBuf<AcPair> d_pair(w);
+  DevBuf<double2> d_x1(w), d_x2(w);
+  DevBuf<double> d_x3(w), d_models(w), d_se(w), d_lo(w), d_hi(w), d_e(w);
+  DevBuf<float> d_vlog10(w), d_logc_n(w), d_logc_k(w);
+  DevBuf<uint32_t> d_si(w);
+  DevBuf<r3d_ac_score> d_out(w);
+  R3D_CUDA_TRY(ctx, d_pair.ensure(1));
+  R3D_CUDA_TRY(ctx, d_x1.ensure(M));
+  R3D_CUDA_TRY(ctx, d_x2.ensure(M));
+  R3D_CUDA_TRY(ctx, d_x3.ensure(M));
+  R3D_CUDA_TRY(ctx, d_models.ensure((size_t)n_models * MS));
+  R3D_CUDA_TRY(ctx, d_se.ensure(cap));
+  R3D_CUDA_TRY(ctx, d_si.ensure(cap));
+  R3D_CUDA_TRY(ctx, d_vlog10.ensure(vlog10.size()));
+  R3D_CUDA_TRY(ctx, d_logc_n.ensure((size_t)M + 2));
+  R3D_CUDA_TRY(ctx, d_logc_k.ensure(hlogc_k.size()));
+  R3D_CUDA_TRY(ctx, d_out.ensure(n_models));
+  if (nper) {
+    R3D_CUDA_TRY(ctx, d_lo.ensure(nper));
+    R3D_CUDA_TRY(ctx, d_hi.ensure(nper));
+    R3D_CUDA_TRY(ctx, d_e.ensure(nper));
+  }
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_pair.p, &ap, sizeof(ap), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_x1.p, h1.data(), (size_t)M * sizeof(double2), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_x2.p, h2.data(), (size_t)M * sizeof(double2), cudaMemcpyHostToDevice, w.stream));
+  if (x3) R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_x3.p, x3, (size_t)M * sizeof(double), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_models.p, models, (size_t)n_models * MS * sizeof(double), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_vlog10.p, vlog10.data(), vlog10.size() * sizeof(float), cudaMemcpyHostToDevice, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_logc_k.p, hlogc_k.data(), hlogc_k.size() * sizeof(float), cudaMemcpyHostToDevice, w.stream));
+  int rc = launch_ac_tables(ctx, w, d_pair.p, 1, d_vlog10.p, d_logc_n.p);
+  if (rc) return rc;
+  rc = debug_acransac_score(ctx, w, model, d_pair.p, d_x1.p, d_x2.p, x3 ? d_x3.p : nullptr, d_logc_n.p, d_logc_k.p, d_models.p,
+                            n_models, M, d_se.p, d_si.p, d_out.p, nper ? d_lo.p : nullptr, nper ? d_hi.p : nullptr,
+                            nper ? d_e.p : nullptr);
+  if (rc) return rc;
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(out, d_out.p, (size_t)n_models * sizeof(r3d_ac_score), cudaMemcpyDeviceToHost, w.stream));
+  if (nper) {
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(lo, d_lo.p, nper * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(hi, d_hi.p, nper * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(e, d_e.p, nper * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  }
+  if (logc_n) R3D_CUDA_TRY(ctx, cudaMemcpyAsync(logc_n, d_logc_n.p, ((size_t)M + 2) * sizeof(float), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+  if (logc_k) std::memcpy(logc_k, hlogc_k.data(), hlogc_k.size() * sizeof(float));
+  return R3D_OK;
+}
 
 extern "C" int r3d_filter_pairs(r3d_ctx* ctx, int model, double precision_px, uint32_t max_iter, const r3d_matches* putative,
                                 const r3d_view_info* views, uint32_t n_views, r3d_matches** out) {

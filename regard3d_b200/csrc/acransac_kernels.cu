@@ -214,3 +214,38 @@ int launch_f7_inliers(r3d_ctx* ctx, DeviceWorker& w, int model, const AcPair* pa
 }
 
 }  // namespace r3d
+
+// ---- r3d_debug_detmath: the deterministic transcendentals on the device and in this translation unit's host code ----
+namespace r3d {
+namespace {
+
+R3D_HD double detmath_eval(int fn, double x) {
+  return fn == 0 ? dm::log10_det(x) : fn == 1 ? dm::cbrt_det(x) : fn == 2 ? dm::cos_det(x) : dm::acos_det(x);
+}
+
+__global__ void k_debug_detmath(int fn, const double* __restrict__ x, uint64_t n, double* __restrict__ y) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x)
+    y[i] = detmath_eval(fn, x[i]);
+}
+
+}  // namespace
+}  // namespace r3d
+
+extern "C" int r3d_debug_detmath(int fn, int on_device, const double* x, uint64_t n, double* y) {
+  if (fn < 0 || fn > 3 || (n && (!x || !y))) return r3d::fail(nullptr, R3D_ERR_INVALID, "r3d_debug_detmath: bad arguments");
+  if (!on_device) {
+    for (uint64_t i = 0; i < n; ++i) y[i] = r3d::detmath_eval(fn, x[i]);
+    return R3D_OK;
+  }
+  if (!n) return R3D_OK;
+  double* d = nullptr;
+  cudaError_t e = cudaMalloc(&d, 2 * n * sizeof(double));
+  if (e == cudaSuccess) e = cudaMemcpy(d, x, n * sizeof(double), cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) {
+    r3d::k_debug_detmath<<<(unsigned)std::min<uint64_t>((n + 255) / 256, 4096), 256>>>(fn, d, n, d + n);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpy(y, d + n, n * sizeof(double), cudaMemcpyDeviceToHost);
+  if (d) cudaFree(d);
+  return e == cudaSuccess ? R3D_OK : r3d::fail(nullptr, R3D_ERR_CUDA, std::string("r3d_debug_detmath: ") + cudaGetErrorString(e));
+}

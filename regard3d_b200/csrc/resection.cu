@@ -362,17 +362,8 @@ int resect_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_resection_view* views,
     std::memcpy(&hX[3 * (size_t)hpairs[a].pt_ofs], X + 3 * v.first, 3 * v.count * sizeof(double));
     std::memcpy(&hx[2 * (size_t)hpairs[a].pt_ofs], x + 2 * v.first, 2 * v.count * sizeof(double));
   });
-  std::vector<float> vlog10(maxM + 2);
-  for (uint32_t k = 0; k <= maxM + 1; ++k) vlog10[k] = std::log10((float)k);
-  std::vector<float> hlogc_k(maxM + 1, 0.f);  // makelogcombi_k: log10 C(n, 3) as the running float sum upstream builds
-  for (uint32_t m = 0; m <= maxM; ++m) {
-    uint32_t k = ac_min_samples(3);
-    if (k >= m) continue;
-    if (m - k < k) k = m - k;
-    float r = 0.f;
-    for (uint32_t i = 1; i <= k; ++i) r += vlog10[m - i + 1] - vlog10[i];
-    hlogc_k[m] = r;
-  }
+  const std::vector<float> vlog10 = ac_vlog10(maxM);
+  const std::vector<float> hlogc_k = ac_logc_k(ac_min_samples(3), vlog10, maxM);
   // ---- size classes of the persistent kernel (shared-memory sort capacity 1024 ... 16384, beyond: global scratch) ----
   constexpr int kClasses = 6;
   std::vector<uint32_t> order[kClasses], horder;
