@@ -639,6 +639,28 @@ int r3d_debug_cholesky(r3d_ctx* ctx, int method, int n, const double* A, const i
  * A is not positive definite. */
 int r3d_debug_chol_solve3(r3d_ctx* ctx, int n, const double* A, const double* Y, int grid, double* X_out);
 
+/* Diagnostics (device): one bundle-adjustment LM step at the problem's parameters, through the code r3d_bundle_adjust
+ * runs per iteration, with the Jacobi scaling made at those parameters.  nB = 6 n_cams (+ 6 n_intr when
+ * refine_intrinsics), nparam = nB + 3 n_pts; parameter order: poses, intrinsic groups, points.  Array outputs are
+ * caller-allocated, NULL ones are skipped; the scalars are always filled. */
+typedef struct {
+  double* g;        /* nparam: scaled gradient J^T r (Huber-corrected, Jacobi-scaled) */
+  double* diag;     /* nparam: scaled diag(J^T J) */
+  double* scale;    /* nparam: Jacobi scaling 1 / (1 + |column|) */
+  double* S;        /* nB x nB: the reduced camera system, both triangles, with D^2 = clamp(diag, 1e-6, 1e32) / radius */
+  double* rhs;      /* nB: its right-hand side */
+  double* Vinv;     /* n_pts x 9: (sum Jp^T Jp + D^2)^-1 per point */
+  double* delta;    /* nparam: the step (scaled coordinates) */
+  uint32_t nB, n_batches, n_long;  /* the batched Schur kernel's CTAs, the points of the CTA-per-point kernel */
+  int not_pd;       /* the Cholesky met a pivot that is not > 0 */
+  double gmax, model_cost_change, dx_norm2, x_norm2;  /* max |unscaled g|, model cost change, |dx|^2, |x|^2 */
+} r3d_ba_step_out;
+/* schur_route 0 = the default plan (batched kernel where it applies), 1 = every point through the CTA-per-point kernel
+ * (as R3D_BA_SCHUR=point); chol_method 0 = dense, 1 = envelope (R3D_ERR_INVALID where that kernel does not apply).
+ * Uses opt->huber_a, refine_intrinsics and prior_huber_a. */
+int r3d_debug_ba_step(r3d_ctx* ctx, const r3d_ba_problem* p, const r3d_ba_options* opt, double radius, int schur_route,
+                      int chol_method, r3d_ba_step_out* out);
+
 #ifdef __cplusplus
 }
 #endif

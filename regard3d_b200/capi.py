@@ -38,10 +38,12 @@ EXPORTS = [
     "r3d_resection_default_options", "r3d_resect_views", "r3d_sfm_resect_views", "r3d_get_resection_timing",
     "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_matches_keep_largest_biedge_component",
     "r3d_transavg_default_options", "r3d_translation_averaging", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
-    "r3d_debug_acransac_score", "r3d_debug_detmath",
+    "r3d_debug_acransac_score", "r3d_debug_detmath", "r3d_debug_ba_step",
 ]
 
 CHOL_DENSE, CHOL_ENVELOPE = 0, 1
+# r3d_debug_ba_step: the Schur route (default plan, or every point through the CTA-per-point kernel)
+SCHUR_PLAN, SCHUR_CTA = 0, 1
 # r3d_ac_score: one model's scores from r3d_debug_acransac_score
 ac_score_dtype = np.dtype([("lb", np.float64), ("nfa", np.float64), ("err", np.float64), ("cnt_hi", np.uint32),
                            ("cnt_lo", np.uint32), ("count", np.uint32), ("k", np.uint32)])
@@ -107,6 +109,13 @@ class BASummary(C.Structure):
     _fields_ = [("iterations", C.c_uint32), ("successful_steps", C.c_uint32), ("initial_cost", C.c_double),
                 ("final_cost", C.c_double), ("termination", C.c_int), ("seconds_total", C.c_double),
                 ("seconds_linear", C.c_double), ("seconds_setup", C.c_double)]
+
+
+class BAStepOut(C.Structure):
+    _fields_ = [("g", C.c_void_p), ("diag", C.c_void_p), ("scale", C.c_void_p), ("S", C.c_void_p), ("rhs", C.c_void_p),
+                ("Vinv", C.c_void_p), ("delta", C.c_void_p), ("nB", C.c_uint32), ("n_batches", C.c_uint32),
+                ("n_long", C.c_uint32), ("not_pd", C.c_int), ("gmax", C.c_double), ("model_cost_change", C.c_double),
+                ("dx_norm2", C.c_double), ("x_norm2", C.c_double)]
 
 
 class RelposeOptions(C.Structure):
@@ -992,6 +1001,27 @@ class Context:
         self._check(lib().r3d_bundle_adjust(self._h, C.byref(s), C.byref(o), C.byref(summ), _p(trace)))
         d = {k: getattr(summ, k) for k, _ in BASummary._fields_}
         return d, trace[: summ.iterations + 1].copy()
+
+    def debug_ba_step(self, p, radius, huber_a=16.0, refine_intrinsics=1, prior_huber_a=0.0, route=SCHUR_PLAN,
+                      chol=CHOL_DENSE):
+        """r3d_debug_ba_step: one LM step of bundle_adjust at p's parameters (p is not changed) and trust-region radius
+        `radius`.  Returns a dict: g, diag, scale, delta (nparam = nB + 3 n_pts), S (nB x nB), rhs (nB), Vinv
+        (n_pts x 3 x 3), and nB, n_batches, n_long, not_pd, gmax, model_cost_change, dx_norm2, x_norm2."""
+        o = BAOptions()
+        lib().r3d_ba_default_options(C.byref(o))
+        o.huber_a, o.refine_intrinsics, o.prior_huber_a = huber_a, refine_intrinsics, prior_huber_a
+        s = self._ba_struct(p)
+        nB = 6 * s.n_cams + (6 * s.n_intr if refine_intrinsics else 0)
+        nparam = nB + 3 * s.n_pts
+        r = {k: np.empty(nparam) for k in ("g", "diag", "scale", "delta")}
+        r["S"], r["rhs"], r["Vinv"] = np.empty((nB, nB)), np.empty(nB), np.empty((s.n_pts, 3, 3))
+        out = BAStepOut(**{k: v.ctypes.data for k, v in r.items()})
+        self._check(lib().r3d_debug_ba_step(self._h, C.byref(s), C.byref(o), C.c_double(radius), C.c_int(route), C.c_int(chol),
+                                            C.byref(out)))
+        for k in ("nB", "n_batches", "n_long", "gmax", "model_cost_change", "dx_norm2", "x_norm2"):
+            r[k] = getattr(out, k)
+        r["not_pd"] = bool(out.not_pd)
+        return r
 
     # ---- multi-GPU bundle adjustment: one process per GPU, points partitioned (sharding.partition_ba) ----
     def comm_unique_id(self):

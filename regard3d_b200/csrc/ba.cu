@@ -949,12 +949,16 @@ __global__ void __launch_bounds__(kEnvThreads, 1) k_chol_envelope(double* A, dou
 }
 
 // ---- back substitution ---------------------------------------------------------------------------
-__global__ void __launch_bounds__(128) k_ba_backsub(Dev d) {
+__global__ void __launch_bounds__(128) k_ba_backsub(Dev d, double inv_radius) {
   const uint32_t ip = blockIdx.x * blockDim.x + threadIdx.x;
   if (ip >= d.n_pts) return;
   const size_t pcol = (size_t)d.nB + 3 * (size_t)ip;
+  const uint32_t b = d.pt_ofs[ip], e = d.pt_ofs[ip + 1];
+  if (b == e) {  // no observation, so no Schur kernel visits the point: V = D^2 (its g_p is 0, so is its step)
+    for (int i = 0; i < 9; ++i) d.Vinv[9 * (size_t)ip + i] = (i % 4) ? 0.0 : 1.0 / (fmin(fmax(d.diag[pcol + i / 4], 1e-6), 1e32) * inv_radius);
+  }
   double t3[3] = {-d.g[pcol], -d.g[pcol + 1], -d.g[pcol + 2]};
-  for (uint32_t t = d.pt_ofs[ip]; t < d.pt_ofs[ip + 1]; ++t) {
+  for (uint32_t t = b; t < e; ++t) {
     double Jc[12], Jg[12], Jp[6], r[2];
     uint32_t cc;
     int cg;
@@ -1384,6 +1388,161 @@ int setup_problem(r3d_ctx* ctx, DeviceWorker& w, const r3d_ba_problem* p, Device
   return R3D_OK;
 }
 
+enum CholChoice { kCholDense, kCholEnvelope, kCholAuto };
+
+struct StepPlan {  // what one LM step needs beyond Dev: the Schur plan, the CTA kernel's scratch, the Cholesky's
+  BatchPlan plan;
+  uint32_t long_grid = 0;
+  double* long_scr = nullptr;
+  int* long_cols = nullptr;
+  double *Lm = nullptr, *Linv = nullptr;
+  bool use_env = false;
+  int env_ctas = r3d::ba::kEnvMaxCluster;  // CTAs of the envelope kernel's cluster
+  int* ft = nullptr;
+};
+
+// after setup_problem(..., &s.plan): scratch of both Schur kernels and of the linear solve; the Cholesky kernel
+// (envelope only where its active-tile limit holds)
+int setup_step(r3d_ctx* ctx, DeviceWorker& w, const r3d_ba_problem* p, DeviceArrays& mem, const Dev& d, CholChoice chol,
+               StepPlan& s) {
+  int rc;
+  const BatchPlan& plan = s.plan;
+  if (plan.n_batches)
+    R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(r3d::ba::k_ba_schur_batched, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                           (int)r3d::ba::kBatchSmemBytes));
+  // scratch of the CTA-per-point kernel: one slice of `long_cap` observations per CTA of its (persistent) grid
+  if (plan.n_long) {
+    s.long_grid = std::min<uint32_t>(plan.n_long, (uint32_t)w.sm_count * 8u);
+    const size_t per_cta = (size_t)plan.long_cap * (r3d::ba::kObsDoubles + 36);
+    // keep the scratch within ~1 GB whatever the track length
+    while (s.long_grid > 1 && per_cta * s.long_grid * sizeof(double) > ((size_t)1 << 30)) s.long_grid /= 2;
+    R3D_CUDA_TRY(ctx, mem.alloc(&s.long_scr, per_cta * s.long_grid));
+    R3D_CUDA_TRY(ctx, mem.alloc(&s.long_cols, (size_t)plan.long_cap * 3 * s.long_grid));
+  }
+  const int nB = (int)d.nB;
+  // Cholesky scratch: L (with the forward-substituted rhs as row nB) and the inverses of its diagonal blocks
+  const int chol_blocks = (nB + r3d::ba::NB - 1) / r3d::ba::NB;
+  R3D_CUDA_TRY(ctx, mem.alloc(&s.Lm, ((size_t)nB + 1) * nB + 64));
+  R3D_CUDA_TRY(ctx, mem.alloc(&s.Linv, (size_t)chol_blocks * r3d::ba::NB * r3d::ba::NB));
+  // Envelope of the reduced system at tile granularity (the union over ranks: every rank factors the summed S)
+  const int ntr = (nB + 1 + r3d::ba::NB - 1) / r3d::ba::NB;
+  std::vector<double> fc(p->n_cams);
+  for (uint32_t c = 0; c < p->n_cams; ++c) fc[c] = -(double)plan.first_cam[c];
+  if (ctx->comm_world > 1 && p->n_cams) {  // min over ranks = -max(-x)
+    double* d_fc = nullptr;
+    R3D_CUDA_TRY(ctx, mem.alloc(&d_fc, p->n_cams));
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_fc, fc.data(), (size_t)p->n_cams * 8, cudaMemcpyHostToDevice, w.stream));
+    if ((rc = comm_allreduce(ctx, w.stream, d_fc, p->n_cams, kCommMax))) return rc;
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(fc.data(), d_fc, (size_t)p->n_cams * 8, cudaMemcpyDeviceToHost, w.stream));
+    R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+  }
+  std::vector<int> ft(ntr, 0);
+  for (int ti = 0; ti < ntr; ++ti) {
+    int first = ti * r3d::ba::NB;
+    for (int r = ti * r3d::ba::NB; r < std::min((ti + 1) * r3d::ba::NB, nB + 1); ++r) {
+      const int fcol = r < 6 * (int)p->n_cams ? 6 * (int)(-fc[r / 6]) : 0;  // intrinsics rows, rhs row: from column 0
+      first = std::min(first, fcol);
+    }
+    ft[ti] = first / r3d::ba::NB;
+  }
+  // per panel: active row tiles -> tile pairs; compare with the dense kernel's two grid barriers + full trailing update
+  {
+    const char* e = getenv("R3D_BA_ENV_CTAS");
+    if (e && atoi(e) >= 1 && atoi(e) <= r3d::ba::kEnvMaxCluster) s.env_ctas = atoi(e);
+  }
+  int max_act = 0;
+  double est_env = 0.0, est_dense = 0.0;
+  for (int k = 0; k < chol_blocks; ++k) {
+    int act = 0;
+    for (int ti = k + 1; ti < ntr; ++ti) act += ft[ti] <= k;
+    max_act = std::max(max_act, act);
+    est_env += 32.0 + 5.0 * std::ceil((double)(act * (act + 1) / 2) / (16.0 * s.env_ctas)) + 0.6 * act;
+    const int rem = ntr - k - 1;
+    est_dense += 20.0 + 3.0 * std::ceil((double)(rem * (rem + 1) / 2) / (4.0 * w.sm_count));
+  }
+  // Measured at C5 (profiles/r02_ba_cholesky_ab.md): the envelope kernel does 7x fewer tile products but its panels
+  // cost 54 us on 8 SMs (register potrf 8, redundant trsm 10 -- shared-memory instruction issue --, fp64 syrk on 8 SMs
+  // 20, cluster barrier 14) against 29 us for the dense cooperative kernel on 148 SMs, so the dense kernel stays the
+  // default; R3D_BA_CHOL=envelope selects the envelope kernel where it applies (A/B and tests), =auto trusts the
+  // estimate.
+  s.use_env = false;
+  if (chol == kCholAuto) s.use_env = max_act <= r3d::ba::kEnvMaxActive && est_env < est_dense;
+  if (chol == kCholEnvelope) s.use_env = max_act <= r3d::ba::kEnvMaxActive;
+  if (s.use_env) {
+    R3D_CUDA_TRY(ctx, mem.alloc(&s.ft, (size_t)ntr));
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(s.ft, ft.data(), (size_t)ntr * sizeof(int), cudaMemcpyHostToDevice, w.stream));
+    R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));  // ft is a local
+  }
+  static const bool dbg = getenv("R3D_DEBUG_TIMING") != nullptr;
+  if (dbg) fprintf(stderr, "[r3d] BA linear solve: %s (n = %d, %d tiles, <= %d active row tiles per panel, estimate %.0f vs %.0f us dense)\n",
+                   s.use_env ? "envelope Cholesky, one cluster" : "dense cooperative Cholesky", nB, ntr, max_act, est_env, est_dense);
+  return R3D_OK;
+}
+
+int read_scal(r3d_ctx* ctx, DeviceWorker& w, const Dev& d, double* h_scal) {
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(h_scal, d.scal, 8 * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+  return R3D_OK;
+}
+
+// gradient + diag at the current parameters (scaled; the Jacobi scaling itself is made from this diag when
+// make_scale), and the largest unscaled gradient component
+int ba_evaluate(r3d_ctx* ctx, DeviceWorker& w, const Dev& d, bool make_scale, double* gmax) {
+  int rc;
+  const size_t nparam = (size_t)d.nB + 3 * (size_t)d.n_pts;
+  const int nB = (int)d.nB;
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.gu, 0, nparam * 8, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.du, 0, nparam * 8, w.stream));
+  r3d::ba::k_ba_eval<<<w.sm_count * 8, 256, 0, w.stream>>>(d);
+  if (d.n_priors && d.owns_shared) r3d::ba::k_ba_priors<<<(d.n_priors + 127) / 128, 128, 0, w.stream>>>(d, d.poses, 1, nullptr);
+  // camera / intrinsic gradient and column norms are sums over every rank's observations
+  if ((rc = comm_allreduce(ctx, w.stream, d.gu, nB, kCommSum))) return rc;
+  if ((rc = comm_allreduce(ctx, w.stream, d.du, nB, kCommSum))) return rc;
+  if (make_scale) r3d::ba::k_ba_make_scale<<<(unsigned)((nparam + 255) / 256), 256, 0, w.stream>>>(d.scale, d.du, nparam);
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.scal + 5, 0, sizeof(double), w.stream));
+  r3d::ba::k_ba_apply_scale<<<(unsigned)((nparam + 255) / 256), 256, 0, w.stream>>>(d.scale, d.gu, d.du, d.g, d.diag, nparam, d.scal + 5);
+  R3D_CUDA_TRY(ctx, cudaGetLastError());
+  if ((rc = comm_allreduce(ctx, w.stream, d.scal + 5, 1, kCommMax))) return rc;
+  double h_scal[8];
+  if ((rc = read_scal(ctx, w, d, h_scal))) return rc;
+  *gmax = h_scal[5];
+  return R3D_OK;
+}
+
+// One LM step at trust-region radius 1 / inv_radius: the reduced camera system S | rhs (Schur kernels, prior U blocks,
+// k_ba_finish_S), its Cholesky solve, the point back-substitution and the candidate parameters; d.scal[1..4] =
+// 2 * model cost change, |dx|^2, |x|^2, not-PD flag.  S_copy (nB * nB + nB, or nullptr) receives S | rhs before the
+// factorisation overwrites it.
+int ba_step(r3d_ctx* ctx, DeviceWorker& w, const Dev& d, const StepPlan& s, double inv_radius, double* S_copy) {
+  int rc;
+  const int nB = (int)d.nB;
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.S, 0, ((size_t)nB * nB + nB) * 8, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.scal, 0, 5 * sizeof(double), w.stream));
+  if (s.plan.n_batches)
+    r3d::ba::k_ba_schur_batched<<<s.plan.n_batches, 256, r3d::ba::kBatchSmemBytes, w.stream>>>(d, s.plan.t, inv_radius);
+  if (s.plan.n_long)  // long tracks and whatever else the batched kernel cannot take
+    r3d::ba::k_ba_schur_cta<<<s.long_grid, r3d::ba::kCtaThreads, 0, w.stream>>>(d, s.plan.d_long, s.plan.n_long, inv_radius,
+                                                                               s.long_scr, s.long_cols, s.plan.long_cap);
+  if (d.n_priors && d.owns_shared) r3d::ba::k_ba_priors<<<(d.n_priors + 127) / 128, 128, 0, w.stream>>>(d, d.poses, 2, nullptr);
+  // the exchange step: partial reduced camera systems of the point partitions -> their sum (NVLink)
+  if ((rc = comm_allreduce(ctx, w.stream, d.S, (size_t)nB * nB + nB, kCommSum))) return rc;
+  {
+    dim3 b(32, 8), g((nB + 31) / 32, (nB + 7) / 8);
+    r3d::ba::k_ba_finish_S<<<g, b, 0, w.stream>>>(d, inv_radius);
+  }
+  if (S_copy)
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(S_copy, d.S, ((size_t)nB * nB + nB) * 8, cudaMemcpyDeviceToDevice, w.stream));
+  if (s.use_env) {
+    if ((rc = envelope_cholesky(ctx, w, d.S, s.Lm, nB, s.ft, s.env_ctas, d.scal + 4, d.delta))) return rc;
+  } else {
+    if ((rc = dense_cholesky(ctx, w, d.S, s.Lm, s.Linv, nB, d.scal + 4, d.delta))) return rc;
+  }
+  r3d::ba::k_ba_backsub<<<(d.n_pts + 127) / 128, 128, 0, w.stream>>>(d, inv_radius);
+  r3d::ba::k_ba_update<<<w.sm_count * 4, 256, 0, w.stream>>>(d, inv_radius);
+  R3D_CUDA_TRY(ctx, cudaGetLastError());
+  return comm_allreduce(ctx, w.stream, d.scal + 1, 3, kCommSum);
+}
+
 }  // namespace
 
 extern "C" {
@@ -1426,101 +1585,21 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
   DeviceArrays mem;
   mem.w = &w;
   Dev d;
-  uint32_t max_obs = 1;
-  BatchPlan plan;
+  StepPlan sp;
   static const bool per_point_schur = getenv("R3D_BA_SCHUR") && std::string(getenv("R3D_BA_SCHUR")) == "point";
-  plan.want_batched = !per_point_schur;
-  int rc = setup_problem(ctx, w, p, mem, d, opt->refine_intrinsics != 0, opt->huber_a, true, &max_obs, &plan);
+  sp.plan.want_batched = !per_point_schur;
+  int rc = setup_problem(ctx, w, p, mem, d, opt->refine_intrinsics != 0, opt->huber_a, true, nullptr, &sp.plan);
   if (rc) return rc;
   d.prior_huber_a = opt->prior_huber_a;
-  if (plan.n_batches)
-    R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(r3d::ba::k_ba_schur_batched, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                           (int)r3d::ba::kBatchSmemBytes));
-  // scratch of the CTA-per-point kernel: one slice of `long_cap` observations per CTA of its (persistent) grid
-  uint32_t long_grid = 0;
-  double* d_long_scr = nullptr;
-  int* d_long_cols = nullptr;
-  if (plan.n_long) {
-    long_grid = std::min<uint32_t>(plan.n_long, (uint32_t)w.sm_count * 8u);
-    const size_t per_cta = (size_t)plan.long_cap * (r3d::ba::kObsDoubles + 36);
-    // keep the scratch within ~1 GB whatever the track length
-    while (long_grid > 1 && per_cta * long_grid * sizeof(double) > ((size_t)1 << 30)) long_grid /= 2;
-    R3D_CUDA_TRY(ctx, mem.alloc(&d_long_scr, per_cta * long_grid));
-    R3D_CUDA_TRY(ctx, mem.alloc(&d_long_cols, (size_t)plan.long_cap * 3 * long_grid));
+  {
+    const char* force = getenv("R3D_BA_CHOL");
+    const CholChoice chol = !force ? kCholDense : std::string(force) == "auto" ? kCholAuto
+                          : std::string(force) == "envelope" ? kCholEnvelope : kCholDense;
+    if ((rc = setup_step(ctx, w, p, mem, d, chol, sp))) return rc;
   }
   sum->seconds_setup = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
-  const size_t nparam = (size_t)d.nB + 3 * (size_t)d.n_pts;
   const int grid_obs = w.sm_count * 8;
-  const int nB = (int)d.nB;
-  // Cholesky scratch: L (with the forward-substituted rhs as row nB) and the inverses of its diagonal blocks
-  double *d_Lm = nullptr, *d_Linv = nullptr;
-  const int chol_blocks = (nB + r3d::ba::NB - 1) / r3d::ba::NB;
-  R3D_CUDA_TRY(ctx, mem.alloc(&d_Lm, ((size_t)nB + 1) * nB + 64));
-  R3D_CUDA_TRY(ctx, mem.alloc(&d_Linv, (size_t)chol_blocks * r3d::ba::NB * r3d::ba::NB));
-  // Envelope of the reduced system at tile granularity (the union over ranks: every rank factors the summed S)
-  bool use_env = false;
-  int env_ctas = r3d::ba::kEnvMaxCluster;  // CTAs of the envelope kernel's cluster
-  int* d_ft = nullptr;
-  {
-    const int ntr = (nB + 1 + r3d::ba::NB - 1) / r3d::ba::NB;
-    std::vector<double> fc(p->n_cams);
-    for (uint32_t c = 0; c < p->n_cams; ++c) fc[c] = -(double)plan.first_cam[c];
-    if (ctx->comm_world > 1 && p->n_cams) {  // min over ranks = -max(-x)
-      double* d_fc = nullptr;
-      R3D_CUDA_TRY(ctx, mem.alloc(&d_fc, p->n_cams));
-      R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_fc, fc.data(), (size_t)p->n_cams * 8, cudaMemcpyHostToDevice, w.stream));
-      if ((rc = comm_allreduce(ctx, w.stream, d_fc, p->n_cams, kCommMax))) return rc;
-      R3D_CUDA_TRY(ctx, cudaMemcpyAsync(fc.data(), d_fc, (size_t)p->n_cams * 8, cudaMemcpyDeviceToHost, w.stream));
-      R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-    }
-    std::vector<int> ft(ntr, 0);
-    for (int ti = 0; ti < ntr; ++ti) {
-      int first = ti * r3d::ba::NB;
-      for (int r = ti * r3d::ba::NB; r < std::min((ti + 1) * r3d::ba::NB, nB + 1); ++r) {
-        const int fcol = r < 6 * (int)p->n_cams ? 6 * (int)(-fc[r / 6]) : 0;  // intrinsics rows, rhs row: from column 0
-        first = std::min(first, fcol);
-      }
-      ft[ti] = first / r3d::ba::NB;
-    }
-    // per panel: active row tiles -> tile pairs; compare with the dense kernel's two grid barriers + full trailing update
-    {
-      const char* e = getenv("R3D_BA_ENV_CTAS");
-      if (e && atoi(e) >= 1 && atoi(e) <= r3d::ba::kEnvMaxCluster) env_ctas = atoi(e);
-    }
-    int max_act = 0;
-    double est_env = 0.0, est_dense = 0.0;
-    for (int k = 0; k < chol_blocks; ++k) {
-      int act = 0;
-      for (int ti = k + 1; ti < ntr; ++ti) act += ft[ti] <= k;
-      max_act = std::max(max_act, act);
-      est_env += 32.0 + 5.0 * std::ceil((double)(act * (act + 1) / 2) / (16.0 * env_ctas)) + 0.6 * act;
-      const int rem = ntr - k - 1;
-      est_dense += 20.0 + 3.0 * std::ceil((double)(rem * (rem + 1) / 2) / (4.0 * w.sm_count));
-    }
-    // Measured at C5 (profiles/r02_ba_cholesky_ab.md): the envelope kernel does 7x fewer tile products but its panels
-    // cost 54 us on 8 SMs (register potrf 8, redundant trsm 10 -- shared-memory instruction issue --, fp64 syrk on 8 SMs
-    // 20, cluster barrier 14) against 29 us for the dense cooperative kernel on 148 SMs, so the dense kernel stays the
-    // default; R3D_BA_CHOL=envelope selects the envelope kernel where it applies (A/B and tests), =auto trusts the
-    // estimate.
-    const char* force = getenv("R3D_BA_CHOL");
-    use_env = false;
-    if (force && std::string(force) == "auto") use_env = max_act <= r3d::ba::kEnvMaxActive && est_env < est_dense;
-    if (force && std::string(force) == "envelope") use_env = max_act <= r3d::ba::kEnvMaxActive;
-    if (use_env) {
-      R3D_CUDA_TRY(ctx, mem.alloc(&d_ft, (size_t)ntr));
-      R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_ft, ft.data(), (size_t)ntr * sizeof(int), cudaMemcpyHostToDevice, w.stream));
-      R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));  // ft is a local
-    }
-    static const bool dbg = getenv("R3D_DEBUG_TIMING") != nullptr;
-    if (dbg) fprintf(stderr, "[r3d] BA linear solve: %s (n = %d, %d tiles, <= %d active row tiles per panel, estimate %.0f vs %.0f us dense)\n",
-                     use_env ? "envelope Cholesky, one cluster" : "dense cooperative Cholesky", nB, ntr, max_act, est_env, est_dense);
-  }
   double h_scal[8];
-  auto read_scal = [&]() -> int {
-    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(h_scal, d.scal, 8 * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
-    R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-    return R3D_OK;
-  };
   auto eval_cost = [&](const double* poses, const double* intr, const double* pts, double* out) -> int {
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.scal, 0, sizeof(double), w.stream));
     r3d::ba::k_ba_cost<<<grid_obs, 256, 0, w.stream>>>(d, poses, intr, pts, d.scal);
@@ -1528,32 +1607,11 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
       r3d::ba::k_ba_priors<<<(d.n_priors + 127) / 128, 128, 0, w.stream>>>(d, poses, 0, d.scal);
     R3D_CUDA_TRY(ctx, cudaGetLastError());
     if ((rc = comm_allreduce(ctx, w.stream, d.scal, 1, kCommSum))) return rc;
-    if ((rc = read_scal())) return rc;
+    if ((rc = read_scal(ctx, w, d, h_scal))) return rc;
     *out = h_scal[0];
     return R3D_OK;
   };
-  bool have_scale = false;
   double gmax = 0;
-  auto evaluate = [&]() -> int {  // gradient + diag at the current parameters
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.gu, 0, nparam * 8, w.stream));
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.du, 0, nparam * 8, w.stream));
-    r3d::ba::k_ba_eval<<<grid_obs, 256, 0, w.stream>>>(d);
-    if (d.n_priors && d.owns_shared) r3d::ba::k_ba_priors<<<(d.n_priors + 127) / 128, 128, 0, w.stream>>>(d, d.poses, 1, nullptr);
-    // camera / intrinsic gradient and column norms are sums over every rank's observations
-    if ((rc = comm_allreduce(ctx, w.stream, d.gu, nB, kCommSum))) return rc;
-    if ((rc = comm_allreduce(ctx, w.stream, d.du, nB, kCommSum))) return rc;
-    if (!have_scale) {
-      r3d::ba::k_ba_make_scale<<<(unsigned)((nparam + 255) / 256), 256, 0, w.stream>>>(d.scale, d.du, nparam);
-      have_scale = true;
-    }
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.scal + 5, 0, sizeof(double), w.stream));
-    r3d::ba::k_ba_apply_scale<<<(unsigned)((nparam + 255) / 256), 256, 0, w.stream>>>(d.scale, d.gu, d.du, d.g, d.diag, nparam, d.scal + 5);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    if ((rc = comm_allreduce(ctx, w.stream, d.scal + 5, 1, kCommMax))) return rc;
-    if ((rc = read_scal())) return rc;
-    gmax = h_scal[5];
-    return R3D_OK;
-  };
 
   double cost = 0;
   if ((rc = eval_cost(d.poses, d.intr, d.pts, &cost))) return rc;
@@ -1561,36 +1619,13 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
   sum->seconds_linear = 0;
   if (cost_trace) cost_trace[0] = cost;
   r3d::LmTrustRegion lm(r3d::lm_params(*opt));
-  if ((rc = evaluate())) return rc;
+  if ((rc = ba_evaluate(ctx, w, d, true, &gmax))) return rc;  // the Jacobi scaling is fixed at the initial parameters
   const bool stop = lm.start(gmax);
   for (uint32_t iter = 1; !stop && iter <= opt->max_iterations; ++iter) {
     lm.iterations = iter;
     const auto t_lin = std::chrono::steady_clock::now();
-    const double inv_radius = 1.0 / lm.radius;
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.S, 0, ((size_t)nB * nB + nB) * 8, w.stream));
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d.scal, 0, 5 * sizeof(double), w.stream));
-    if (plan.n_batches)
-      r3d::ba::k_ba_schur_batched<<<plan.n_batches, 256, r3d::ba::kBatchSmemBytes, w.stream>>>(d, plan.t, inv_radius);
-    if (plan.n_long)  // long tracks and whatever else the batched kernel cannot take
-      r3d::ba::k_ba_schur_cta<<<long_grid, r3d::ba::kCtaThreads, 0, w.stream>>>(d, plan.d_long, plan.n_long, inv_radius, d_long_scr,
-                                                                             d_long_cols, plan.long_cap);
-    if (d.n_priors && d.owns_shared) r3d::ba::k_ba_priors<<<(d.n_priors + 127) / 128, 128, 0, w.stream>>>(d, d.poses, 2, nullptr);
-    // the exchange step: partial reduced camera systems of the point partitions -> their sum (NVLink)
-    if ((rc = comm_allreduce(ctx, w.stream, d.S, (size_t)nB * nB + nB, kCommSum))) return rc;
-    {
-      dim3 b(32, 8), g((nB + 31) / 32, (nB + 7) / 8);
-      r3d::ba::k_ba_finish_S<<<g, b, 0, w.stream>>>(d, inv_radius);
-    }
-    if (use_env) {
-      if ((rc = envelope_cholesky(ctx, w, d.S, d_Lm, nB, d_ft, env_ctas, d.scal + 4, d.delta))) return rc;
-    } else {
-      if ((rc = dense_cholesky(ctx, w, d.S, d_Lm, d_Linv, nB, d.scal + 4, d.delta))) return rc;
-    }
-    r3d::ba::k_ba_backsub<<<(d.n_pts + 127) / 128, 128, 0, w.stream>>>(d);
-    r3d::ba::k_ba_update<<<w.sm_count * 4, 256, 0, w.stream>>>(d, inv_radius);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    if ((rc = comm_allreduce(ctx, w.stream, d.scal + 1, 3, kCommSum))) return rc;
-    if ((rc = read_scal())) return rc;
+    if ((rc = ba_step(ctx, w, d, sp, 1.0 / lm.radius, nullptr))) return rc;
+    if ((rc = read_scal(ctx, w, d, h_scal))) return rc;
     sum->seconds_linear += std::chrono::duration<double>(std::chrono::steady_clock::now() - t_lin).count();
     const double model_cost_change = 0.5 * h_scal[1];
     bool accepted = false;
@@ -1607,7 +1642,7 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
         std::swap(d.pts, d.pts_new);
         cost = new_cost;
         if (cost_trace) cost_trace[iter] = cost;
-        if ((rc = evaluate())) return rc;
+        if ((rc = ba_evaluate(ctx, w, d, false, &gmax))) return rc;
         if (lm.converged(gmax)) break;
       }
     }
@@ -1625,6 +1660,48 @@ int r3d_bundle_adjust(r3d_ctx* ctx, r3d_ba_problem* p, const r3d_ba_options* opt
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(p->points, d.pts, 3 * (size_t)p->n_pts * 8, cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
   sum->seconds_total = std::chrono::duration<double>(std::chrono::steady_clock::now() - t_begin).count();
+  return R3D_OK;
+}
+
+int r3d_debug_ba_step(r3d_ctx* ctx, const r3d_ba_problem* p, const r3d_ba_options* opt, double radius, int schur_route,
+                      int chol_method, r3d_ba_step_out* out) {
+  if (!ctx || !p || !opt || !out || !(radius > 0.0) || (schur_route != 0 && schur_route != 1) || (chol_method != 0 && chol_method != 1))
+    return fail(ctx, R3D_ERR_INVALID, "r3d_debug_ba_step: bad arguments");
+  DeviceWorker& w = ctx->workers[0];
+  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
+  DeviceArrays mem;
+  mem.w = &w;
+  Dev d;
+  StepPlan sp;
+  sp.plan.want_batched = schur_route == 0;
+  int rc = setup_problem(ctx, w, p, mem, d, opt->refine_intrinsics != 0, opt->huber_a, true, nullptr, &sp.plan);
+  if (rc) return rc;
+  d.prior_huber_a = opt->prior_huber_a;
+  if ((rc = setup_step(ctx, w, p, mem, d, chol_method ? kCholEnvelope : kCholDense, sp))) return rc;
+  if (chol_method && !sp.use_env) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_ba_step: the envelope kernel does not take this system");
+  const size_t nB = d.nB, nparam = nB + 3 * (size_t)d.n_pts;
+  double* S_copy;
+  R3D_CUDA_TRY(ctx, mem.alloc(&S_copy, nB * nB + nB));
+  double gmax = 0.0;
+  if ((rc = ba_evaluate(ctx, w, d, true, &gmax))) return rc;
+  if ((rc = ba_step(ctx, w, d, sp, 1.0 / radius, S_copy))) return rc;
+  double h_scal[8];
+  if ((rc = read_scal(ctx, w, d, h_scal))) return rc;
+  const std::pair<double*, const double*> arrays[] = {{out->g, d.g}, {out->diag, d.diag}, {out->scale, d.scale}, {out->delta, d.delta}};
+  for (const auto& a : arrays)
+    if (a.first) R3D_CUDA_TRY(ctx, cudaMemcpyAsync(a.first, a.second, nparam * 8, cudaMemcpyDeviceToHost, w.stream));
+  if (out->S) R3D_CUDA_TRY(ctx, cudaMemcpyAsync(out->S, S_copy, nB * nB * 8, cudaMemcpyDeviceToHost, w.stream));
+  if (out->rhs) R3D_CUDA_TRY(ctx, cudaMemcpyAsync(out->rhs, S_copy + nB * nB, nB * 8, cudaMemcpyDeviceToHost, w.stream));
+  if (out->Vinv) R3D_CUDA_TRY(ctx, cudaMemcpyAsync(out->Vinv, d.Vinv, 9 * (size_t)d.n_pts * 8, cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+  out->nB = d.nB;
+  out->n_batches = sp.plan.n_batches;
+  out->n_long = sp.plan.n_long;
+  out->not_pd = h_scal[4] != 0.0;
+  out->gmax = gmax;
+  out->model_cost_change = 0.5 * h_scal[1];
+  out->dx_norm2 = h_scal[2];
+  out->x_norm2 = h_scal[3];
   return R3D_OK;
 }
 

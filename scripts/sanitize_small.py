@@ -50,6 +50,17 @@ if what in ("ba", "all"):
     s, trace = ctx.bundle_adjust(arrs, max_iterations=3)
     print("ba:", s["iterations"], "iterations, cost", trace[0], "->", trace[-1])
     ctx.ba_residuals(arrs)
+    # the CTA-per-point Schur kernel and the points no Schur kernel visits: point 0 gets a 36-observation track (every
+    # camera, camera 0 five times), one more point has no observation at all
+    extra = np.concatenate([np.arange(8), np.zeros(28, int)]).astype(np.uint32)
+    arrs["obs_cam"] = np.concatenate([arrs["obs_cam"], extra])
+    arrs["obs_pt"] = np.concatenate([arrs["obs_pt"], np.zeros(len(extra), np.uint32)])
+    arrs["obs_xy"] = np.concatenate([arrs["obs_xy"], arrs["obs_xy"][:1] + np.linspace(-1.0, 1.0, len(extra))[:, None]])
+    arrs["points"] = np.concatenate([arrs["points"], arrs["points"][:1] + 1.0])
+    s, trace = ctx.bundle_adjust(arrs, max_iterations=3)
+    print("ba (long track, repeated camera, unobserved point):", s["iterations"], "iterations, cost", trace[0], "->", trace[-1])
+    step = ctx.debug_ba_step(arrs, 1e4)
+    print("ba step: %d batches, %d CTA points, |delta| %.3g" % (step["n_batches"], step["n_long"], np.linalg.norm(step["delta"])))
 if what in ("cascade", "all"):
     s8 = synth.make_scene(3, n_feats, 128, "sift", seed=6, as_u8=True)
     ctx.clear_regions()
