@@ -577,8 +577,9 @@ int r3d_debug_post_process_many(int lanes, r3d_indmatch* const* ms, uint64_t* co
 int64_t r3d_debug_post_process_ranked(r3d_indmatch* m, int64_t n, const float* xyI, uint32_t n_keypoints, const float* xyJ);
 
 /* Diagnostics (host only): 1 when the library's device-side restatement of std::mt19937 +
- * std::uniform_int_distribution<uint32_t> (the ACRANSAC sample stream) reproduces this process's <random>; the
- * filters then run entirely on the device, otherwise samples are drawn on the host, round by round. */
+ * std::uniform_int_distribution<uint32_t> (the ACRANSAC sample stream) reproduces this process's <random>.  When it
+ * does not (another standard library), r3d_filter_pairs, r3d_relative_poses and r3d_resect_views return
+ * R3D_ERR_UNSUPPORTED. */
 int r3d_debug_rng_selftest(void);
 /* Diagnostics (device): the AC-RANSAC kernel's scoring of caller-supplied models on one pair, through the device code
  * the F / H / E filters, r3d_relative_poses and r3d_resect_views run.  model: internal id 0 = F (symmetric epipolar

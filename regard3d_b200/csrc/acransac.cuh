@@ -35,25 +35,6 @@ struct AcPointSrc {      // per pair: where its matched positions come from and 
   uint32_t nI, nJ, identity, pad_;
 };
 
-struct AcHyp {           // one RANSAC iteration of one pair
-  uint32_t pair;
-  uint32_t sample[7];
-};
-
-struct AcScore {         // per (hypothesis, model)
-  double nfa;            // best NFA over k (inf if none)
-  double err;            // residual at the best k (errorMax)
-  uint32_t k;            // best k (number of inliers)
-  uint32_t count;        // residuals <= max_thr (classic-RANSAC phase of ACRANSAC)
-};
-
-struct AcInlierReq {
-  uint32_t pair;
-  uint32_t k;            // number of inliers wanted (prefix of the sorted residuals)
-  uint32_t out_ofs;
-  uint32_t hyp_model;    // hypothesis * MAX_MODELS + model: where this round's model matrix lives on the device
-};
-
 struct AcFusedOut {      // per pair, written by the persistent kernel (acransac_fused.cu)
   double minNFA, errorMax;
   uint32_t n_inliers;    // 0 when minNFA >= 0; else the best model's inliers, listed in residual order
@@ -76,6 +57,38 @@ int launch_acransac_fused(r3d_ctx* ctx, DeviceWorker& w, int model, bool huge, c
                           const uint2* matches, uint2* out_matches, AcFusedOut* out, double* out_model, uint32_t grid,
                           const double* x3 = nullptr);
 
+// The one driver of k_acransac_fused, shared by the filters (run_fused) and resection (resect_range), in two steps so
+// that each caller times the launches alone (acransac_host.cu).  plan(): cuts the problems into size classes
+// (shared-memory sort capacity 1024 ... 16384 matches; beyond that the "huge" class sorts in global scratch), largest
+// first within a class, sizes the grid of every class, allocates the scratch and uploads the launch order;
+// R3D_ERR_UNSUPPORTED when the device sample stream disagrees with this process's <random> (rng_selftest).  launch():
+// one persistent launch per class, the huge class first, adding them to `launches`; no synchronisation.  The object
+// owns the scratch the launches use: the caller keeps it until it has synchronised w.stream.
+struct AcFused {
+  static constexpr int kClasses = 6;  // caps 1024, 2048, 4096, 8192, 16384, huge
+  int model = 0;
+  uint32_t class_ofs[kClasses + 1] = {}, caps[kClasses] = {}, grids[kClasses] = {};
+  std::vector<uint32_t> horder;       // problem ids, class after class
+  DevArr<uint32_t> order, work, si, pool;
+  DevArr<double> se;
+  explicit AcFused(DeviceWorker& w) : order(w), work(w), si(w), pool(w), se(w) {}
+  int plan(r3d_ctx* ctx, DeviceWorker& w, int model, const std::vector<AcPair>& pairs);
+  int launch(r3d_ctx* ctx, DeviceWorker& w, const AcPair* d_pairs, const double2* x1, const double2* x2, const double* x3,
+             const float* logc_n, const float* logc_k, uint32_t max_iter, const uint2* matches, uint2* out_matches,
+             AcFusedOut* out, double* out_model, uint64_t& launches);
+};
+
+// The log-combinatorial tables of a batch of problems (acransac_host.cu).  upload(): the log10 table k = 0 .. maxM + 1
+// (single precision, as upstream's makelogcombi builds it) and logc_k = makelogcombi_k, log10 C(n, ns) for n = 0 .. maxM
+// (the running float sum upstream builds), copied to the device; logc_n sized to tbl_total entries, for
+// launch_ac_tables to fill from vlog10.
+struct AcTables {
+  std::vector<float> h_vlog10, h_logc_k;
+  DevArr<float> vlog10, logc_n, logc_k;
+  explicit AcTables(DeviceWorker& w) : vlog10(w), logc_n(w), logc_k(w) {}
+  int upload(r3d_ctx* ctx, DeviceWorker& w, uint32_t ns, uint32_t maxM, uint64_t tbl_total);
+};
+
 // r3d_debug_acransac_score on one pair already on the device (acransac_fused.cu): d_pair->pt_ofs = tbl_ofs = 0,
 // d_se / d_si: debug_acransac_cap(M) entries, d_lo / d_hi / d_e: n_models x M or null
 uint32_t debug_acransac_cap(uint32_t M);
@@ -83,17 +96,12 @@ int debug_acransac_score(r3d_ctx* ctx, DeviceWorker& w, int model, const AcPair*
                          const double* d_x3, const float* d_logc_n, const float* d_logc_k, const double* d_models, uint32_t n_models,
                          uint32_t M, double* d_se, uint32_t* d_si, r3d_ac_score* d_out, double* d_lo, double* d_hi, double* d_e);
 
-// the host's log10 table k = 0 .. maxM + 1 (single precision, as upstream's makelogcombi builds it) that k_ac_tables
-// sums, and makelogcombi_k: log10 C(n, ns) for n = 0 .. maxM as the running float sum upstream builds (acransac_host.cu)
-std::vector<float> ac_vlog10(uint32_t maxM);
-std::vector<float> ac_logc_k(uint32_t ns, const std::vector<float>& vlog10, uint32_t maxM);
-
 struct AcBestModel {      // per pair of the putative map (r3d_relative_poses): the kept pair's best model, errorMax
   double model[9];       // row-major; F = K2^-T E K1^-1 for the essential model
   double errorMax;       // squared residual of the last inlier
 };
 // AC-RANSAC of the pairs [p0, p1) of a putative map on one worker (acransac_host.cu); result[p]: inliers of pair p.
-// best (may be null; device-resident path only): the best model and errorMax of every kept pair
+// best (may be null): the best model and errorMax of every kept pair
 int filter_pairs_model(r3d_ctx* ctx, DeviceWorker& w, int model, double precision_px, uint32_t max_iter, const r3d_matches* put,
                        const r3d_view_info* views, uint32_t n_views, uint64_t p0, uint64_t p1, r3d_filter_timing& T,
                        std::vector<std::vector<r3d_indmatch>>& result, std::vector<AcBestModel>* best = nullptr);
@@ -102,12 +110,5 @@ int filter_pairs_model(r3d_ctx* ctx, DeviceWorker& w, int model, double precisio
 int launch_ac_points(r3d_ctx* ctx, DeviceWorker& w, const AcPair* pairs, const AcPointSrc* src, uint32_t n_pairs,
                      const uint2* matches, double2* x1, double2* x2, uint32_t* bad_flag);
 int launch_ac_tables(r3d_ctx* ctx, DeviceWorker& w, const AcPair* pairs, uint32_t n_pairs, const float* vlog10, float* logc_n);
-int launch_f7_solve(r3d_ctx* ctx, DeviceWorker& w, int model, const AcPair* pairs, const double2* x1, const double2* x2,
-                    const AcHyp* hyps, uint32_t n_hyp, double* F, uint32_t* nmodels);
-int launch_f7_score(r3d_ctx* ctx, DeviceWorker& w, int model, const AcPair* pairs, const double2* x1, const double2* x2,
-                    const AcHyp* hyps, uint32_t n_hyp, const double* F, const uint32_t* nmodels, const float* logc_n,
-                    const float* logc_k, uint32_t cap, AcScore* scores);
-int launch_f7_inliers(r3d_ctx* ctx, DeviceWorker& w, int model, const AcPair* pairs, const double2* x1, const double2* x2,
-                      const AcInlierReq* reqs, uint32_t n_req, const double* F, uint32_t cap, uint32_t* out);
 
 }  // namespace r3d

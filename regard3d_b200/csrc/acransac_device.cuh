@@ -1,5 +1,5 @@
-// acransac_device.cuh -- device functions shared by the AC-RANSAC kernels (acransac_kernels.cu: the host-driven
-// round kernels; acransac_fused.cu: the persistent one-CTA-per-pair kernel).  Every translation unit that includes
+// acransac_device.cuh -- device functions of the AC-RANSAC kernels (acransac_fused.cu: the persistent one-CTA-per-pair
+// kernel; p3p.cuh builds on the solvers and residuals here).  Every translation unit that includes
 // this header MUST be compiled with --fmad=false (regard3d_b200/build.py): each double operation rounds once, exactly
 // like the host arithmetic of the CPU restatement, so discrete decisions are reproducible (see detmath.cuh).
 // Upstream semantics: SURVEY.md Appendix A.4-A.6.

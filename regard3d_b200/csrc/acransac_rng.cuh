@@ -8,9 +8,9 @@
 //     product = g() * range;  low = (uint32) product;
 //     if (low < range) { threshold = -range % range; while (low < threshold) { product = g() * range; low = ...; } }
 //     return (product >> 32) + a;
-// and for the full range simply g().  r3d_create() checks this restatement against the host's own <random> once
-// (rng_selftest(), context.cu); when the two disagree (another standard library) the filter keeps drawing on the host
-// (acransac_host.cu), so results never depend on this file being right for an unknown library.
+// and for the full range simply g().  rng_selftest() (acransac_fused.cu) checks this restatement against the host's own
+// <random> once per process; when the two disagree (another standard library) every AC-RANSAC entry point returns
+// R3D_ERR_UNSUPPORTED (AcFused::plan), so results never depend on this file being right for an unknown library.
 #pragma once
 #include <stdint.h>
 

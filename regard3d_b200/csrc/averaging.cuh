@@ -3,7 +3,6 @@
 #include "r3d_internal.cuh"
 #include "lm_trust_region.cuh"
 
-#include <chrono>
 #include <vector>
 
 namespace r3d {
@@ -51,29 +50,11 @@ __global__ void __launch_bounds__(kThreads) k_avg_step(const double* __restrict_
   }
 }
 
-inline double now_ms() {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
-}
-
 // 2-edge-connected components of an undirected multigraph on nodes 0..n-1 (edge k = (eu[k], ev[k]); parallel edges are
 // not bridges, self-loops are ignored): bridges by Tarjan's low-link (iterative DFS), then connected components of the
 // remaining edges.  Returns the component with the most nodes (>= 2; a tie keeps the one holding the smallest node), or
 // -1; comp[v] = component of v, -1 for nodes without edges.  (rotavg.cu)
 int largest_biedge_component(uint32_t n, const std::vector<uint32_t>& eu, const std::vector<uint32_t>& ev, std::vector<int>& comp);
-
-template <typename T>
-struct DevArr {  // device scratch out of the worker's pool (context.cu)
-  DeviceWorker* w;
-  T* p = nullptr;
-  explicit DevArr(DeviceWorker& worker) : w(&worker) {}
-  DevArr(const DevArr&) = delete;
-  DevArr& operator=(const DevArr&) = delete;
-  ~DevArr() { if (p) pool_release(*w, p); }
-  bool alloc(size_t n) {
-    p = (T*)pool_alloc(*w, std::max<size_t>(n, 1) * sizeof(T));
-    return p != nullptr;
-  }
-};
 
 }  // namespace ra
 }  // namespace r3d

@@ -10,7 +10,6 @@
 
 #include <algorithm>
 #include <atomic>
-#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -31,10 +30,6 @@ struct BatchPair {
   PairDesc pd;
 };
 
-double now_ms() {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
-}
-
 float pair_eps(const ViewDev& vi, const ViewDev& vj) {
   if (vi.int_ops && vj.int_ops) return 0.f;  // integer path: exact keys (the chunk-id packing is covered by pack_rel)
   const double nI = vi.max_norm, nJ = vj.max_norm;
@@ -44,19 +39,6 @@ float pair_eps(const ViewDev& vi, const ViewDev& vj) {
   e *= 1.001;
   return (float)e + 1e-30f;
 }
-
-struct EventTimer {
-  cudaEvent_t ev[5];
-  bool ok = false;
-  EventTimer() {
-    ok = true;
-    for (auto& e : ev)
-      if (cudaEventCreate(&e) != cudaSuccess) ok = false;
-  }
-  ~EventTimer() {
-    for (auto& e : ev) cudaEventDestroy(e);
-  }
-};
 
 }  // namespace
 
@@ -548,38 +530,17 @@ static int match_pairs_impl(r3d_ctx* ctx, const uint32_t* pairs, uint64_t n_pair
   }
   // Shard the (I-sorted) pair list into contiguous, cost-balanced ranges: one per device, no
   // collective; every device holds all regions.
-  std::vector<uint64_t> cut(nw + 1, 0);
-  if (nw > 1) {
-    std::vector<double> cost(n_pairs + 1, 0.0);
-    DeviceWorker& w0 = ctx->workers[0];
-    for (uint64_t p = 0; p < n_pairs; ++p) {
-      auto a = w0.views.find(pairs[2 * p]), b = w0.views.find(pairs[2 * p + 1]);
-      const double c = (a != w0.views.end() && b != w0.views.end()) ? (double)a->second.n * (double)b->second.n : 0.0;
-      cost[p + 1] = cost[p] + c + 1.0;
-    }
-    for (size_t k = 1; k < nw; ++k) {
-      const double target = cost[n_pairs] * (double)k / (double)nw;
-      cut[k] = (uint64_t)(std::lower_bound(cost.begin(), cost.end(), target) - cost.begin());
-      if (cut[k] > n_pairs) cut[k] = n_pairs;
-    }
-  }
-  cut[nw] = n_pairs;
+  DeviceWorker& w0 = ctx->workers[0];
+  const std::vector<uint64_t> cut = balanced_cuts(n_pairs, nw, [&](uint64_t p) {
+    auto a = w0.views.find(pairs[2 * p]), b = w0.views.find(pairs[2 * p + 1]);
+    return (a != w0.views.end() && b != w0.views.end()) ? (double)a->second.n * (double)b->second.n : 0.0;
+  });
   std::vector<std::vector<r3d_span>> res(nw);
   std::vector<std::vector<r3d_slab>> res_slabs(nw);
-  std::vector<int> rcs(nw, R3D_OK);
-  if (nw == 1) {
-    rcs[0] = match_on_worker(ctx, ctx->workers[0], pairs, n_pairs, dist_ratio, flags, res[0], res_slabs[0], nullptr);
-  } else {
-    std::vector<std::thread> th;
-    for (size_t k = 0; k < nw; ++k)
-      th.emplace_back([&, k]() {
-        rcs[k] = match_on_worker(ctx, ctx->workers[k], pairs + 2 * cut[k], cut[k + 1] - cut[k], dist_ratio, flags,
-                                 res[k], res_slabs[k], nullptr);
-      });
-    for (auto& t : th) t.join();
-  }
-  for (int rc : rcs)
-    if (rc) return rc;
+  const int rc = fan_out(ctx, [&](size_t k, DeviceWorker& w) {
+    return match_on_worker(ctx, w, pairs + 2 * cut[k], cut[k + 1] - cut[k], dist_ratio, flags, res[k], res_slabs[k], nullptr);
+  });
+  if (rc) return rc;
   {
     r3d_match_timing sum{};
     for (auto& wk : ctx->workers) {

@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #include <atomic>
+#include <chrono>
 #include <functional>
 #include <map>
 #include <mutex>
@@ -229,6 +230,86 @@ int envelope_cholesky(r3d_ctx* ctx, DeviceWorker& w, double* A, double* L, int n
 int prepare_views(r3d_ctx* ctx, DeviceWorker& w);
 void* pool_alloc(DeviceWorker& w, size_t bytes);  // nullptr on failure
 void pool_release(DeviceWorker& w, void* p);
+
+// device scratch out of the worker's size-bucketed pool: no cudaMalloc / cudaFree per call -- both synchronise the
+// device and cost up to a second per call on multi-GPU boxes.  Everything that touches these blocks is ordered on
+// w.stream, so a released block may be handed out again at once.  alloc(n): max(n, 1) elements, false when the pool
+// cannot provide them; a second alloc releases the earlier block.
+template <typename T>
+struct DevArr {
+  DeviceWorker* w;
+  T* p = nullptr;
+  explicit DevArr(DeviceWorker& worker) : w(&worker) {}
+  DevArr(const DevArr&) = delete;
+  DevArr& operator=(const DevArr&) = delete;
+  ~DevArr() { pool_release(*w, p); }
+  bool alloc(size_t n) {
+    pool_release(*w, p);
+    p = (T*)pool_alloc(*w, std::max<size_t>(n, 1) * sizeof(T));
+    return p != nullptr;
+  }
+};
+
+// N CUDA events, destroyed with the object; create(false): ordering only (cudaEventDisableTiming)
+template <int N>
+struct Events {
+  cudaEvent_t e[N] = {};
+  Events() = default;
+  Events(const Events&) = delete;
+  Events& operator=(const Events&) = delete;
+  ~Events() {
+    for (cudaEvent_t x : e)
+      if (x) cudaEventDestroy(x);
+  }
+  cudaError_t create(bool timing = true) {
+    for (cudaEvent_t& x : e) {
+      const cudaError_t r = cudaEventCreateWithFlags(&x, timing ? cudaEventDefault : cudaEventDisableTiming);
+      if (r != cudaSuccess) return r;
+    }
+    return cudaSuccess;
+  }
+  float ms(int a, int b) const {  // elapsed time between two recorded timing events
+    float t = 0.f;
+    cudaEventElapsedTime(&t, e[a], e[b]);
+    return t;
+  }
+};
+
+inline double now_ms() {
+  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
+}
+
+// Independent work items [0, n) spread over `parts` devices: cut[k] .. cut[k + 1] is part k, contiguous ranges of equal
+// sums of weight(i) + 1 (prefix sums, then lower_bound on k / parts of the total).
+template <typename Weight>
+std::vector<uint64_t> balanced_cuts(uint64_t n, size_t parts, Weight weight) {
+  std::vector<uint64_t> cut(parts + 1, 0);
+  cut[parts] = n;
+  if (parts < 2) return cut;
+  std::vector<double> cost(n + 1, 0.0);
+  for (uint64_t i = 0; i < n; ++i) cost[i + 1] = cost[i] + (double)weight(i) + 1.0;
+  for (size_t k = 1; k < parts; ++k)
+    cut[k] = std::min<uint64_t>(n, (uint64_t)(std::lower_bound(cost.begin(), cost.end(), cost[n] * (double)k / (double)parts) - cost.begin()));
+  return cut;
+}
+
+// fn(k, worker k) for every worker of the context: inline for a single worker, otherwise on one thread per worker.
+// Returns the first non-zero return code in worker order.
+template <typename Fn>
+int fan_out(r3d_ctx* ctx, Fn&& fn) {
+  const size_t nw = ctx->workers.size();
+  std::vector<int> rcs(nw, R3D_OK);
+  if (nw == 1) {
+    rcs[0] = fn((size_t)0, ctx->workers[0]);
+  } else {
+    std::vector<std::thread> th;
+    for (size_t k = 0; k < nw; ++k) th.emplace_back([&, k]() { rcs[k] = fn(k, ctx->workers[k]); });
+    for (auto& t : th) t.join();
+  }
+  for (int rc : rcs)
+    if (rc) return rc;
+  return R3D_OK;
+}
 
 // dynamic-scheduling parallel loop on the persistent host pool (host_pool.cpp); n_threads bounds the
 // concurrency of THIS loop (the caller counts as one)

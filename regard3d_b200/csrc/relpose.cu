@@ -20,17 +20,12 @@
 #include "lm_trust_region.cuh"
 #include "relpose_math.cuh"
 
-#include <chrono>
 #include <cstring>
 #include <numeric>
 
 namespace r3d {
 
 namespace {
-
-double now_ms() {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
-}
 
 struct RpPair {            // a pair that reached the cheirality stage
   uint32_t in_ofs, n_in;   // its AC-RANSAC inliers in x_in1 / x_in2 (residual order)
@@ -418,20 +413,6 @@ __global__ void __launch_bounds__(kBThreads) k_relpose_ba(const RpPair* __restri
 #undef F
 }
 
-template <typename T>
-struct DevArr {  // device scratch out of the worker's pool (context.cu)
-  DeviceWorker* w;
-  T* p = nullptr;
-  explicit DevArr(DeviceWorker& worker) : w(&worker) {}
-  DevArr(const DevArr&) = delete;
-  DevArr& operator=(const DevArr&) = delete;
-  ~DevArr() { if (p) pool_release(*w, p); }
-  bool alloc(size_t n) {
-    p = (T*)pool_alloc(*w, std::max<size_t>(n, 1) * sizeof(T));
-    return p != nullptr;
-  }
-};
-
 // pairs [p0, p1) of the map on worker w
 int relpose_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_matches* m, const r3d_view_info* views, uint32_t n_views,
                   const r3d_relpose_options& opt, uint64_t p0, uint64_t p1, r3d_relative_pose* out,
@@ -505,24 +486,21 @@ int relpose_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_matches* m, const r3d
   DevArr<RpCheir> d_ch(w);
   if (!d_pairs.alloc(nc) || !d_x1.alloc(n_in) || !d_x2.alloc(n_in) || !d_ch.alloc(nc))
     return fail(ctx, R3D_ERR_NOMEM, "r3d_relative_poses: device scratch");
-  cudaEvent_t ev[4];
-  for (auto& e : ev) R3D_CUDA_TRY(ctx, cudaEventCreate(&e));
-  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 4; ++i) cudaEventDestroy(e[i]); } } evg{ev};
+  Events<4> ev;
+  R3D_CUDA_TRY(ctx, ev.create());
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_pairs.p, hp.data(), nc * sizeof(RpPair), cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_x1.p, hx1.data(), n_in * sizeof(double2), cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_x2.p, hx2.data(), n_in * sizeof(double2), cudaMemcpyHostToDevice, w.stream));
   // ---- 2. cheirality ----
-  R3D_CUDA_TRY(ctx, cudaEventRecord(ev[0], w.stream));
+  R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[0], w.stream));
   k_relpose_cheirality<<<nc, kCThreads, 0, w.stream>>>(d_pairs.p, d_x1.p, d_x2.p, d_ch.p);
   R3D_CUDA_TRY(ctx, cudaGetLastError());
-  R3D_CUDA_TRY(ctx, cudaEventRecord(ev[1], w.stream));
+  R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[1], w.stream));
   T.kernel_launches += 1;
   std::vector<RpCheir> hch(nc);
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(hch.data(), d_ch.p, nc * sizeof(RpCheir), cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, ev[0], ev[1]);
-  T.ms_cheirality = ms;
+  T.ms_cheirality = ev.ms(0, 1);
   std::vector<uint32_t> ok;  // candidates with a motion
   for (uint32_t a = 0; a < nc; ++a) {
     r3d_relative_pose& o = out[cand[a]];
@@ -568,16 +546,15 @@ int relpose_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_matches* m, const r3d
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_ba.p, hba.data(), nc * sizeof(RpBa), cudaMemcpyHostToDevice, w.stream));
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_order.p, order.data(), order.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, w.stream));
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_work.p, 0, sizeof(uint32_t), w.stream));
-    R3D_CUDA_TRY(ctx, cudaEventRecord(ev[2], w.stream));
+    R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[2], w.stream));
     k_relpose_ba<<<grid, kBThreads, 0, w.stream>>>(d_pairs.p, d_order.p, (uint32_t)order.size(), d_work.p, d_a1.p, d_a2.p, d_ba.p, lm_params(opt.ba),
                                                    d_scr.p, cap);
     R3D_CUDA_TRY(ctx, cudaGetLastError());
-    R3D_CUDA_TRY(ctx, cudaEventRecord(ev[3], w.stream));
+    R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[3], w.stream));
     T.kernel_launches += 1;
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(hba.data(), d_ba.p, nc * sizeof(RpBa), cudaMemcpyDeviceToHost, w.stream));
     R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-    cudaEventElapsedTime(&ms, ev[2], ev[3]);
-    T.ms_refine = ms;
+    T.ms_refine = ev.ms(2, 3);
     for (uint32_t a : ok) {
       r3d_relative_pose& o = out[cand[a]];
       const RpBa& b = hba[a];
@@ -629,29 +606,12 @@ extern "C" int r3d_relative_poses(r3d_ctx* ctx, const r3d_matches* matches, cons
   const uint64_t P = matches->pairs.size() / 2;
   std::vector<std::vector<r3d_indmatch>> inl(P);
   // the pairs are independent: contiguous ranges of equal match counts, one per device (the rule of r3d_filter_pairs)
-  const size_t nw = ctx->workers.size();
-  std::vector<uint64_t> cut(nw + 1, 0);
-  {
-    std::vector<double> cost(P + 1, 0.0);
-    for (uint64_t p = 0; p < P; ++p) cost[p + 1] = cost[p] + (double)matches->per[p].size() + 1.0;
-    for (size_t k = 1; k < nw; ++k)
-      cut[k] = std::min<uint64_t>(P, (uint64_t)(std::lower_bound(cost.begin(), cost.end(), cost[P] * (double)k / (double)nw) - cost.begin()));
-    cut[nw] = P;
-  }
-  std::vector<int> rcs(nw, R3D_OK);
-  std::vector<r3d_relpose_timing> tms(nw);
-  if (nw == 1) {
-    rcs[0] = relpose_range(ctx, ctx->workers[0], matches, views, n_views, *opt, 0, P, out, inl, tms[0]);
-  } else {
-    std::vector<std::thread> th;
-    for (size_t k = 0; k < nw; ++k)
-      th.emplace_back([&, k]() {
-        rcs[k] = relpose_range(ctx, ctx->workers[k], matches, views, n_views, *opt, cut[k], cut[k + 1], out, inl, tms[k]);
-      });
-    for (auto& t : th) t.join();
-  }
-  for (int rc : rcs)
-    if (rc) return rc;
+  const std::vector<uint64_t> cut = balanced_cuts(P, ctx->workers.size(), [&](uint64_t p) { return matches->per[p].size(); });
+  std::vector<r3d_relpose_timing> tms(ctx->workers.size());
+  const int rc = fan_out(ctx, [&](size_t k, DeviceWorker& w) {
+    return relpose_range(ctx, w, matches, views, n_views, *opt, cut[k], cut[k + 1], out, inl, tms[k]);
+  });
+  if (rc) return rc;
   r3d_relpose_timing sum{};
   for (const r3d_relpose_timing& t : tms) {
     sum.ms_ransac = std::max(sum.ms_ransac, t.ms_ransac);

@@ -15,7 +15,6 @@
 //      region of the bundle adjustment.  The 6 x 6 normal equations are reduced in a fixed order (no floating-point
 //      atomics), so a call is reproducible.  FP64 throughout; bound by FP64 latency, not by tensor cores or HBM.
 #include "acransac.cuh"
-#include "acransac_rng.cuh"
 #include "ba_model.cuh"
 #include "detmath.cuh"
 #include "lm_trust_region.cuh"
@@ -24,19 +23,13 @@
 #include "r3d_sfm.h"
 
 #include <algorithm>
-#include <chrono>
 #include <cmath>
 #include <cstring>
 #include <limits>
-#include <thread>
 
 namespace r3d {
 
 namespace {
-
-double now_ms() {
-  return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now().time_since_epoch()).count();
-}
 
 struct RsView {            // a view that reached the AC-RANSAC stage (device)
   uint32_t ofs, M;         // its correspondences in the device arrays
@@ -282,20 +275,6 @@ __global__ void __launch_bounds__(kRThreads) k_resect_refine(const RsView* __res
   }
 }
 
-template <typename T>
-struct DevArr {  // device scratch out of the worker's pool (context.cu)
-  DeviceWorker* w;
-  T* p = nullptr;
-  explicit DevArr(DeviceWorker& worker) : w(&worker) {}
-  DevArr(const DevArr&) = delete;
-  DevArr& operator=(const DevArr&) = delete;
-  ~DevArr() { if (p) pool_release(*w, p); }
-  bool alloc(size_t n) {
-    p = (T*)pool_alloc(*w, std::max<size_t>(n, 1) * sizeof(T));
-    return p != nullptr;
-  }
-};
-
 void angle_axis_to_rotation(const double* aa, double* R) { r3d_sfm::angle_axis_to_rotation(aa, R); }
 
 void set_pose(r3d_resection& o, const double* R, const double* t) {
@@ -326,8 +305,6 @@ int resect_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_resection_view* views,
     T.ms_host = now_ms() - t0;
     return R3D_OK;
   }
-  if (!rng_selftest())
-    return fail(ctx, R3D_ERR_INVALID, "r3d_resect_views: the device sample stream disagrees with this process's <random>");
   const uint32_t n = (uint32_t)cand.size();
   // ---- per view set-up: the a-contrario adaptor for resection with known K (point-to-point, pixel units) ----
   std::vector<AcPair> hpairs(n);
@@ -362,102 +339,60 @@ int resect_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_resection_view* views,
     std::memcpy(&hX[3 * (size_t)hpairs[a].pt_ofs], X + 3 * v.first, 3 * v.count * sizeof(double));
     std::memcpy(&hx[2 * (size_t)hpairs[a].pt_ofs], x + 2 * v.first, 2 * v.count * sizeof(double));
   });
-  const std::vector<float> vlog10 = ac_vlog10(maxM);
-  const std::vector<float> hlogc_k = ac_logc_k(ac_min_samples(3), vlog10, maxM);
-  // ---- size classes of the persistent kernel (shared-memory sort capacity 1024 ... 16384, beyond: global scratch) ----
-  constexpr int kClasses = 6;
-  std::vector<uint32_t> order[kClasses], horder;
-  uint32_t class_ofs[kClasses + 1] = {0}, caps[kClasses] = {0}, grids[kClasses] = {0}, huge_maxM = 0;
-  for (uint32_t a = 0; a < n; ++a) {
-    const uint32_t M = hpairs[a].M;
-    int c = 0;
-    while (c < 5 && (1024u << c) < M) ++c;
-    if (M > 16384u) { c = 5; huge_maxM = std::max(huge_maxM, M); }
-    order[c].push_back(a);
-  }
-  size_t si_need = 0, huge_need = 0;
-  for (int c = 0; c < kClasses; ++c) {
-    std::stable_sort(order[c].begin(), order[c].end(), [&](uint32_t p, uint32_t q) { return hpairs[p].M > hpairs[q].M; });
-    class_ofs[c] = (uint32_t)horder.size();
-    horder.insert(horder.end(), order[c].begin(), order[c].end());
-    const uint32_t cnt = (uint32_t)order[c].size();
-    if (!cnt) continue;
-    const bool huge = c == 5;
-    uint32_t cap = 1024u << c;
-    if (huge) {
-      cap = 32768;
-      while (cap < huge_maxM) cap <<= 1;
-    }
-    uint32_t grid = std::min<uint32_t>(cnt, (uint32_t)w.sm_count * (uint32_t)acransac_fused_ctas_per_sm(3, cap, huge));
-    if (huge) grid = std::min<uint32_t>(grid, (uint32_t)w.sm_count);
-    caps[c] = cap;
-    grids[c] = grid;
-    si_need = std::max(si_need, (size_t)grid * cap);
-    if (huge) huge_need = (size_t)grid * cap;
-  }
-  class_ofs[kClasses] = (uint32_t)horder.size();
+  // ---- the persistent AC-RANSAC kernel's tables, size classes and scratch ----
+  AcTables tab(w);
+  AcFused fused(w);
+  int rc = tab.upload(ctx, w, ac_min_samples(3), maxM, tbl_total);
+  if (rc) return rc;
+  rc = fused.plan(ctx, w, 3, hpairs);
+  if (rc) return rc;
   std::vector<uint32_t> lm_order(n);  // refinement: most correspondences first
   for (uint32_t a = 0; a < n; ++a) lm_order[a] = a;
   std::stable_sort(lm_order.begin(), lm_order.end(), [&](uint32_t p, uint32_t q) { return hpairs[p].M > hpairs[q].M; });
 
   DevArr<AcPair> d_pairs(w);
   DevArr<RsView> d_views(w);
-  DevArr<double> d_X(w), d_x3(w), d_se(w), d_model(w);
+  DevArr<double> d_X(w), d_x3(w), d_model(w);
   DevArr<double2> d_xo(w), d_x1(w), d_x2(w);
   DevArr<uint2> d_idm(w), d_outm(w);
-  DevArr<float> d_vlog10(w), d_logc_n(w), d_logc_k(w);
-  DevArr<uint32_t> d_order(w), d_lm_order(w), d_work(w), d_si(w), d_pool(w);
+  DevArr<uint32_t> d_lm_order(w), d_lm_work(w);
   DevArr<AcFusedOut> d_out(w);
   DevArr<RsLm> d_lm(w);
   if (!d_pairs.alloc(n) || !d_views.alloc(n) || !d_X.alloc(3 * pt_total) || !d_x3.alloc(pt_total) || !d_xo.alloc(pt_total) ||
       !d_x1.alloc(pt_total) || !d_x2.alloc(pt_total) || !d_idm.alloc(pt_total) || !d_outm.alloc(pt_total) ||
-      !d_vlog10.alloc(vlog10.size()) || !d_logc_n.alloc(tbl_total) || !d_logc_k.alloc(hlogc_k.size()) || !d_order.alloc(n) ||
-      !d_lm_order.alloc(n) || !d_work.alloc(kClasses + 1) || !d_si.alloc(si_need) || !d_se.alloc(huge_need) ||
-      !d_pool.alloc(huge_need) || !d_model.alloc(12 * (size_t)n) || !d_out.alloc(n) || !d_lm.alloc(n))
+      !d_lm_order.alloc(n) || !d_lm_work.alloc(1) || !d_model.alloc(12 * (size_t)n) || !d_out.alloc(n) || !d_lm.alloc(n))
     return fail(ctx, R3D_ERR_NOMEM, "r3d_resect_views: device scratch");
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_pairs.p, hpairs.data(), n * sizeof(AcPair), cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_views.p, hviews.data(), n * sizeof(RsView), cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_X.p, hX.data(), hX.size() * sizeof(double), cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_xo.p, hx.data(), hx.size() * sizeof(double), cudaMemcpyHostToDevice, w.stream));
-  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_vlog10.p, vlog10.data(), vlog10.size() * sizeof(float), cudaMemcpyHostToDevice, w.stream));
-  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_logc_k.p, hlogc_k.data(), hlogc_k.size() * sizeof(float), cudaMemcpyHostToDevice, w.stream));
-  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_order.p, horder.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_lm_order.p, lm_order.data(), n * sizeof(uint32_t), cudaMemcpyHostToDevice, w.stream));
-  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_work.p, 0, (kClasses + 1) * sizeof(uint32_t), w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_lm_work.p, 0, sizeof(uint32_t), w.stream));
   R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_lm.p, 0xff, n * sizeof(RsLm), w.stream));  // termination -1: not refined
-  cudaEvent_t ev[3];
-  for (auto& e : ev) R3D_CUDA_TRY(ctx, cudaEventCreate(&e));
-  struct EvGuard { cudaEvent_t* e; ~EvGuard() { for (int i = 0; i < 3; ++i) cudaEventDestroy(e[i]); } } evg{ev};
-  R3D_CUDA_TRY(ctx, cudaEventRecord(ev[0], w.stream));
+  Events<3> ev;
+  R3D_CUDA_TRY(ctx, ev.create());
+  R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[0], w.stream));
   for (uint32_t a0 = 0; a0 < n; a0 += 65535u) {  // gridDim.y limit
     const uint32_t na = std::min(65535u, n - a0);
     k_resect_points<<<dim3(8, na), 256, 0, w.stream>>>(d_views.p + a0, d_X.p, d_xo.p, d_x1.p, d_x3.p, d_x2.p, d_idm.p);
     T.kernel_launches += 1;
   }
   R3D_CUDA_TRY(ctx, cudaGetLastError());
-  {
-    const int rc = launch_ac_tables(ctx, w, d_pairs.p, n, d_vlog10.p, d_logc_n.p);
-    if (rc) return rc;
-    T.kernel_launches += 1;
-  }
-  for (int c = kClasses - 1; c >= 0; --c) {  // the long-running classes first
-    const uint32_t cnt = class_ofs[c + 1] - class_ofs[c];
-    if (!cnt) continue;
-    const int rc = launch_acransac_fused(ctx, w, 3, c == 5, d_pairs.p, d_order.p + class_ofs[c], cnt, d_work.p + c, d_x1.p, d_x2.p,
-                                         d_logc_n.p, d_logc_k.p, caps[c], opt.max_iter, d_se.p, d_si.p, d_pool.p, d_idm.p, d_outm.p,
-                                         d_out.p, d_model.p, grids[c], d_x3.p);
-    if (rc) return rc;
-    T.kernel_launches += 1;
-  }
-  R3D_CUDA_TRY(ctx, cudaEventRecord(ev[1], w.stream));
+  rc = launch_ac_tables(ctx, w, d_pairs.p, n, tab.vlog10.p, tab.logc_n.p);
+  if (rc) return rc;
+  T.kernel_launches += 1;
+  rc = fused.launch(ctx, w, d_pairs.p, d_x1.p, d_x2.p, d_x3.p, tab.logc_n.p, tab.logc_k.p, opt.max_iter, d_idm.p, d_outm.p, d_out.p,
+                    d_model.p, T.kernel_launches);
+  if (rc) return rc;
+  R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[1], w.stream));
   if (opt.refine) {
     const uint32_t grid = std::min<uint32_t>(n, (uint32_t)w.sm_count);
-    k_resect_refine<<<grid, kRThreads, 0, w.stream>>>(d_views.p, d_lm_order.p, n, d_work.p + kClasses, d_out.p, d_model.p, d_outm.p,
+    k_resect_refine<<<grid, kRThreads, 0, w.stream>>>(d_views.p, d_lm_order.p, n, d_lm_work.p, d_out.p, d_model.p, d_outm.p,
                                                       d_x1.p, d_x3.p, d_xo.p, d_lm.p, lm_params(opt.ba));
     R3D_CUDA_TRY(ctx, cudaGetLastError());
     T.kernel_launches += 1;
   }
-  R3D_CUDA_TRY(ctx, cudaEventRecord(ev[2], w.stream));
+  R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[2], w.stream));
   std::vector<AcFusedOut> hout(n);
   std::vector<double> hmodel(12 * (size_t)n);
   std::vector<RsLm> hlm(n);
@@ -467,11 +402,8 @@ int resect_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_resection_view* views,
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(hlm.data(), d_lm.p, n * sizeof(RsLm), cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(houtm.data(), d_outm.p, pt_total * sizeof(uint2), cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-  float ms = 0.f;
-  cudaEventElapsedTime(&ms, ev[0], ev[1]);
-  T.ms_ransac = ms;
-  cudaEventElapsedTime(&ms, ev[1], ev[2]);
-  T.ms_refine = ms;
+  T.ms_ransac = ev.ms(0, 1);
+  T.ms_refine = ev.ms(1, 2);
   T.ms_device_total = T.ms_ransac + T.ms_refine;
   for (uint32_t a = 0; a < n; ++a) {
     const AcFusedOut& f = hout[a];
@@ -548,27 +480,12 @@ extern "C" int r3d_resect_views(r3d_ctx* ctx, const r3d_resection_view* views, u
   std::vector<std::vector<uint32_t>> inl(n_views);
   // the views are independent: contiguous ranges of equal correspondence counts, one per device (the rule of
   // r3d_relative_poses)
-  const size_t nw = ctx->workers.size();
-  std::vector<uint32_t> cut(nw + 1, 0);
-  {
-    std::vector<double> cost(n_views + 1, 0.0);
-    for (uint32_t v = 0; v < n_views; ++v) cost[v + 1] = cost[v] + (double)views[v].count + 1.0;
-    for (size_t k = 1; k < nw; ++k)
-      cut[k] = std::min<uint32_t>(n_views, (uint32_t)(std::lower_bound(cost.begin(), cost.end(), cost[n_views] * (double)k / (double)nw) - cost.begin()));
-    cut[nw] = n_views;
-  }
-  std::vector<int> rcs(nw, R3D_OK);
-  std::vector<r3d_resection_timing> tms(nw);
-  if (nw == 1) {
-    rcs[0] = resect_range(ctx, ctx->workers[0], views, 0, n_views, X, x, *opt, out, inl, tms[0]);
-  } else {
-    std::vector<std::thread> th;
-    for (size_t k = 0; k < nw; ++k)
-      th.emplace_back([&, k]() { rcs[k] = resect_range(ctx, ctx->workers[k], views, cut[k], cut[k + 1], X, x, *opt, out, inl, tms[k]); });
-    for (auto& t : th) t.join();
-  }
-  for (int rc : rcs)
-    if (rc) return rc;
+  const std::vector<uint64_t> cut = balanced_cuts(n_views, ctx->workers.size(), [&](uint64_t v) { return views[v].count; });
+  std::vector<r3d_resection_timing> tms(ctx->workers.size());
+  const int rc = fan_out(ctx, [&](size_t k, DeviceWorker& w) {
+    return resect_range(ctx, w, views, (uint32_t)cut[k], (uint32_t)cut[k + 1], X, x, *opt, out, inl, tms[k]);
+  });
+  if (rc) return rc;
   r3d_resection_timing sum{};
   for (const r3d_resection_timing& t : tms) {
     sum.ms_ransac = std::max(sum.ms_ransac, t.ms_ransac);

@@ -26,7 +26,6 @@
 
 #include <cooperative_groups.h>
 
-#include <chrono>
 #include <cmath>
 #include <cstring>
 #include <numeric>
@@ -640,11 +639,6 @@ double init_value(uint64_t k) {
   return (double)(z >> 11) * (1.0 / 9007199254740992.0) - 0.5;
 }
 
-struct Events {
-  cudaEvent_t e[6] = {};
-  ~Events() { for (auto x : e) if (x) cudaEventDestroy(x); }
-};
-
 int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views, const r3d_rotavg_options& opt,
                        double* rotations, uint8_t* view_kept, uint8_t* edge_kept, uint32_t* edge_support, r3d_rotavg_summary& S) {
   const double t0 = now_ms();
@@ -692,8 +686,8 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
         rot_soa[(size_t)(3 * a + b) * E + p] = r.I < r.J ? r.rotation[3 * a + b] : r.rotation[3 * b + a];
   }
   for (uint32_t v = 0; v < nn; ++v) up_ofs[v + 1] += up_ofs[v];
-  Events ev;
-  for (auto& x : ev.e) R3D_CUDA_TRY(ctx, cudaEventCreate(&x));
+  Events<6> ev;
+  R3D_CUDA_TRY(ctx, ev.create());
   std::vector<uint32_t> support(E, 0);
   if (E) {
     DevArr<uint32_t> d_ofs(w), d_nbr(w), d_sup(w), d_work(w);
@@ -723,9 +717,7 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(support.data(), d_sup.p, E * sizeof(uint32_t), cudaMemcpyDeviceToHost, w.stream));
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(cnt, d_cnt.p, sizeof(cnt), cudaMemcpyDeviceToHost, w.stream));
     R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ev.e[0], ev.e[1]);
-    S.ms_triplets = ms;
+    S.ms_triplets = ev.ms(0, 1);
     S.n_triplets = cnt[0];
     S.n_valid_triplets = cnt[1];
   }
@@ -833,11 +825,7 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
   std::vector<double> Rl(9 * (size_t)m);
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(Rl.data(), d_Rout.p, Rl.size() * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-  {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ev.e[2], ev.e[3]);
-    S.ms_init = ms;
-  }
+  S.ms_init = ev.ms(2, 3);
   // ---- 4. refinement ----
   if (opt.refine) {
     std::vector<double> aa(3 * (size_t)m);
@@ -926,9 +914,7 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
     R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[5], w.stream));
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(aa.data(), cur, N * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
     R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, ev.e[4], ev.e[5]);
-    S.ms_refine = ms;
+    S.ms_refine = ev.ms(4, 5);
     // back to matrices, the gauge again
     std::vector<double> R0(9);
     rp::angle_axis_to_rotation(&aa[0], R0.data());
@@ -982,7 +968,7 @@ extern "C" int r3d_debug_chol_solve3(r3d_ctx* ctx, int n, const double* A, const
   if ((rc = ra::trsm3_grid(ctx, w, &grid))) return rc;
   const int nblk = (n + kCholNB - 1) / kCholNB;
   // as rotation_averaging allocates them: M | unused rhs row, L with the slack of dense_cholesky's contract
-  ra::DevArr<double> d_A(w), d_L(w), d_Linv(w), d_x(w), d_Y(w), d_Z(w), d_flag(w);
+  DevArr<double> d_A(w), d_L(w), d_Linv(w), d_x(w), d_Y(w), d_Z(w), d_flag(w);
   if (!d_A.alloc((size_t)(n + 1) * n) || !d_L.alloc((size_t)(n + 1) * n + 64) || !d_Linv.alloc((size_t)nblk * kCholNB * kCholNB) ||
       !d_x.alloc(n) || !d_Y.alloc(3 * (size_t)n) || !d_Z.alloc(3 * (size_t)n) || !d_flag.alloc(1))
     return fail(ctx, R3D_ERR_NOMEM, "r3d_debug_chol_solve3: device scratch");

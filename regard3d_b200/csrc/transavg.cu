@@ -23,8 +23,6 @@
 namespace r3d {
 namespace ta {
 
-using ra::DevArr;
-
 constexpr int kChordal = 2;  // R3D_TRANSAVG_L2_CHORDAL
 constexpr int kSoftL1 = 3;   // R3D_TRANSAVG_SOFTL1
 constexpr int kRThreads = 256;
@@ -320,15 +318,10 @@ double start_value(uint64_t k) {
   return (double)(z >> 11) * (1.0 / 9007199254740992.0);
 }
 
-struct Events {
-  cudaEvent_t e[2] = {};
-  ~Events() { for (auto x : e) if (x) cudaEventDestroy(x); }
-};
-
 int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use, const double* rot,
                           const uint8_t* rot_kept, uint32_t n_views, const r3d_transavg_options& opt, double* centers,
                           double* translations, uint8_t* view_kept, uint8_t* edge_kept, r3d_transavg_summary& S) {
-  const double t0 = ra::now_ms();
+  const double t0 = now_ms();
   const char* fn = "r3d_translation_averaging: ";
   DeviceWorker& w = ctx->workers[0];
   R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
@@ -361,7 +354,7 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
   std::vector<int> comp;
   const int best = ra::largest_biedge_component(n_views, eu, ev, comp);
   if (best < 0) {
-    S.ms_host = ra::now_ms() - t0;
+    S.ms_host = now_ms() - t0;
     return R3D_OK;
   }
   std::vector<uint32_t> local(n_views, UINT32_MAX), kview;
@@ -435,8 +428,8 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_ed.p, ed.data(), ed.size() * sizeof(double), cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_cur.p, x.data(), Nv * sizeof(double), cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_scal.p, 0, 8 * sizeof(double), w.stream));
-  Events evt;
-  for (auto& y : evt.e) R3D_CUDA_TRY(ctx, cudaEventCreate(&y));
+  Events<2> evt;
+  R3D_CUDA_TRY(ctx, evt.create());
   R3D_CUDA_TRY(ctx, cudaEventRecord(evt.e[0], w.stream));
   double scal[8] = {0, 0, 0, 0, 0, 0, 0, 0};
   auto read_scal = [&]() -> int {
@@ -528,11 +521,7 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
   R3D_CUDA_TRY(ctx, cudaEventRecord(evt.e[1], w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(x.data(), cur, Nv * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-  {
-    float ms = 0.f;
-    cudaEventElapsedTime(&ms, evt.e[0], evt.e[1]);
-    S.ms_solve = ms;
-  }
+  S.ms_solve = evt.ms(0, 1);
   // centres and translations (t = -R C)
   for (uint32_t a = 0; a < m; ++a) {
     const uint32_t v = kview[a];
@@ -552,7 +541,7 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
     }
   }
   S.ms_device_total = S.ms_solve;
-  S.ms_host = ra::now_ms() - t0 - S.ms_device_total;
+  S.ms_host = now_ms() - t0 - S.ms_device_total;
   return R3D_OK;
 }
 
