@@ -662,6 +662,79 @@ typedef struct {
 int r3d_debug_ba_step(r3d_ctx* ctx, const r3d_ba_problem* p, const r3d_ba_options* opt, double radius, int schur_route,
                       int chol_method, r3d_ba_step_out* out);
 
+/* ---- keypoints (SURVEY.md 3: the feature stage's detector) ------------------------------------------------------ */
+/* Fast-AKAZE, Regard3D's default detector: Regard3DFeatures::detectKeypoints' "Fast-AKAZE" branch
+ * (src/Regard3DFeatures.cpp:590-614) with cv::AKAZE2 of src/thirdparty/fast-akaze.  Input: float gray images in
+ * [0, 1] as R3DFeaturesThread::processWorkItem builds them (src/threads/R3DFeaturesThread.cpp:162-191); decoding stays
+ * with the caller.  PM_G2 is the only diffusivity the detector implements. */
+#define R3D_AKAZE_DIFF_PM_G2 1 /* KAZE::DIFF_PM_G2 */
+typedef struct {
+  float threshold;     /* detector response threshold (R3DFParams::threshold_, default 0.001) */
+  int32_t octaves;     /* 4 */
+  int32_t sublevels;   /* 4 */
+  int32_t diffusivity; /* R3D_AKAZE_DIFF_PM_G2 */
+} r3d_akaze_options;
+void r3d_akaze_default_options(r3d_akaze_options* out);
+
+/* cv::KeyPoint as the detector leaves it, in upstream order (levels ascending, then each level's candidate order):
+ * size = diameter, angle in degrees after Regard3D's conversion (radians * 180 / pi + 90, wrapped into [0, 360]),
+ * class_id = evolution level. */
+typedef struct {
+  float x, y, size, angle, response;
+  int32_t octave, class_id;
+} r3d_akaze_keypoint;
+
+/* one evolution level of an image of the given size: (octave, sublevel), its shape, derivative kernel scale, border,
+ * sigma, diffusion time, octave ratio and the number of FED steps that lead to it from the previous level */
+typedef struct {
+  int32_t octave, sublevel, width, height, sigma_size, border;
+  float esigma, etime, ratio;
+  uint32_t n_tau;
+} r3d_akaze_level;
+/* the level table of a width x height image; returns the number of levels (at most cap are written) or < 0 */
+int r3d_akaze_levels(uint32_t width, uint32_t height, const r3d_akaze_options* opt, r3d_akaze_level* out, int cap);
+
+/* Keypoints of a batch of images (opaque, host memory). */
+typedef struct r3d_features r3d_features;
+/* images[i]: width[i] x height[i] row-major float32.  R3D_ERR_INVALID before any work for a side <= 2, a non-finite
+ * pixel or a bad option.  The images are dealt to the context's devices in contiguous slices and processed there in
+ * batches bounded by the device memory; the result does not depend on the number of devices.  An image too small for
+ * the first level (2 border + 1 >= a side, border 29 at the defaults) has no keypoints: upstream asserts instead. */
+int r3d_akaze_detect(r3d_ctx* ctx, const float* const* images, const uint32_t* widths, const uint32_t* heights,
+                     uint32_t n_images, const r3d_akaze_options* opt, r3d_features** out);
+uint32_t r3d_features_num_images(const r3d_features* f);
+uint32_t r3d_features_count(const r3d_features* f, uint32_t image);
+const r3d_akaze_keypoint* r3d_features_get(const r3d_features* f, uint32_t image);
+void r3d_free_features(r3d_features* f);
+
+/* per-stage device time of the last r3d_akaze_detect (CUDA events, milliseconds, summed over batches and devices) */
+typedef struct {
+  double upload_ms;        /* images host -> device, workspace clears */
+  double scale_space_ms;   /* blur, Scharr, k-percentile, Hessian, conductivity, FED */
+  double candidates_ms;    /* 3x3 maxima and their raster-order compaction */
+  double same_level_ms;    /* the same-level pass alone */
+  double cross_level_ms;   /* the lower- and the upper-level pass */
+  double refine_orient_ms; /* subpixel refinement, orientation, copies back */
+  double total_ms;
+  uint32_t images, batches, keypoints, kernel_launches, devices;
+} r3d_akaze_timing;
+int r3d_get_akaze_timing(const r3d_ctx* ctx, r3d_akaze_timing* out);
+
+/* Diagnostics: one image through r3d_akaze_detect's kernels, every level kept.  arrays: per level, in level order,
+ * Lt, Lsmooth, Lx, Ly, Ldet (5 x width x height floats each); kcontrast: per level (0 for a single-level image);
+ * cands / flags: per level, in level order, the candidates after the same-level pass (angle -1) and their deletion
+ * flags (bit 0: by the lower-level pass, bit 1: after the upper-level pass); cand_counts: per level.  Returns
+ * R3D_ERR_INVALID when more than cand_cap candidates exist. */
+int r3d_debug_akaze_levels(r3d_ctx* ctx, const float* image, uint32_t width, uint32_t height, const r3d_akaze_options* opt,
+                           float* arrays, float* kcontrast, r3d_akaze_keypoint* cands, uint8_t* flags, uint32_t cand_cap,
+                           uint32_t* cand_counts);
+
+/* Diagnostics: the subpixel refinement kernel alone on n points of one level (its Ldet, width x height, octave ratio):
+ * out = the refined points; a rejected point (|d| > 1) is returned unchanged with class_id -1.  A singular 2x2
+ * system solves to d = 0, as cv::solve leaves it. */
+int r3d_debug_akaze_refine(r3d_ctx* ctx, const float* ldet, uint32_t width, uint32_t height, float ratio,
+                           const r3d_akaze_keypoint* in, uint32_t n, r3d_akaze_keypoint* out);
+
 #ifdef __cplusplus
 }
 #endif

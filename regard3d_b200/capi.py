@@ -39,6 +39,9 @@ EXPORTS = [
     "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_matches_keep_largest_biedge_component",
     "r3d_transavg_default_options", "r3d_translation_averaging", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
     "r3d_debug_acransac_score", "r3d_debug_detmath", "r3d_debug_ba_step",
+    "r3d_akaze_default_options", "r3d_akaze_levels", "r3d_akaze_detect", "r3d_features_num_images", "r3d_features_count",
+    "r3d_features_get", "r3d_free_features", "r3d_get_akaze_timing", "r3d_debug_akaze_levels",
+    "r3d_debug_akaze_refine",
 ]
 
 CHOL_DENSE, CHOL_ENVELOPE = 0, 1
@@ -48,6 +51,43 @@ SCHUR_PLAN, SCHUR_CTA = 0, 1
 ac_score_dtype = np.dtype([("lb", np.float64), ("nfa", np.float64), ("err", np.float64), ("cnt_hi", np.uint32),
                            ("cnt_lo", np.uint32), ("count", np.uint32), ("k", np.uint32)])
 DETMATH_LOG10, DETMATH_CBRT, DETMATH_COS, DETMATH_ACOS = 0, 1, 2, 3
+
+
+AKAZE_DIFF_PM_G2 = 1
+# r3d_akaze_keypoint: angle in degrees after Regard3D's conversion; class_id = evolution level
+akaze_keypoint_dtype = np.dtype([("x", np.float32), ("y", np.float32), ("size", np.float32), ("angle", np.float32),
+                                 ("response", np.float32), ("octave", np.int32), ("class_id", np.int32)])
+akaze_level_dtype = np.dtype([("octave", np.int32), ("sublevel", np.int32), ("width", np.int32), ("height", np.int32),
+                              ("sigma_size", np.int32), ("border", np.int32), ("esigma", np.float32),
+                              ("etime", np.float32), ("ratio", np.float32), ("n_tau", np.uint32)])
+AKAZE_ARRAYS = ("Lt", "Lsmooth", "Lx", "Ly", "Ldet")
+
+
+class AkazeOptions(C.Structure):
+    _fields_ = [("threshold", C.c_float), ("octaves", C.c_int32), ("sublevels", C.c_int32), ("diffusivity", C.c_int32)]
+
+
+class AkazeTiming(C.Structure):
+    _fields_ = [("upload_ms", C.c_double), ("scale_space_ms", C.c_double), ("candidates_ms", C.c_double), ("same_level_ms", C.c_double),
+                ("cross_level_ms", C.c_double), ("refine_orient_ms", C.c_double), ("total_ms", C.c_double),
+                ("images", C.c_uint32), ("batches", C.c_uint32), ("keypoints", C.c_uint32),
+                ("kernel_launches", C.c_uint32), ("devices", C.c_uint32)]
+
+
+def akaze_options(threshold=0.001, octaves=4, sublevels=4, diffusivity=AKAZE_DIFF_PM_G2):
+    o = AkazeOptions()
+    lib().r3d_akaze_default_options(C.byref(o))
+    o.threshold, o.octaves, o.sublevels, o.diffusivity = threshold, octaves, sublevels, diffusivity
+    return o
+
+
+def akaze_levels(width, height, **opts):
+    """The detector's level table of a width x height image (akaze_level_dtype)."""
+    out = np.zeros(64, akaze_level_dtype)
+    n = lib().r3d_akaze_levels(C.c_uint32(width), C.c_uint32(height), C.byref(akaze_options(**opts)), _p(out), C.c_int(64))
+    if n < 0:
+        raise R3DError(n, "r3d_akaze_levels: bad arguments")
+    return out[:n].copy()
 
 
 class R3DError(RuntimeError):
@@ -215,6 +255,11 @@ def lib():
         L = C.CDLL(LIB_PATH)
         L.r3d_last_error.restype = C.c_char_p
         L.r3d_last_error.argtypes = [C.c_void_p]
+        L.r3d_features_count.restype = C.c_uint32
+        L.r3d_features_count.argtypes = [C.c_void_p, C.c_uint32]
+        L.r3d_features_get.restype = C.c_void_p
+        L.r3d_features_get.argtypes = [C.c_void_p, C.c_uint32]
+        L.r3d_free_features.argtypes = [C.c_void_p]
         L.r3d_matches_num_pairs.restype = C.c_uint64
         L.r3d_matches_num_pairs.argtypes = [C.c_void_p]
         L.r3d_matches_total.restype = C.c_uint64
@@ -708,6 +753,75 @@ class Context:
         self._check(lib().r3d_liop_describe(self._h, _p(image), C.c_uint32(image.shape[1]), C.c_uint32(image.shape[0]),
                                             _p(kps), C.c_uint32(len(kps)), C.c_float(kp_size_factor), _p(desc)))
         return desc
+
+    def akaze_detect(self, images, **opts):
+        """Fast-AKAZE keypoints of a list of (h, w) float32 gray images in [0, 1]: one akaze_keypoint_dtype array per
+        image, in upstream order."""
+        imgs = [np.ascontiguousarray(im, np.float32) for im in images]
+        n = len(imgs)
+        ptrs = (C.c_void_p * max(n, 1))(*[im.ctypes.data for im in imgs])
+        ws = np.array([im.shape[1] if im.ndim == 2 else 0 for im in imgs] or [0], np.uint32)
+        hs = np.array([im.shape[0] if im.ndim == 2 else 0 for im in imgs] or [0], np.uint32)
+        f = C.c_void_p()
+        self._check(lib().r3d_akaze_detect(self._h, ptrs, _p(ws), _p(hs), C.c_uint32(n), C.byref(akaze_options(**opts)),
+                                           C.byref(f)))
+        try:
+            out = []
+            for i in range(n):
+                k = lib().r3d_features_count(f, C.c_uint32(i))
+                a = np.zeros(k, akaze_keypoint_dtype)
+                if k:
+                    C.memmove(a.ctypes.data, lib().r3d_features_get(f, C.c_uint32(i)), k * akaze_keypoint_dtype.itemsize)
+                out.append(a)
+            return out
+        finally:
+            lib().r3d_free_features(f)
+
+    def akaze_timing(self):
+        t = AkazeTiming()
+        self._check(lib().r3d_get_akaze_timing(self._h, C.byref(t)))
+        return {k: getattr(t, k) for k, _ in AkazeTiming._fields_}
+
+    def debug_akaze_refine(self, ldet, ratio, keypoints):
+        """The refinement kernel alone on points (akaze_keypoint_dtype) of one level's Ldet; rejected: class_id -1."""
+        ldet = np.ascontiguousarray(ldet, np.float32)
+        kps = np.ascontiguousarray(keypoints, akaze_keypoint_dtype)
+        out = np.zeros_like(kps)
+        self._check(lib().r3d_debug_akaze_refine(self._h, _p(ldet), C.c_uint32(ldet.shape[1]), C.c_uint32(ldet.shape[0]),
+                                                 C.c_float(ratio), _p(kps), C.c_uint32(len(kps)), _p(out)))
+        return out
+
+    def debug_akaze_levels(self, image, **opts):
+        """One image through the detector's kernels: per level a dict with the level record, kcontrast, the five
+        arrays (AKAZE_ARRAYS), the candidates after the same-level pass and their deletion flags after the lower- and
+        the upper-level pass."""
+        image = np.ascontiguousarray(image, np.float32)
+        h, w = image.shape
+        lv = akaze_levels(w, h, **{k: v for k, v in opts.items() if k != "threshold"})
+        npx = sum(int(l["width"]) * int(l["height"]) for l in lv)
+        cap = sum((int(l["width"]) + 1) // 2 * ((int(l["height"]) + 1) // 2) for l in lv)
+        arrays = np.zeros(5 * npx, np.float32)
+        kc = np.zeros(max(len(lv), 1), np.float32)
+        cands = np.zeros(max(cap, 1), akaze_keypoint_dtype)
+        flags = np.zeros(max(cap, 1), np.uint8)
+        counts = np.zeros(max(len(lv), 1), np.uint32)
+        self._check(lib().r3d_debug_akaze_levels(self._h, _p(image), C.c_uint32(w), C.c_uint32(h),
+                                                 C.byref(akaze_options(**opts)), _p(arrays), _p(kc), _p(cands), _p(flags),
+                                                 C.c_uint32(cap), _p(counts)))
+        out, a, c = [], 0, 0
+        for i, l in enumerate(lv):
+            lw, lh = int(l["width"]), int(l["height"])
+            d = {"level": l, "kcontrast": float(kc[i])}
+            for name in AKAZE_ARRAYS:
+                d[name] = arrays[a:a + lw * lh].reshape(lh, lw)
+                a += lw * lh
+            n = int(counts[i])
+            d["candidates"] = cands[c:c + n].copy()
+            d["deleted_lower"] = (flags[c:c + n] & 1).astype(bool)
+            d["deleted_upper"] = (flags[c:c + n] & 2).astype(bool)
+            c += n
+            out.append(d)
+        return out
 
     def debug_liop_process(self, patches):
         patches = np.ascontiguousarray(patches, np.float32).reshape(-1, 41 * 41)

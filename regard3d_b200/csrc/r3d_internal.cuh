@@ -174,6 +174,7 @@ struct r3d_ctx {
   r3d_filter_timing filter_timing{};
   r3d_relpose_timing relpose_timing{};
   r3d_resection_timing resection_timing{};
+  r3d_akaze_timing akaze_timing{};
   int host_threads = 0;
   // optional NCCL communicator (comm.cu): only the bundle adjustment exchanges data between ranks
   void* nccl_comm = nullptr;
