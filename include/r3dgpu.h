@@ -612,6 +612,13 @@ int r3d_debug_cascade_view(r3d_ctx* ctx, uint32_t view_id, uint32_t* code, uint1
  * the tensor-core pass produced for (view_db, view_query), and the pair's error bound. */
 int r3d_debug_candidate_keys(r3d_ctx* ctx, uint32_t view_db, uint32_t view_query, uint32_t* keys,
                              float* eps_abs);
+/* Diagnostics: the fp16 tensor-core operands of one view, prepared as the next matching call prepares them (every
+ * uploaded view of the first device).  *n_pad: padded rows; *kp: halves per operand row, 0 when the view has no fp16
+ * operands (integer path or exact scan only).  opQ / opD (may be NULL): n_pad x kp fp16 bit patterns of the query and
+ * database roles; stats (may be NULL): max ||a||^2, max ||fp16(a)||^2, max ||a - fp16(a)||^2, max |a_k| over the rows;
+ * *e0 (may be NULL): the norm-split exponent of the device (S0 = 2^e0, S1 = 2^(e0-11)). */
+int r3d_debug_view_operands(r3d_ctx* ctx, uint32_t view_id, uint32_t* n_pad, uint32_t* kp, uint16_t* opQ, uint16_t* opD,
+                            float* stats, int* e0);
 
 /* Diagnostics (runs on the host, no GPU needed): residual and analytic Jacobian (2 x 15: intrinsics
  * 0..5, pose 6..11, point 12..14) of one observation, as the BA kernels evaluate them. */

@@ -41,7 +41,7 @@ EXPORTS = [
     "r3d_debug_acransac_score", "r3d_debug_detmath", "r3d_debug_ba_step",
     "r3d_akaze_default_options", "r3d_akaze_levels", "r3d_akaze_detect", "r3d_features_num_images", "r3d_features_count",
     "r3d_features_get", "r3d_free_features", "r3d_get_akaze_timing", "r3d_debug_akaze_levels",
-    "r3d_debug_akaze_refine",
+    "r3d_debug_akaze_refine", "r3d_debug_view_operands",
 ]
 
 CHOL_DENSE, CHOL_ENVELOPE = 0, 1
@@ -866,6 +866,20 @@ class Context:
         eps = C.c_float()
         self._check(lib().r3d_debug_candidate_keys(self._h, C.c_uint32(view_db), C.c_uint32(view_query), _p(keys), C.byref(eps)))
         return keys, eps.value
+
+    def debug_view_operands(self, view_id):
+        """The view's fp16 operands as the next matching call prepares them: dict with opQ, opD (n_pad x kp float16,
+        None when the view has none), stats (max ||a||^2, max ||fp16(a)||^2, max ||a - fp16(a)||^2, max |a_k|) and
+        the device's norm-split exponent e0."""
+        n_pad, kp, e0 = C.c_uint32(), C.c_uint32(), C.c_int()
+        self._check(lib().r3d_debug_view_operands(self._h, C.c_uint32(view_id), C.byref(n_pad), C.byref(kp), None, None,
+                                                  None, None))
+        opQ = np.zeros((n_pad.value, kp.value), np.float16)
+        opD = np.zeros((n_pad.value, kp.value), np.float16)
+        stats = np.zeros(4, np.float32)
+        self._check(lib().r3d_debug_view_operands(self._h, C.c_uint32(view_id), C.byref(n_pad), C.byref(kp), _p(opQ),
+                                                  _p(opD), _p(stats), C.byref(e0)))
+        return {"opQ": opQ if kp.value else None, "opD": opD if kp.value else None, "stats": stats, "e0": e0.value}
 
     def debug_cholesky(self, A, method=CHOL_DENSE, ft=None, grid=0):
         """r3d_debug_cholesky on A ((n+1) x n: the matrix, whose lower triangle is read, and b as row n).  Returns

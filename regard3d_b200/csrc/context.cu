@@ -342,7 +342,9 @@ int r3d_upload_regions(r3d_ctx* ctx, uint32_t view_id, const void* desc, uint32_
     v.n = n; v.dim = dim; v.dtype = (uint32_t)dtype;
     v.n_pad = (uint32_t)pad_up((int)(n ? n : 1), kRowPad);
     v.int_ops = int_operand(dtype, dim);
-    v.tc_ok = v.int_ops || dim <= 240;  // fp16: Kp <= 256 columns; wider descriptors are matched by the exact scan only
+    // fp16: Kp <= 256 columns, and the exact re-rank reads whole 4-byte words of a row; wider descriptors and uint8 rows
+    // of D % 4 != 0 bytes are matched by the exact scan only
+    v.tc_ok = v.int_ops || (dim <= 240 && (dtype == R3D_F32 || dim % 4 == 0));
     v.kp = v.int_ops ? 0u : (uint32_t)operand_cols((int)(dim && v.tc_ok ? dim : 16));
     const size_t rb = dtype == R3D_F32 ? (size_t)dim * 4 : (size_t)dim;
     // >= one row: the extent of the u8 maps; integer path: whole 32-row groups of the permuted database map
@@ -387,6 +389,25 @@ int r3d_upload_regions(r3d_ctx* ctx, uint32_t view_id, const void* desc, uint32_
     guard.armed = false;
     w.views[view_id] = std::move(v);
   }
+  return R3D_OK;
+}
+
+int r3d_debug_view_operands(r3d_ctx* ctx, uint32_t view_id, uint32_t* n_pad, uint32_t* kp, uint16_t* opQ, uint16_t* opD,
+                            float* stats, int* e0) {
+  if (!ctx || !n_pad || !kp || ctx->workers.empty()) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_view_operands: bad arguments");
+  DeviceWorker& w = ctx->workers[0];
+  int rc = prepare_views(ctx, w);  // as the next matching call would
+  if (rc) return rc;
+  auto it = w.views.find(view_id);
+  if (it == w.views.end()) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_view_operands: unknown view");
+  const ViewDev& v = it->second;
+  *n_pad = v.n_pad;
+  *kp = (v.tc_ok && !v.int_ops) ? v.kp : 0u;
+  const size_t halves = (size_t)*n_pad * *kp;
+  if (opQ && halves) R3D_CUDA_TRY(ctx, cudaMemcpy(opQ, v.d_opQ, halves * sizeof(__half), cudaMemcpyDeviceToHost));
+  if (opD && halves) R3D_CUDA_TRY(ctx, cudaMemcpy(opD, v.d_opD, halves * sizeof(__half), cudaMemcpyDeviceToHost));
+  if (stats) R3D_CUDA_TRY(ctx, cudaMemcpy(stats, v.d_stats, 4 * sizeof(float), cudaMemcpyDeviceToHost));
+  if (e0) *e0 = w.e0;
   return R3D_OK;
 }
 

@@ -30,12 +30,17 @@ struct BatchPair {
   PairDesc pd;
 };
 
-float pair_eps(const ViewDev& vi, const ViewDev& vj) {
+// e0: the worker's norm-split exponent the views were prepared under (prepare_views runs first)
+float pair_eps(const ViewDev& vi, const ViewDev& vj, int e0) {
   if (vi.int_ops && vj.int_ops) return 0.f;  // integer path: exact keys (the chunk-id packing is covered by pack_rel)
   const double nI = vi.max_norm, nJ = vj.max_norm;
   double e = 2.0 * ((double)vi.max_dnorm * nJ + (double)vi.max_hnorm * (double)vj.max_dnorm);
-  e += std::ldexp(nI * nI + nJ * nJ, -21);         // two-piece fp16 split of the squared norms
-  e += std::ldexp((nI + nJ) * (nI + nJ), -18);     // fp32 accumulation inside the tensor core
+  // two-piece fp16 split of the squared norms: per row 2^-22 ||a||^2 while p0, p1 are normal, plus at most 2^(e0-36)
+  // when they are fp16 subnormals (a row far smaller than the largest norm of the worker's views)
+  e += std::ldexp(nI * nI + nJ * nJ, -21) + std::ldexp(1.0, e0 - 35);
+  // fp32 accumulation inside the tensor core: measured on H100 up to 2^-22 (nI + nJ)^2 per k16 step (products aligned to
+  // the running sum lose up to a quarter ulp each); twice that per step, and never less than 2^-18 (nI + nJ)^2
+  e += std::ldexp((double)std::max(8, operand_ksteps((int)vi.dim)) * (nI + nJ) * (nI + nJ), -21);
   e *= 1.001;
   return (float)e + 1e-30f;
 }
@@ -137,7 +142,7 @@ static int match_on_worker(r3d_ctx* ctx, DeviceWorker& w, const uint32_t* pairs,
     pd.descI = vi.d_desc; pd.descJ = vj.d_desc;
     pd.normI = vi.d_norm; pd.normJ = vj.d_norm;
     pd.use_tc = (!cascade && (flags & R3D_MATCH_EXACT_SCAN) == 0 && vi.tc_ok && vj.tc_ok && vi.n_pad <= kMaxDbRowsTC && vi.kp <= kMaxKBlocks * kKBlock) ? 1u : 0u;
-    pd.eps_abs = pair_eps(vi, vj);
+    pd.eps_abs = pair_eps(vi, vj, w.e0);
     {
       uint32_t nchunks = vi.n_pad / kChunk, bits = 4;
       while ((1u << bits) < nchunks) ++bits;
@@ -631,7 +636,7 @@ int r3d_debug_candidate_keys(r3d_ctx* ctx, uint32_t view_db, uint32_t view_query
   int rc = match_on_worker(ctx, w, pr, 1, 1.0f, R3D_MATCH_DEFAULT, dummy, dummy_slabs, &nn, &k);
   if (rc) return rc;
   std::memcpy(keys, k.data(), k.size() * sizeof(uint4));
-  if (eps_abs) *eps_abs = pair_eps(iI->second, iJ->second);
+  if (eps_abs) *eps_abs = pair_eps(iI->second, iJ->second, w.e0);
   return R3D_OK;
 }
 

@@ -2,6 +2,7 @@
 import numpy as np
 import pytest
 
+import fp16_keys_ref as ref
 from conftest import dict_sets, match_sets
 from regard3d_b200 import synth
 
@@ -86,25 +87,12 @@ def test_search_neighbours_bit_exact(gpu_ctx, oracle):
 
 
 def test_candidate_error_bound_holds(gpu_ctx):
-    """The certification relies on |candidate value - real distance| <= eps_abs + 2^-11 |value|."""
+    """The certification relies on |candidate value - real distance| <= eps_abs + 2^(b-23) |value|: checked term by term
+    against the float64 reference (fp16_keys_ref.check_pair) on LIOP-144, 2048 x 2048.  The other shapes and data kinds
+    are in tests/test_gpu_match_fp16_bound.py."""
     sc = synth.make_scene(2, 2048, 144, "liop", seed=14)
     _upload(gpu_ctx, sc)
-    keys, eps = gpu_ctx.debug_candidate_keys(0, 1, 2048)
-    A = sc["descs"][0].astype(np.float64)
-    B = sc["descs"][1].astype(np.float64)
-    D = (B * B).sum(1)[:, None] + (A * A).sum(1)[None, :] - 2 * B @ A.T
-    CH = 8                                     # r3d::kChunk
-    cm = D.reshape(2048, 2048 // CH, CH).min(2)
-    bits = 8                                   # 2048 rows / 8 = 256 chunks
-    kv = keys[:2048, :6].view(np.float32).astype(np.float64)
-    kc = (keys[:2048, :6] & ((1 << bits) - 1)).astype(np.int64)
-    pack = 2.0 ** (bits - 23)
-    true_at = np.take_along_axis(cm, kc, 1)
-    assert (np.abs(kv - true_at) <= eps + np.abs(kv) * pack + 1e-12).all()
-    # and the keys are the 6 smallest chunk minima up to that slack
-    srt = np.sort(cm, 1)[:, :6]
-    assert (np.abs(kv - srt) <= 2 * (eps + np.abs(srt) * pack)).all()
-    assert (np.diff(kv, axis=1) >= 0).all()
+    ref.check_pair(gpu_ctx, 0, 1, sc["descs"][0], sc["descs"][1], "synthetic LIOP-144 2048x2048")
 
 
 def test_full_size_properties_c2_slice(gpu_ctx, r3dlib):
