@@ -742,6 +742,53 @@ int r3d_debug_akaze_levels(r3d_ctx* ctx, const float* image, uint32_t width, uin
 int r3d_debug_akaze_refine(r3d_ctx* ctx, const float* ldet, uint32_t width, uint32_t height, float ratio,
                            const r3d_akaze_keypoint* in, uint32_t n, r3d_akaze_keypoint* out);
 
+/* ---- feature extraction (SURVEY.md 3: the feature stage, detector + descriptor + files) ------------------------- */
+/* R3DFeaturesThread::extractFeaturesAndDescriptors for the "Fast-AKAZE" detector list (Regard3D's default,
+ * src/Regard3DFeatures.cpp:133): per image detectAndExtract (:206-222) = the Fast-AKAZE branch (:590-614) +
+ * extractLIOPFeatures (:719-861), then KeypointSet::saveToBinFile (src/threads/R3DFeaturesThread.cpp:200). */
+typedef struct {
+  r3d_akaze_options akaze;        /* threshold = R3DFParams::threshold_ */
+  float kp_size_factor;           /* 8: getKpSizeFactor("Fast-AKAZE"), :691-716 */
+  const char* out_dir;            /* NULL: no files; else <out_dir>/<basenames[i]>.feat / .desc */
+  const char* const* basenames;   /* n_images names without extension; required when out_dir is set */
+} r3d_extract_options;
+void r3d_extract_default_options(r3d_extract_options* out);
+/* Each image is uploaded once; its keypoints (r3d_akaze_detect's, in upstream order) are described with LIOP
+ * (r3d_liop_describe's kernel and bits) while it is still resident, and the descriptors of a batch are computed on a
+ * second stream while the next batch builds its scale space.  With out_dir set, one host thread per device writes
+ * <basename>.feat / .desc in OpenMVG's layout (r3d_save_features) while the device goes on.  The images are dealt to the
+ * context's devices as r3d_akaze_detect deals them; the result does not depend on the number of devices.
+ * R3D_ERR_INVALID before any work or file for everything r3d_akaze_detect rejects, a kp_size_factor that is not finite
+ * and > 0, an empty out_dir, a missing or empty basename, or out == NULL without out_dir.  A file that cannot be
+ * written: R3D_ERR_IO naming the path (files written before stay on disk).  cb (may be NULL) receives
+ * 0.2 + 0.4 * done / n_images, message "", each time an image is finished (its files written when out_dir is set), as
+ * src/threads/R3DFeaturesThread.cpp:211-228 does; never concurrently, never decreasing.  out (may be NULL when out_dir
+ * is set): per image in image order, the keypoints (r3d_features_get) and their descriptors (r3d_features_descriptors);
+ * r3d_features_count is the reference's numberOfKeypoints_ entry of the image -- the reference lists those in
+ * thread-completion order, here they are in image order. */
+int r3d_extract_features(r3d_ctx* ctx, const float* const* images, const uint32_t* widths, const uint32_t* heights,
+                         uint32_t n_images, const r3d_extract_options* opt, r3d_progress_cb cb, void* user,
+                         r3d_features** out);
+/* count x 144 float32 in keypoint order; NULL for r3d_akaze_detect results and for images without keypoints */
+const float* r3d_features_descriptors(const r3d_features* f, uint32_t image);
+/* Host only: KeypointSet::saveToBinFile = openMVG saveFeatsToFile + saveDescsToBinFile.  feat_path: one line
+ * "x y scale orientation\n" per keypoint (std::ostream <<, precision 6, classic locale); desc_path: a size_t count, then
+ * n x dim float32.  xyso: n x 4 = x, y, scale (= size / 2), orientation (degrees).  R3D_ERR_IO naming the path. */
+int r3d_save_features(const char* feat_path, const char* desc_path, const float* xyso, const float* desc, uint64_t n,
+                      uint32_t dim);
+/* the last r3d_extract_features: device stage times (CUDA events, summed over batches and devices), the host time of
+ * the descriptor downloads and of the file writing (summed over the writer threads), the call's wall time */
+typedef struct {
+  double upload_ms;   /* images host -> device, workspace clears */
+  double detect_ms;   /* r3d_akaze_timing's stages after the upload */
+  double describe_ms; /* k_liop on the second stream */
+  double d2h_ms;      /* descriptors device -> host */
+  double write_ms;    /* .feat / .desc formatting and writing */
+  double total_ms;
+  uint32_t images, batches, keypoints, kernel_launches, devices;
+} r3d_extract_timing;
+int r3d_get_extract_timing(const r3d_ctx* ctx, r3d_extract_timing* out);
+
 #ifdef __cplusplus
 }
 #endif

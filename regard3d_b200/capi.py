@@ -42,6 +42,8 @@ EXPORTS = [
     "r3d_akaze_default_options", "r3d_akaze_levels", "r3d_akaze_detect", "r3d_features_num_images", "r3d_features_count",
     "r3d_features_get", "r3d_free_features", "r3d_get_akaze_timing", "r3d_debug_akaze_levels",
     "r3d_debug_akaze_refine", "r3d_debug_view_operands",
+    "r3d_extract_default_options", "r3d_extract_features", "r3d_features_descriptors", "r3d_save_features",
+    "r3d_get_extract_timing",
 ]
 
 CHOL_DENSE, CHOL_ENVELOPE = 0, 1
@@ -72,6 +74,33 @@ class AkazeTiming(C.Structure):
                 ("cross_level_ms", C.c_double), ("refine_orient_ms", C.c_double), ("total_ms", C.c_double),
                 ("images", C.c_uint32), ("batches", C.c_uint32), ("keypoints", C.c_uint32),
                 ("kernel_launches", C.c_uint32), ("devices", C.c_uint32)]
+
+
+class ExtractOptions(C.Structure):
+    _fields_ = [("akaze", AkazeOptions), ("kp_size_factor", C.c_float), ("out_dir", C.c_char_p),
+                ("basenames", C.POINTER(C.c_char_p))]
+
+
+class ExtractTiming(C.Structure):
+    _fields_ = [("upload_ms", C.c_double), ("detect_ms", C.c_double), ("describe_ms", C.c_double), ("d2h_ms", C.c_double),
+                ("write_ms", C.c_double), ("total_ms", C.c_double), ("images", C.c_uint32), ("batches", C.c_uint32),
+                ("keypoints", C.c_uint32), ("kernel_launches", C.c_uint32), ("devices", C.c_uint32)]
+
+
+def save_features(feat_path, desc_path, keypoints, descriptors):
+    """Host only (no GPU): KeypointSet::saveToBinFile.  keypoints: akaze_keypoint_dtype, or (n, 4) float32 x, y, scale,
+    orientation (scale = size / 2); descriptors (n, dim) float32."""
+    if isinstance(keypoints, np.ndarray) and keypoints.dtype == akaze_keypoint_dtype:
+        xyso = np.stack([keypoints["x"], keypoints["y"], keypoints["size"] / np.float32(2), keypoints["angle"]], 1)
+    else:
+        xyso = keypoints
+    xyso = np.ascontiguousarray(xyso, np.float32).reshape(-1, 4)
+    desc = np.ascontiguousarray(descriptors, np.float32)
+    dim = desc.shape[1] if desc.ndim == 2 and desc.shape[1] else 144
+    rc = lib().r3d_save_features(os.fsencode(feat_path), os.fsencode(desc_path), _p(xyso), _p(desc), C.c_uint64(len(xyso)),
+                                 C.c_uint32(dim))
+    if rc:
+        raise R3DError(rc, lib().r3d_last_error(None).decode())
 
 
 def akaze_options(threshold=0.001, octaves=4, sublevels=4, diffusivity=AKAZE_DIFF_PM_G2):
@@ -260,6 +289,8 @@ def lib():
         L.r3d_features_get.restype = C.c_void_p
         L.r3d_features_get.argtypes = [C.c_void_p, C.c_uint32]
         L.r3d_free_features.argtypes = [C.c_void_p]
+        L.r3d_features_descriptors.restype = C.c_void_p
+        L.r3d_features_descriptors.argtypes = [C.c_void_p, C.c_uint32]
         L.r3d_matches_num_pairs.restype = C.c_uint64
         L.r3d_matches_num_pairs.argtypes = [C.c_void_p]
         L.r3d_matches_total.restype = C.c_uint64
@@ -776,6 +807,48 @@ class Context:
             return out
         finally:
             lib().r3d_free_features(f)
+
+    def extract_features(self, images, out_dir=None, basenames=None, threshold=1e-3, kp_size_factor=8.0, progress=None):
+        """Fast-AKAZE keypoints described with LIOP-144, each image uploaded once: one (akaze_keypoint_dtype array,
+        (n, 144) float32) pair per image.  out_dir: also write <out_dir>/<basenames[i]>.feat / .desc; progress(fraction,
+        message, user), as compute_matches takes it, runs after each finished image (0.2 + 0.4 done / n)."""
+        imgs = [np.ascontiguousarray(im, np.float32) for im in images]
+        n = len(imgs)
+        ptrs = (C.c_void_p * max(n, 1))(*[im.ctypes.data for im in imgs])
+        ws = np.array([im.shape[1] if im.ndim == 2 else 0 for im in imgs] or [0], np.uint32)
+        hs = np.array([im.shape[0] if im.ndim == 2 else 0 for im in imgs] or [0], np.uint32)
+        o = ExtractOptions()
+        lib().r3d_extract_default_options(C.byref(o))
+        o.akaze = akaze_options(threshold=threshold)
+        o.kp_size_factor = kp_size_factor
+        names = None
+        if out_dir is not None:
+            o.out_dir = os.fsencode(out_dir)
+        if basenames is not None:
+            names = (C.c_char_p * max(len(basenames), 1))(*[None if b is None else os.fsencode(b) for b in basenames])
+            o.basenames = C.cast(names, C.POINTER(C.c_char_p))
+        cb = PROGRESS_CB(progress) if progress else C.cast(None, PROGRESS_CB)
+        f = C.c_void_p()
+        self._check(lib().r3d_extract_features(self._h, ptrs, _p(ws), _p(hs), C.c_uint32(n), C.byref(o), cb, None,
+                                               C.byref(f)))
+        try:
+            out = []
+            for i in range(n):
+                k = lib().r3d_features_count(f, C.c_uint32(i))
+                a = np.zeros(k, akaze_keypoint_dtype)
+                d = np.zeros((k, 144), np.float32)
+                if k:
+                    C.memmove(a.ctypes.data, lib().r3d_features_get(f, C.c_uint32(i)), k * akaze_keypoint_dtype.itemsize)
+                    C.memmove(d.ctypes.data, lib().r3d_features_descriptors(f, C.c_uint32(i)), d.nbytes)
+                out.append((a, d))
+            return out
+        finally:
+            lib().r3d_free_features(f)
+
+    def extract_timing(self):
+        t = ExtractTiming()
+        self._check(lib().r3d_get_extract_timing(self._h, C.byref(t)))
+        return {k: getattr(t, k) for k, _ in ExtractTiming._fields_}
 
     def akaze_timing(self):
         t = AkazeTiming()

@@ -126,7 +126,73 @@ bool R3DComputeMatches::computeMatches(R3DFParams& params, bool svgOutput, const
   return true;
 }
 
+bool R3DComputeMatches::extractFeatures(const std::vector<const float*>& images, const R3DFParams& params,
+                                        const R3DProjectPaths& paths) {
+  if (!ctx_) return false;
+  if (params.keypointDetectorList_ != std::vector<std::string>{"Fast-AKAZE"}) {
+    lastError_ = "extractFeatures: only the detector list {\"Fast-AKAZE\"} runs on the GPU";
+    return false;
+  }
+  const uint32_t n = (uint32_t)imageInfoVector_.size();
+  if (images.size() != n) {
+    lastError_ = "extractFeatures: one image per ImageInfo expected";
+    return false;
+  }
+  std::vector<std::string> bases(n);
+  std::vector<const char*> base_ptrs(n);
+  std::vector<uint32_t> widths(n), heights(n);
+  for (uint32_t v = 0; v < n; ++v) {
+    bases[v] = strip_ext(imageInfoVector_[v].filename_);  // R3DFeaturesThread.cpp:132-136
+    base_ptrs[v] = bases[v].c_str();
+    widths[v] = (uint32_t)imageInfoVector_[v].imageWidth_;
+    heights[v] = (uint32_t)imageInfoVector_[v].imageHeight_;
+  }
+  r3d_extract_options o;
+  r3d_extract_default_options(&o);
+  o.akaze.threshold = params.threshold_;
+  o.out_dir = paths.relativeMatchesPath_.c_str();
+  o.basenames = base_ptrs.data();
+  r3d_features* f = nullptr;
+  const int rc = r3d_extract_features(ctx_, images.data(), widths.data(), heights.data(), n, &o, progress_trampoline,
+                                      this, &f);
+  if (rc != R3D_OK) {
+    lastError_ = r3d_last_error(ctx_);
+    return false;
+  }
+  statistics_.numberOfKeypoints_.resize(n);
+  for (uint32_t v = 0; v < n; ++v) statistics_.numberOfKeypoints_[v] = (int)r3d_features_count(f, v);
+  r3d_free_features(f);
+  return true;
+}
+
 }  // namespace r3d_shim
+
+// C hook so the Python tests can drive the shim's feature extraction: detector "Fast-AKAZE" unless detector is given
+extern "C" int r3d_shim_extract_features(const char* matches_dir, const char* const* image_filenames, const float* const* images,
+                                         const uint32_t* widths, const uint32_t* heights, uint32_t n, float threshold,
+                                         const char* detector, uint32_t* n_keypoints_out, float* last_progress) {
+  r3d_shim::R3DComputeMatches cm;
+  float last = -1.f;
+  cm.setMainFrame([&](float f, const std::string&) { last = f; });
+  r3d_shim::ImageInfoVector iiv(n);
+  for (uint32_t v = 0; v < n; ++v) {
+    iiv[v].filename_ = image_filenames[v];
+    iiv[v].imageWidth_ = (int)widths[v];
+    iiv[v].imageHeight_ = (int)heights[v];
+  }
+  cm.addImages(iiv);
+  r3d_shim::R3DFParams params;
+  params.keypointDetectorList_ = {detector ? detector : "Fast-AKAZE"};
+  params.threshold_ = threshold;
+  r3d_shim::R3DProjectPaths paths;
+  paths.relativeMatchesPath_ = matches_dir;
+  const bool ok = cm.extractFeatures(std::vector<const float*>(images, images + n), params, paths);
+  *last_progress = last;
+  if (!ok) return -1;
+  const auto& st = cm.getStatistics();
+  for (uint32_t v = 0; v < n; ++v) n_keypoints_out[v] = (uint32_t)st.numberOfKeypoints_[v];
+  return 0;
+}
 
 // C hook so the Python tests can drive the C++ shim end to end.
 extern "C" int r3d_shim_compute_matches(const char* matches_dir, const char* const* image_filenames, const uint32_t* widths,

@@ -65,6 +65,13 @@ class R3DComputeMatches {
   bool computeMatches(R3DFParams& params, bool svgOutput, const R3DProjectPaths& paths, int cameraModel,
                       int matchingAlgorithm);
 
+  // twin of R3DFeaturesThread::extractFeaturesAndDescriptors (src/threads/R3DFeaturesThread.cpp:128-209) for the
+  // "Fast-AKAZE" detector list: images[v] is imageInfoVector_[v] decoded by the caller to float gray in [0, 1]
+  // (width x height row-major, :161-191).  Writes <basename>.feat / .desc under paths.relativeMatchesPath_, fills
+  // statistics_.numberOfKeypoints_ (image order) and reports 0.2 .. 0.6 through the progress sink.  Any other detector
+  // list: false with lastError() set.
+  bool extractFeatures(const std::vector<const float*>& images, const R3DFParams& params, const R3DProjectPaths& paths);
+
   void updateProgress(float progress, const std::string& msg);
 
   struct R3DComputeMatchesStatistics {

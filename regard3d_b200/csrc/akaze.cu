@@ -23,13 +23,16 @@
 #include <chrono>
 #include <climits>
 #include <cmath>
+#include <condition_variable>
 #include <cstring>
+#include <deque>
 #include <memory>
 #include <thread>
 #include <vector>
 
 struct r3d_features {
   std::vector<std::vector<r3d_akaze_keypoint>> kps;
+  std::vector<std::vector<float>> desc;  // r3d_extract_features only: per image kps[i].size() x 144
 };
 
 namespace r3d {
@@ -709,10 +712,23 @@ struct Timer {
 
 dim3 grid2(int w, int h, int n) { return dim3((w + 31) / 32, (h + 7) / 8, n); }
 
-// One batch of images on one device.  kps[b]: the image's keypoints on return.
+// r3d_extract_features' state of one batch between its detection and its descriptors: run_batch leaves the original
+// images resident (slot b = the batch's image b) and releases everything else; launch_describe runs k_liop on
+// w.copy_stream, which the next batch's scale space overlaps; finish_describe downloads and releases.
+struct Pending {
+  uint32_t i0 = 0, i1 = 0;         // the batch's images, with or without levels
+  std::vector<uint32_t> slot_img;  // image of each slot
+  liop::Slots S{};
+  std::vector<void*> held;         // image blocks, maps, descriptors
+  float* d_desc = nullptr;
+  uint32_t n = 0;                  // keypoints of the batch
+};
+
+// One batch of images on one device.  kps[b]: the image's keypoints on return.  keep: hand the original images to
+// keep->held / keep->S instead of releasing them.
 int run_batch(r3d_ctx* ctx, DeviceWorker& w, std::vector<Image*>& imgs, float threshold,
               std::vector<std::vector<r3d_akaze_keypoint>*>& kps_out, const Debug* dbg, double* stage_ms,
-              uint32_t* launches) {
+              uint32_t* launches, Pending* keep = nullptr) {
   const int B = (int)imgs.size();
   cudaStream_t st = w.stream;
   int nl = 0;
@@ -740,11 +756,16 @@ int run_batch(r3d_ctx* ctx, DeviceWorker& w, std::vector<Image*>& imgs, float th
   for (int b = 0; b < B; ++b) {
     Image& im = *imgs[b];
     const size_t P = (size_t)im.W * im.H;
-    float* base = (float*)alloc(image_bytes(im));
-    if (!base) return fail(ctx, R3D_ERR_NOMEM, "r3d_akaze_detect: device allocation failed");
+    // the original image in a block of its own (no stage writes it): r3d_extract_features describes from it later
+    float* base = (float*)alloc(image_bytes(im) - P * 4);
+    float* img = (float*)pool_alloc(w, P * 4);
+    if (img) (keep ? keep->held : blocks).push_back(img);
+    if (!base || !img) return fail(ctx, R3D_ERR_NOMEM, "r3d_akaze_detect: device allocation failed");
     ImgMem& m = M[b];
+    m.img = img;
+    if (keep) keep->S.img[b] = img, keep->S.w[b] = im.W, keep->S.h[b] = im.H;
     float* p = base;
-    for (float** q : {&m.img, &m.ls, &m.sx, &m.sy, &m.flow, &m.lstep, &m.tmp, &m.lxx, &m.lxy, &m.lyy}) *q = p, p += P;
+    for (float** q : {&m.ls, &m.sx, &m.sy, &m.flow, &m.lstep, &m.tmp, &m.lxx, &m.lxy, &m.lyy}) *q = p, p += P;
     for (const r3d_akaze_level& l : im.lv) {
       const size_t lp = (size_t)l.width * l.height;
       m.Lt.push_back(p), p += lp;
@@ -1171,6 +1192,222 @@ int prepare(r3d_ctx* ctx, const float* const* images, const uint32_t* widths, co
   return R3D_OK;
 }
 
+// The maps on the host (libm cos / sin, as r3d_liop_describe computes them), 24 B per keypoint to the device, k_liop
+// on w.copy_stream, timed by ev[0] / ev[1].  The stream is idle here: finish_describe waited for the previous batch.
+int launch_describe(r3d_ctx* ctx, DeviceWorker& w, Pending& p, const std::vector<std::vector<r3d_akaze_keypoint>>& kps,
+                    float factor, const liop::Tables* d_T, const cudaEvent_t* ev) {
+  p.S.n = (int)p.slot_img.size();
+  uint32_t n = 0;
+  for (int s = 0; s < p.S.n; ++s) p.S.first[s] = n, n += (uint32_t)kps[p.slot_img[s]].size();
+  p.S.first[p.S.n] = n;
+  p.n = n;
+  if (n == 0) return R3D_OK;
+  std::vector<float> hM((size_t)n * 6);
+  parallel_for(ctx->host_threads, (size_t)p.S.n, [&](size_t s) {
+    const std::vector<r3d_akaze_keypoint>& k = kps[p.slot_img[s]];
+    float* m = &hM[(size_t)p.S.first[s] * 6];
+    for (size_t j = 0; j < k.size(); ++j) liop::affine_of(k[j].x, k[j].y, k[j].size, k[j].angle, factor, m + 6 * j);
+  });
+  float* d_M = (float*)pool_alloc(w, hM.size() * 4);
+  if (d_M) p.held.push_back(d_M);
+  p.d_desc = (float*)pool_alloc(w, (size_t)n * liop::kDim * 4);
+  if (p.d_desc) p.held.push_back(p.d_desc);
+  if (!d_M || !p.d_desc) return fail(ctx, R3D_ERR_NOMEM, "r3d_extract_features: device allocation failed");
+  const cudaStream_t cs = w.copy_stream;
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_M, hM.data(), hM.size() * 4, cudaMemcpyHostToDevice, cs));
+  R3D_CUDA_TRY(ctx, cudaEventRecord(ev[0], cs));
+  if (int rc = liop::describe(ctx, cs, p.S, d_M, n, d_T, p.d_desc)) return rc;
+  R3D_CUDA_TRY(ctx, cudaEventRecord(ev[1], cs));
+  return R3D_OK;
+}
+
+// waits for the batch's descriptors, downloads them per image and releases the batch's images
+int finish_describe(r3d_ctx* ctx, DeviceWorker& w, Pending& p, std::vector<std::vector<float>>& desc,
+                    const cudaEvent_t* ev, double* describe_ms, double* d2h_ms) {
+  if (p.n) {
+    R3D_CUDA_TRY(ctx, cudaEventSynchronize(ev[1]));
+    float ms = 0.0f;
+    R3D_CUDA_TRY(ctx, cudaEventElapsedTime(&ms, ev[0], ev[1]));
+    *describe_ms += ms;
+    const auto t0 = std::chrono::steady_clock::now();
+    for (size_t s = 0; s < p.slot_img.size(); ++s) {
+      const size_t k = p.S.first[s + 1] - p.S.first[s];
+      std::vector<float>& d = desc[p.slot_img[s]];
+      d.resize(k * liop::kDim);
+      if (k)
+        R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d.data(), p.d_desc + (size_t)p.S.first[s] * liop::kDim,
+                                          k * liop::kDim * 4, cudaMemcpyDeviceToHost, w.copy_stream));
+    }
+    R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.copy_stream));
+    *d2h_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  }
+  for (void* q : p.held) pool_release(w, q);
+  p.held.clear();
+  p.n = 0;
+  return R3D_OK;
+}
+
+// r3d_extract_features' host side: describe the batches, then hand each finished image to the device's file writer or
+// report it directly
+struct Extract {
+  float factor;
+  const char* out_dir;
+  const char* const* basenames;
+  bool keep;                        // the caller wants the arrays (out != NULL); else the writer frees them
+  std::function<void()> finished;   // one image done: progress
+};
+
+// one host thread per device: formats and writes the files of finished images while the device works on
+struct Writer {
+  std::mutex mu;
+  std::condition_variable cv;
+  std::deque<uint32_t> q;
+  bool closed = false;
+  std::atomic<bool> failed{false};
+  std::string bad;  // the first path that could not be written
+  double ms = 0.0;
+  std::thread th;
+  void push(uint32_t i) {
+    {
+      std::lock_guard<std::mutex> lk(mu);
+      q.push_back(i);
+    }
+    cv.notify_one();
+  }
+  void close() {
+    {
+      std::lock_guard<std::mutex> lk(mu);
+      closed = true;
+    }
+    cv.notify_one();
+    if (th.joinable()) th.join();
+  }
+  void run(r3d_features& F, const Extract& X) {
+    for (;;) {
+      uint32_t i;
+      {
+        std::unique_lock<std::mutex> lk(mu);
+        cv.wait(lk, [&] { return closed || !q.empty(); });
+        if (q.empty()) return;
+        i = q.front();
+        q.pop_front();
+      }
+      if (failed) continue;
+      const auto t0 = std::chrono::steady_clock::now();
+      const std::vector<r3d_akaze_keypoint>& k = F.kps[i];
+      std::vector<float> xyso(k.size() * 4);
+      for (size_t j = 0; j < k.size(); ++j)  // SIOPointFeature: scale = size / 2 (Regard3DFeatures.cpp:846-849)
+        xyso[4 * j] = k[j].x, xyso[4 * j + 1] = k[j].y, xyso[4 * j + 2] = k[j].size / 2.0f, xyso[4 * j + 3] = k[j].angle;
+      const std::string base = std::string(X.out_dir) + "/" + X.basenames[i];
+      const std::string feat = base + ".feat", desc = base + ".desc";
+      if (const char* b = save_features(feat.c_str(), desc.c_str(), xyso.data(), F.desc[i].data(), k.size(), liop::kDim)) {
+        bad = b;
+        failed = true;
+      } else {
+        if (!X.keep) std::vector<r3d_akaze_keypoint>().swap(F.kps[i]), std::vector<float>().swap(F.desc[i]);
+        X.finished();
+      }
+      ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    }
+  }
+};
+
+struct Acc {  // one device's share of a call
+  double ms[kStages] = {}, describe_ms = 0.0, d2h_ms = 0.0;
+  uint32_t launches = 0, batches = 0, keypoints = 0;
+  int rc = R3D_OK;
+};
+
+// r3d_akaze_detect (X == nullptr) and r3d_extract_features: the images are dealt to the context's devices in
+// contiguous slices; each device runs its slice in batches of at most kMaxBatch images and half its free memory, on a
+// host thread of its own.  With X, batch b's descriptors are computed on the second stream while batch b + 1 builds its
+// scale space, and W[d] writes the files.
+int run_devices(r3d_ctx* ctx, std::vector<Image>& ims, float threshold, r3d_features& F, const Extract* X,
+                std::vector<std::unique_ptr<Writer>>* W, std::vector<Acc>& acc) {
+  const uint32_t n_images = (uint32_t)ims.size();
+  const int nd = (int)acc.size();
+  auto run_device = [&](int d) {
+    Acc& A = acc[d];
+    DeviceWorker& w = ctx->workers[d];
+    const uint32_t i0 = (uint32_t)((uint64_t)n_images * d / nd), i1 = (uint32_t)((uint64_t)n_images * (d + 1) / nd);
+    auto cuda = [&](cudaError_t e, const char* what) {
+      if (e != cudaSuccess) A.rc = fail(ctx, R3D_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
+      return e == cudaSuccess;
+    };
+    if (!cuda(cudaSetDevice(w.device), "cudaSetDevice")) return;
+    size_t free_b = 0, total_b = 0;
+    if (!cuda(cudaMemGetInfo(&free_b, &total_b), "cudaMemGetInfo")) return;
+    const size_t budget = std::max<size_t>(free_b / 2, (size_t)1 << 28);
+    Pending prev, cur;
+    liop::Tables* d_T = nullptr;
+    Events<2> ev;
+    struct Cleanup {  // on every exit: nothing on the second stream may still read a block that goes back to the pool
+      DeviceWorker& w;
+      Pending &a, &b;
+      liop::Tables*& t;
+      ~Cleanup() {
+        cudaStreamSynchronize(w.copy_stream);
+        for (Pending* p : {&a, &b})
+          for (void* q : p->held) pool_release(w, q);
+        pool_release(w, t);
+      }
+    } cleanup{w, prev, cur, d_T};
+    if (X) {
+      if (!cuda(ev.create(true), "cudaEventCreate")) return;
+      if (!(d_T = liop::tables_to_device(w, w.stream)) || !cuda(cudaStreamSynchronize(w.stream), "tables")) {
+        A.rc = fail(ctx, R3D_ERR_NOMEM, "r3d_extract_features: device allocation failed");
+        return;
+      }
+    }
+    // the images of a finished batch go to the writer, or are reported at once
+    auto finish = [&](Pending& p) -> int {
+      if (int rc = finish_describe(ctx, w, p, F.desc, ev.e, &A.describe_ms, &A.d2h_ms)) return rc;
+      for (uint32_t i = p.i0; i < p.i1; ++i) {
+        A.keypoints += (uint32_t)F.kps[i].size();
+        if (W) (*W)[d]->push(i);
+        else X->finished();
+      }
+      p.i0 = p.i1 = 0;
+      return R3D_OK;
+    };
+    for (uint32_t i = i0; i < i1;) {
+      if (W && (*W)[d]->failed) return;  // a file could not be written: the call fails, stop early
+      std::vector<akaze::Image*> work;  // images too small for a single level have no keypoints and stay out
+      std::vector<std::vector<r3d_akaze_keypoint>*> wout;
+      size_t bytes = 0;
+      int taken = 0;
+      cur = Pending();
+      cur.i0 = i;
+      while (i < i1 && taken < akaze::kMaxBatch && (taken == 0 || bytes + akaze::image_bytes(ims[i]) <= budget)) {
+        bytes += akaze::image_bytes(ims[i]);
+        if (!ims[i].lv.empty()) work.push_back(&ims[i]), wout.push_back(&F.kps[i]), cur.slot_img.push_back(i);
+        ++taken, ++i;
+      }
+      cur.i1 = i;
+      if (!work.empty() &&
+          (A.rc = run_batch(ctx, w, work, threshold, wout, nullptr, A.ms, &A.launches, X ? &cur : nullptr)))
+        return;
+      ++A.batches;
+      if (!X) continue;
+      if ((A.rc = finish(prev))) return;
+      if ((A.rc = launch_describe(ctx, w, cur, F.kps, X->factor, d_T, ev.e))) return;
+      if (cur.n) ++A.launches;
+      std::swap(prev, cur);
+    }
+    if (X) A.rc = finish(prev);
+  };
+  if (nd == 1) {
+    run_device(0);
+  } else {
+    std::vector<std::thread> th;
+    for (int d = 0; d < nd; ++d) th.emplace_back(run_device, d);
+    for (std::thread& t : th) t.join();
+  }
+  for (const Acc& A : acc)
+    if (A.rc) return A.rc;
+  return R3D_OK;
+}
+
 }  // namespace akaze
 }  // namespace r3d
 
@@ -1202,52 +1439,11 @@ extern "C" int r3d_akaze_detect(r3d_ctx* ctx, const float* const* images, const 
   const auto t0 = std::chrono::steady_clock::now();
   std::unique_ptr<r3d_features> F(new r3d_features());
   F->kps.resize(n_images);
-  // the images are dealt to the context's devices in contiguous slices; each device runs its slice in batches of at
-  // most kMaxBatch images and half its free memory, on a host thread of its own
   const int nd = (int)std::min<size_t>(ctx->workers.size(), std::max<uint32_t>(n_images, 1));
-  struct Acc {
-    double ms[akaze::kStages] = {};
-    uint32_t launches = 0, batches = 0;
-    int rc = R3D_OK;
-  };
-  std::vector<Acc> acc(nd);
-  auto run_device = [&](int d) {
-    Acc& A = acc[d];
-    DeviceWorker& w = ctx->workers[d];
-    const uint32_t i0 = (uint32_t)((uint64_t)n_images * d / nd), i1 = (uint32_t)((uint64_t)n_images * (d + 1) / nd);
-    auto cuda = [&](cudaError_t e, const char* what) {
-      if (e != cudaSuccess) A.rc = fail(ctx, R3D_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
-      return e == cudaSuccess;
-    };
-    if (!cuda(cudaSetDevice(w.device), "cudaSetDevice")) return;
-    size_t free_b = 0, total_b = 0;
-    if (!cuda(cudaMemGetInfo(&free_b, &total_b), "cudaMemGetInfo")) return;
-    const size_t budget = std::max<size_t>(free_b / 2, (size_t)1 << 28);
-    for (uint32_t i = i0; i < i1;) {
-      std::vector<akaze::Image*> work;  // images too small for a single level have no keypoints and stay out
-      std::vector<std::vector<r3d_akaze_keypoint>*> wout;
-      size_t bytes = 0;
-      int taken = 0;
-      while (i < i1 && taken < akaze::kMaxBatch && (taken == 0 || bytes + akaze::image_bytes(ims[i]) <= budget)) {
-        bytes += akaze::image_bytes(ims[i]);
-        if (!ims[i].lv.empty()) work.push_back(&ims[i]), wout.push_back(&F->kps[i]);
-        ++taken, ++i;
-      }
-      if (!work.empty() && (A.rc = akaze::run_batch(ctx, w, work, opt->threshold, wout, nullptr, A.ms, &A.launches)))
-        return;
-      ++A.batches;
-    }
-  };
-  if (nd == 1) {
-    run_device(0);
-  } else {
-    std::vector<std::thread> th;
-    for (int d = 0; d < nd; ++d) th.emplace_back(run_device, d);
-    for (std::thread& t : th) t.join();
-  }
+  std::vector<akaze::Acc> acc(nd);
+  if ((rc = akaze::run_devices(ctx, ims, opt->threshold, *F, nullptr, nullptr, acc))) return rc;
   r3d_akaze_timing T{};
-  for (const Acc& A : acc) {
-    if (A.rc) return A.rc;
+  for (const akaze::Acc& A : acc) {
     T.upload_ms += A.ms[0], T.scale_space_ms += A.ms[1], T.candidates_ms += A.ms[2], T.same_level_ms += A.ms[3];
     T.cross_level_ms += A.ms[4], T.refine_orient_ms += A.ms[5];
     T.kernel_launches += A.launches, T.batches += A.batches;
@@ -1273,6 +1469,87 @@ extern "C" void r3d_free_features(r3d_features* f) { delete f; }
 extern "C" int r3d_get_akaze_timing(const r3d_ctx* ctx, r3d_akaze_timing* out) {
   if (!ctx || !out) return R3D_ERR_INVALID;
   *out = ctx->akaze_timing;
+  return R3D_OK;
+}
+
+extern "C" void r3d_extract_default_options(r3d_extract_options* out) {
+  if (!out) return;
+  r3d_akaze_default_options(&out->akaze);
+  out->kp_size_factor = 8.0f;
+  out->out_dir = nullptr;
+  out->basenames = nullptr;
+}
+
+extern "C" int r3d_extract_features(r3d_ctx* ctx, const float* const* images, const uint32_t* widths,
+                                    const uint32_t* heights, uint32_t n_images, const r3d_extract_options* opt,
+                                    r3d_progress_cb cb, void* user, r3d_features** out) {
+  if (out) *out = nullptr;
+  if (!opt || !std::isfinite(opt->kp_size_factor) || opt->kp_size_factor <= 0.0f)
+    return fail(ctx, R3D_ERR_INVALID, "r3d_extract_features: bad options");
+  const bool files = opt->out_dir != nullptr;
+  if (files) {
+    if (!*opt->out_dir || (n_images && !opt->basenames))
+      return fail(ctx, R3D_ERR_INVALID, "r3d_extract_features: empty out_dir or no basenames");
+    for (uint32_t i = 0; i < n_images; ++i)
+      if (!opt->basenames[i] || !*opt->basenames[i])
+        return fail(ctx, R3D_ERR_INVALID, "r3d_extract_features: basename " + std::to_string(i) + " is missing");
+  } else if (!out) {
+    return fail(ctx, R3D_ERR_INVALID, "r3d_extract_features: neither out nor out_dir");
+  }
+  std::vector<akaze::Image> ims;
+  int rc = akaze::prepare(ctx, images, widths, heights, n_images, &opt->akaze, ims);
+  if (rc) return rc;
+  const auto t0 = std::chrono::steady_clock::now();
+  std::unique_ptr<r3d_features> F(new r3d_features());
+  F->kps.resize(n_images);
+  F->desc.resize(n_images);
+  const int nd = (int)std::min<size_t>(ctx->workers.size(), std::max<uint32_t>(n_images, 1));
+  // R3DFeaturesThread::sendMsgToMainFrame (src/threads/R3DFeaturesThread.cpp:211-228), one call at a time
+  std::mutex progress_mu;
+  uint32_t done = 0;
+  akaze::Extract X{opt->kp_size_factor, opt->out_dir, opt->basenames, out != nullptr, [&] {
+                     std::lock_guard<std::mutex> lk(progress_mu);
+                     ++done;
+                     const float finished = static_cast<float>(done) / static_cast<int>(n_images);
+                     if (cb) cb(finished * 0.4f + 0.2f, "", user);
+                   }};
+  std::vector<std::unique_ptr<akaze::Writer>> W;
+  if (files)
+    for (int d = 0; d < nd; ++d) {
+      W.emplace_back(new akaze::Writer());
+      akaze::Writer* wr = W.back().get();
+      wr->th = std::thread([wr, &F, &X] { wr->run(*F, X); });
+    }
+  std::vector<akaze::Acc> acc(nd);
+  rc = akaze::run_devices(ctx, ims, opt->akaze.threshold, *F, &X, files ? &W : nullptr, acc);
+  r3d_extract_timing T{};
+  for (std::unique_ptr<akaze::Writer>& wr : W) {
+    wr->close();
+    T.write_ms += wr->ms;
+    if (!rc && wr->failed) rc = fail(ctx, R3D_ERR_IO, "r3d_extract_features: cannot write " + wr->bad);
+  }
+  if (rc) return rc;
+  for (const akaze::Acc& A : acc) {
+    T.upload_ms += A.ms[0];
+    for (int s = 1; s < akaze::kStages; ++s) T.detect_ms += A.ms[s];
+    T.describe_ms += A.describe_ms, T.d2h_ms += A.d2h_ms;
+    T.kernel_launches += A.launches, T.batches += A.batches, T.keypoints += A.keypoints;
+  }
+  T.total_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  T.images = n_images;
+  T.devices = (uint32_t)nd;
+  ctx->extract_timing = T;
+  if (out) *out = F.release();
+  return R3D_OK;
+}
+
+extern "C" const float* r3d_features_descriptors(const r3d_features* f, uint32_t image) {
+  return f && image < f->desc.size() && !f->desc[image].empty() ? f->desc[image].data() : nullptr;
+}
+
+extern "C" int r3d_get_extract_timing(const r3d_ctx* ctx, r3d_extract_timing* out) {
+  if (!ctx || !out) return R3D_ERR_INVALID;
+  *out = ctx->extract_timing;
   return R3D_OK;
 }
 

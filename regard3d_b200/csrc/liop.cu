@@ -7,7 +7,8 @@
 //   warp   cv::warpAffine(img, patch 41x41, M, INTER_LINEAR | WARP_INVERSE_MAP)  :803       k_liop: stage 1
 //   blur   cv::GaussianBlur(patch, sigma 1.2)  (11 taps, BORDER_REFLECT_101)     :807       k_liop: stage 2
 //   desc   r3d_vl_liopdesc_process (src/thirdparty/liop/vl_liop.c:434-575)       :828       k_liop: stages 3-5
-// One CTA per keypoint.  The descriptor is order based: 673 disc pixels ranked by intensity with the reference's own
+// One CTA per keypoint of a whole batch of images: a by-value table (Slots) holds each image's pointer and shape and
+// the range of keypoints that sample it; r3d_liop_describe launches it with one slot.  The descriptor is order based: 673 disc pixels ranked by intensity with the reference's own
 // quick sort (vl_qsort-def.h:123-162 -- the order of EQUAL intensities is a property of that exact procedure, and
 // equal intensities are common in flat image regions), six rank bins, per pixel the order pattern of 4 neighbours
 // sampled on a radius-6 circle, weighted by the number of neighbour pairs that differ by more than 5/255 of the
@@ -21,7 +22,7 @@ namespace r3d {
 namespace liop {
 
 constexpr int kSide = 41, kPix = kSide * kSide;
-constexpr int kNeigh = 4, kSpatialBins = 6, kDim = 144;
+constexpr int kNeigh = 4, kSpatialBins = 6;
 constexpr int kMaxDisc = 704;          // >= number of disc pixels (673 for a 41x41 patch, radius 6)
 constexpr int kThreads = 128;
 
@@ -44,8 +45,8 @@ __device__ __forceinline__ long long floor_d(double x) {  // vl_floor_d
   return (x >= 0 || (double)xi == x) ? xi : xi - 1;
 }
 
-__global__ void __launch_bounds__(kThreads) k_liop(const float* __restrict__ img, int w, int h, const float* __restrict__ Ms,
-                                                   uint32_t n, const Tables* __restrict__ T, float* __restrict__ desc_out) {
+__global__ void __launch_bounds__(kThreads) k_liop(Slots S, const float* __restrict__ Ms, uint32_t n,
+                                                   const Tables* __restrict__ T, float* __restrict__ desc_out) {
   __shared__ float s_a[kPix], s_b[kPix];
   __shared__ unsigned long long s_sort[kMaxDisc];  // (intensity bits << 32) | disc index: swapped as one word
   __shared__ uint16_t s_rank_of[kMaxDisc];         // sorted position -> disc index
@@ -54,6 +55,10 @@ __global__ void __launch_bounds__(kThreads) k_liop(const float* __restrict__ img
   __shared__ float s_thr, s_norm;
   const uint32_t kp = blockIdx.x;
   if (kp >= n) return;
+  int slot = 0;
+  while (slot + 1 < S.n && kp >= S.first[slot + 1]) ++slot;
+  const float* __restrict__ img = S.img[slot];
+  const int w = S.w[slot], h = S.h[slot];
   const int tid = threadIdx.x;
   const bool raw_patches = Ms == nullptr;  // diagnostics: img holds n ready 41x41 patches (stages 1-2 skipped)
   if (raw_patches) {
@@ -254,7 +259,7 @@ static const Tables& host_tables() {
 
 // The 2x3 inverse map of src/Regard3DFeatures.cpp:766-800 (float arithmetic; cos / sin in double by the host's libm,
 // exactly what the reference's host code evaluates)
-static void affine_of(float x, float y, float kp_size, float kp_angle, float factor, float* M) {
+void affine_of(float x, float y, float kp_size, float kp_angle, float factor, float* M) {
   const float angle = -90.0f - kp_angle;
   const float scale = kp_size / (float)kSide * factor;
   const float alpha = (float)(scale * std::cos(angle * M_PI / 180.0f));
@@ -266,6 +271,23 @@ static void affine_of(float x, float y, float kp_size, float kp_angle, float fac
   M[3] = -beta;
   M[4] = alpha;
   M[5] = alpha * trans_y - beta * trans_x + beta * x + (1.0f - alpha) * y;
+}
+
+Tables* tables_to_device(DeviceWorker& w, cudaStream_t st) {
+  Tables* d = (Tables*)pool_alloc(w, sizeof(Tables));
+  if (d && cudaMemcpyAsync(d, &host_tables(), sizeof(Tables), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+    pool_release(w, d);
+    return nullptr;
+  }
+  return d;
+}
+
+int describe(r3d_ctx* ctx, cudaStream_t st, const Slots& S, const float* d_M, uint32_t n, const Tables* d_T,
+             float* d_desc) {
+  if (n == 0) return R3D_OK;
+  k_liop<<<n, kThreads, 0, st>>>(S, d_M, n, d_T, d_desc);
+  R3D_CUDA_TRY(ctx, cudaGetLastError());
+  return R3D_OK;
 }
 
 }  // namespace liop
@@ -301,8 +323,10 @@ extern "C" int r3d_liop_describe(r3d_ctx* ctx, const float* image, uint32_t widt
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_img, image, (size_t)width * height * 4, cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_M, hM.data(), hM.size() * 4, cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_T, &T, sizeof(liop::Tables), cudaMemcpyHostToDevice, w.stream));
-  liop::k_liop<<<n, liop::kThreads, 0, w.stream>>>(d_img, (int)width, (int)height, d_M, n, d_T, d_desc);
-  R3D_CUDA_TRY(ctx, cudaGetLastError());
+  liop::Slots S{};
+  S.img[0] = d_img, S.w[0] = (int)width, S.h[0] = (int)height, S.first[1] = n, S.n = 1;
+  int rc = liop::describe(ctx, w.stream, S, d_M, n, d_T, d_desc);
+  if (rc) return rc;
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(desc_out, d_desc, (size_t)n * liop::kDim * 4, cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
   return R3D_OK;
@@ -327,8 +351,10 @@ extern "C" int r3d_debug_liop_process(r3d_ctx* ctx, const float* patches, uint32
   if (!d_p || !d_desc || !d_T) return fail(ctx, R3D_ERR_NOMEM, "r3d_debug_liop_process: device allocation failed");
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_p, patches, (size_t)n * liop::kPix * 4, cudaMemcpyHostToDevice, w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_T, &T, sizeof(liop::Tables), cudaMemcpyHostToDevice, w.stream));
-  liop::k_liop<<<n, liop::kThreads, 0, w.stream>>>(d_p, liop::kSide, liop::kSide, nullptr, n, d_T, d_desc);
-  R3D_CUDA_TRY(ctx, cudaGetLastError());
+  liop::Slots S{};
+  S.img[0] = d_p, S.w[0] = liop::kSide, S.h[0] = liop::kSide, S.first[1] = n, S.n = 1;
+  int rc = liop::describe(ctx, w.stream, S, nullptr, n, d_T, d_desc);
+  if (rc) return rc;
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(desc_out, d_desc, (size_t)n * liop::kDim * 4, cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
   return R3D_OK;

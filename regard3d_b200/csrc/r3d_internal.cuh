@@ -175,6 +175,7 @@ struct r3d_ctx {
   r3d_relpose_timing relpose_timing{};
   r3d_resection_timing resection_timing{};
   r3d_akaze_timing akaze_timing{};
+  r3d_extract_timing extract_timing{};
   int host_threads = 0;
   // optional NCCL communicator (comm.cu): only the bundle adjustment exchanges data between ranks
   void* nccl_comm = nullptr;
@@ -361,6 +362,28 @@ void build_view_ranks(const float* xy, uint32_t n, std::vector<uint32_t>& yrank,
                       uint32_t* n_slots);
 void post_process_pairs(int lanes, r3d_indmatch* const* ms, size_t* counts, const float* const* xyIs, const float* const* xyJs,
                         bool coord_dedup, const ViewRankRef* ranks);
+
+// r3d_save_features without the argument checks (features_io.cpp): nullptr, or the path that could not be written
+const char* save_features(const char* feat_path, const char* desc_path, const float* xyso, const float* desc, uint64_t n,
+                          uint32_t dim);
+
+// LIOP-144 (liop.cu), shared by r3d_liop_describe and r3d_extract_features (akaze.cu)
+namespace liop {
+constexpr int kDim = 144, kMaxSlots = 16;
+struct Tables;
+struct Slots {  // by value: keypoints first[s] .. first[s + 1] - 1 sample image s (img[s], w[s] x h[s], row-major)
+  const float* img[kMaxSlots];
+  int w[kMaxSlots], h[kMaxSlots];
+  uint32_t first[kMaxSlots + 1];
+  int n;
+};
+// the inverse affine map of one keypoint (host, libm cos / sin): 6 floats
+void affine_of(float x, float y, float kp_size, float kp_angle, float factor, float* M);
+// the sampling tables in a pool block of w, uploaded on st; nullptr on failure
+Tables* tables_to_device(DeviceWorker& w, cudaStream_t st);
+// k_liop on st: one CTA per keypoint, d_M n x 6, d_desc n x kDim
+int describe(r3d_ctx* ctx, cudaStream_t st, const Slots& S, const float* d_M, uint32_t n, const Tables* d_T, float* d_desc);
+}  // namespace liop
 
 // driver entry points
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
