@@ -1,7 +1,7 @@
 // lm_trust_region.cuh -- the trust-region policy of Ceres' Levenberg-Marquardt, shared by the library's least-squares
-// solvers: bundle adjustment (ba.cu), rotation and translation averaging (rotavg.cu, transavg.cu) drive it from the
-// host, the two-view bundle adjustment (relpose.cu, k_relpose_ba) and the pose refinement (resection.cu,
-// k_resect_refine) from every thread of a CTA.  Policy only: it launches nothing, synchronises nothing and reads no
+// solvers: bundle adjustment (ba.cu) and rotation and translation averaging (averaging.cuh's averaging_lm, for
+// rotavg.cu and transavg.cu) drive it from the host, the two-view bundle adjustment (relpose.cu, k_relpose_ba) and the
+// pose refinement (resection.cu, k_resect_refine) from every thread of a CTA.  Policy only: it launches nothing, synchronises nothing and reads no
 // memory; the callers keep their evaluations, linear solves and data movement.  The CPU restatements under oracle/ keep
 // their own copies of these rules on purpose: they are the independent references the solvers are tested against.
 //

@@ -15,9 +15,10 @@
 //      (ba.cu), block inverse iteration with 3 right-hand sides (k_rotavg_trsm3: blocked forward / backward
 //      substitution, one cooperative launch) and a 3 x 3 Cholesky-QR (k_rotavg_orth), then the sign, the SO(3)
 //      projection of every 3 x 3 block (relpose_math.cuh's Jacobi SVD) and the gauge (k_rotavg_project).
-//   4. refinement: Levenberg-Marquardt (lm_trust_region.cuh's trust region) on the angle-axis of every kept view,
-//      residual log(R_ij^T R_j R_i^T) with forward-mode duals, dense normal equations by one owner per block row (no
-//      floating-point atomics), k_chol_fused, fixed-order reductions: repeated calls are bit-identical.
+//   4. refinement: Levenberg-Marquardt (averaging.cuh's loop around lm_trust_region.cuh's trust region) on the
+//      angle-axis of every kept view: k_rotavg_eval (residual log(R_ij^T R_j R_i^T) with forward-mode duals),
+//      k_rotavg_system (dense normal equations by one owner per block row, no floating-point atomics), k_chol_fused,
+//      fixed-order reductions: repeated calls are bit-identical.
 #include "r3d_internal.cuh"
 #include "averaging.cuh"
 #include "ba_model.cuh"
@@ -326,42 +327,6 @@ __global__ void __launch_bounds__(kOThreads) k_rotavg_project(const double* __re
 }
 
 // ---- 4. refinement ----------------------------------------------------------------------------------------------
-// forward-mode dual with the 6 partials of (angle-axis of the edge's first view, angle-axis of its second view)
-struct Dual {
-  double a;
-  double v[6];
-};
-__device__ __forceinline__ Dual dconst(double x) { Dual r; r.a = x; for (int i = 0; i < 6; ++i) r.v[i] = 0.0; return r; }
-__device__ __forceinline__ Dual operator+(const Dual& x, const Dual& y) { Dual r; r.a = x.a + y.a; for (int i = 0; i < 6; ++i) r.v[i] = x.v[i] + y.v[i]; return r; }
-__device__ __forceinline__ Dual operator-(const Dual& x, const Dual& y) { Dual r; r.a = x.a - y.a; for (int i = 0; i < 6; ++i) r.v[i] = x.v[i] - y.v[i]; return r; }
-__device__ __forceinline__ Dual operator-(const Dual& x) { Dual r; r.a = -x.a; for (int i = 0; i < 6; ++i) r.v[i] = -x.v[i]; return r; }
-__device__ __forceinline__ Dual operator*(const Dual& x, const Dual& y) { Dual r; r.a = x.a * y.a; for (int i = 0; i < 6; ++i) r.v[i] = x.a * y.v[i] + x.v[i] * y.a; return r; }
-__device__ __forceinline__ Dual operator/(const Dual& x, const Dual& y) {
-  Dual r; const double inv = 1.0 / y.a; r.a = x.a * inv;
-  for (int i = 0; i < 6; ++i) r.v[i] = (x.v[i] - r.a * y.v[i]) * inv;
-  return r;
-}
-__device__ __forceinline__ Dual operator+(const Dual& x, double s) { Dual r = x; r.a += s; return r; }
-__device__ __forceinline__ Dual operator-(double s, const Dual& x) { Dual r = -x; r.a += s; return r; }
-__device__ __forceinline__ Dual operator*(double s, const Dual& x) { Dual r; r.a = x.a * s; for (int i = 0; i < 6; ++i) r.v[i] = x.v[i] * s; return r; }
-__device__ __forceinline__ Dual sqrt(const Dual& x) { Dual r; r.a = ::sqrt(x.a); const double d = 0.5 / r.a; for (int i = 0; i < 6; ++i) r.v[i] = x.v[i] * d; return r; }
-__device__ __forceinline__ Dual sin(const Dual& x) { Dual r; r.a = ::sin(x.a); const double c = ::cos(x.a); for (int i = 0; i < 6; ++i) r.v[i] = c * x.v[i]; return r; }
-__device__ __forceinline__ Dual cos(const Dual& x) { Dual r; r.a = ::cos(x.a); const double s = -::sin(x.a); for (int i = 0; i < 6; ++i) r.v[i] = s * x.v[i]; return r; }
-__device__ __forceinline__ Dual atan2(const Dual& y, const Dual& x) {
-  Dual r; r.a = ::atan2(y.a, x.a); const double d = 1.0 / (x.a * x.a + y.a * y.a);
-  for (int i = 0; i < 6; ++i) r.v[i] = (x.a * y.v[i] - y.a * x.v[i]) * d;
-  return r;
-}
-__device__ __forceinline__ double sqrt(double x) { return ::sqrt(x); }
-__device__ __forceinline__ double sin(double x) { return ::sin(x); }
-__device__ __forceinline__ double cos(double x) { return ::cos(x); }
-__device__ __forceinline__ double atan2(double y, double x) { return ::atan2(y, x); }
-__device__ __forceinline__ double val(const Dual& x) { return x.a; }
-__device__ __forceinline__ double val(double x) { return x; }
-template <class T> __device__ __forceinline__ T mk(double x);
-template <> __device__ __forceinline__ double mk<double>(double x) { return x; }
-template <> __device__ __forceinline__ Dual mk<Dual>(double x) { return dconst(x); }
-
 // ceres::AngleAxisToRotationMatrix (row-major)
 template <class T>
 __device__ void aa_to_R(const T* aa, T* R) {
@@ -432,11 +397,11 @@ __global__ void k_rotavg_eval(const double* __restrict__ aa, const uint2* __rest
   const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
   if (e >= ne) return;
   const uint2 v = ab[e];
-  Dual xa[3], xb[3], r[3];
+  Dual<6> xa[3], xb[3], r[3];
   for (int k = 0; k < 3; ++k) {
-    xa[k] = dconst(aa[3 * (size_t)v.x + k]);
+    xa[k] = dconst<6>(aa[3 * (size_t)v.x + k]);
     xa[k].v[k] = 1.0;
-    xb[k] = dconst(aa[3 * (size_t)v.y + k]);
+    xb[k] = dconst<6>(aa[3 * (size_t)v.y + k]);
     xb[k].v[3 + k] = 1.0;
   }
   edge_residual(xa, xb, Rk + 9 * (size_t)e, r);
@@ -461,62 +426,23 @@ __global__ void k_rotavg_cost(const double* __restrict__ aa, const uint2* __rest
   cost[e] = 0.5 * ba::huber_rho(r[0] * r[0] + r[1] * r[1] + r[2] * r[2], huber_a, &rho1);
 }
 
-// out[0] = sum of v[0..n) (fixed order)
-__global__ void __launch_bounds__(kOThreads) k_rotavg_sum(const double* __restrict__ v, uint32_t n, double* __restrict__ out) {
-  __shared__ double red[kOThreads / 32];
-  double s = 0.0;
-  for (uint32_t i = threadIdx.x; i < n; i += kOThreads) s += v[i];
-  s = block_sum_fixed<kOThreads>(s, red);
-  if (threadIdx.x == 0) out[0] = s;
-}
-
-// Owner per view a (one CTA), its incident edges in neighbour order.  mode 0: the Jacobi scale 1 / (1 + ||column||)
-// of its 3 columns; mode 1: gradient g = J^T r and diag(J^T J) (scaled); mode 2: its block row of J^T J + D^2
-// (scaled) into the zeroed (N + 1) x N system and -g into the right-hand-side row N.
-__global__ void __launch_bounds__(128) k_rotavg_normal(int mode, const uint32_t* __restrict__ inc_ofs, const uint32_t* __restrict__ inc_nbr,
+// Owner per view a (one CTA), its incident edges in neighbour order: its block row of J^T J + D^2 (scaled after the
+// block products) into the zeroed (N + 1) x N system and -g into the right-hand-side row N.  Off-diagonal blocks first,
+// one per incident edge.
+__global__ void __launch_bounds__(128) k_rotavg_system(const uint32_t* __restrict__ inc_ofs, const uint32_t* __restrict__ inc_nbr,
                                                        const uint32_t* __restrict__ inc_edge, const uint2* __restrict__ ab,
-                                                       const double* __restrict__ res, const double* __restrict__ jac, uint32_t m,
-                                                       double* __restrict__ scale, double* __restrict__ g, double* __restrict__ diag,
-                                                       double inv_radius, double* __restrict__ A) {
+                                                       const double* __restrict__ jac, uint32_t m, double* __restrict__ scale,
+                                                       double* __restrict__ g, double* __restrict__ diag, double inv_radius,
+                                                       double* __restrict__ A) {
   const uint32_t a = blockIdx.x, tid = threadIdx.x;
   const uint32_t N = 3 * m;
   const uint32_t b0 = inc_ofs[a], b1 = inc_ofs[a + 1];
   auto col = [&](uint32_t e, uint32_t v) -> int { return ab[e].x == v ? 0 : 3; };
-  if (mode == 0) {
-    if (tid < 3) {
-      double n2 = 0.0;
-      for (uint32_t p = b0; p < b1; ++p) {
-        const uint32_t e = inc_edge[p];
-        const int o = col(e, a) + (int)tid;
-        for (int i = 0; i < 3; ++i) n2 += jac[18 * (size_t)e + 6 * i + o] * jac[18 * (size_t)e + 6 * i + o];
-      }
-      scale[3 * a + tid] = 1.0 / (1.0 + ::sqrt(n2));
-    }
-    return;
-  }
-  if (mode == 1) {
-    if (tid < 6) {
-      const int k = (int)tid % 3;
-      const double sk = scale[3 * a + k];
-      double s = 0.0;
-      for (uint32_t p = b0; p < b1; ++p) {
-        const uint32_t e = inc_edge[p];
-        const int o = col(e, a) + k;
-        for (int i = 0; i < 3; ++i) {
-          const double j = jac[18 * (size_t)e + 6 * i + o] * sk;
-          s += tid < 3 ? j * res[3 * (size_t)e + i] : j * j;
-        }
-      }
-      if (tid < 3) g[3 * a + k] = s;
-      else diag[3 * a + k] = s;
-    }
-    return;
-  }
-  // mode 2: off-diagonal blocks, one per incident edge
   for (uint32_t p = b0 + tid; p < b1; p += blockDim.x) {
     const uint32_t e = inc_edge[p], b = inc_nbr[p];
     const int oa = col(e, a), ob = 3 - oa;
     const double* J = jac + 18 * (size_t)e;
+#pragma unroll 1  // rolled: 56 registers, 64 unrolled
     for (int k = 0; k < 3; ++k)
       for (int l = 0; l < 3; ++l) {
         const double s = J[oa + k] * J[ob + l] + J[6 + oa + k] * J[6 + ob + l] + J[12 + oa + k] * J[12 + ob + l];
@@ -628,6 +554,19 @@ int largest_biedge_component(uint32_t n, const std::vector<uint32_t>& eu, const 
   for (size_t c = 0; c < size.size(); ++c)  // components are numbered by their smallest node
     if (size[c] >= 2 && (best < 0 || size[c] > size[(size_t)best])) best = (int)c;
   return best;
+}
+
+void incidence_lists(uint32_t m, const std::vector<uint2>& edges, std::vector<uint32_t>& ofs, std::vector<uint32_t>& nbr,
+                     std::vector<uint32_t>& edge) {
+  const uint32_t ne = (uint32_t)edges.size();
+  ofs.assign(m + 1, 0);
+  nbr.resize(2 * (size_t)ne);
+  edge.resize(2 * (size_t)ne);
+  for (const uint2& e : edges) { ofs[e.x + 1]++; ofs[e.y + 1]++; }
+  for (uint32_t a = 0; a < m; ++a) ofs[a + 1] += ofs[a];
+  std::vector<uint32_t> pos(ofs.begin(), ofs.end() - 1);
+  for (uint32_t e = 0; e < ne; ++e) { nbr[pos[edges[e].y]] = edges[e].x; edge[pos[edges[e].y]++] = e; }
+  for (uint32_t e = 0; e < ne; ++e) { nbr[pos[edges[e].x]] = edges[e].y; edge[pos[edges[e].x]++] = e; }
 }
 
 // the deterministic start of the inverse iteration (the oracle draws the same numbers)
@@ -756,16 +695,8 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
   S.n_kept_views = m;
   S.n_kept_edges = ne;
   for (uint32_t v : kview) view_kept[v] = 1;
-  // incidence lists in neighbour order
-  std::vector<uint32_t> inc_ofs(m + 1, 0), inc_nbr(2 * (size_t)ne), inc_edge(2 * (size_t)ne);
-  for (const uint2& e : kab) { inc_ofs[e.x + 1]++; inc_ofs[e.y + 1]++; }
-  for (uint32_t a = 0; a < m; ++a) inc_ofs[a + 1] += inc_ofs[a];
-  {
-    std::vector<uint32_t> pos(inc_ofs.begin(), inc_ofs.end() - 1);
-    // edges sorted by (a, b): for view v the entries (b < v) arrive in b order first, then (v, b > v) in b order
-    for (uint32_t e = 0; e < ne; ++e) { inc_nbr[pos[kab[e].y]] = kab[e].x; inc_edge[pos[kab[e].y]++] = e; }
-    for (uint32_t e = 0; e < ne; ++e) { inc_nbr[pos[kab[e].x]] = kab[e].y; inc_edge[pos[kab[e].x]++] = e; }
-  }
+  std::vector<uint32_t> inc_ofs, inc_nbr, inc_edge;
+  incidence_lists(m, kab, inc_ofs, inc_nbr, inc_edge);
   uint32_t max_deg = 0;
   for (uint32_t a = 0; a < m; ++a) max_deg = std::max(max_deg, inc_ofs[a + 1] - inc_ofs[a]);
   // ---- 3. L2 initialisation ----
@@ -840,77 +771,19 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
     const uint32_t eg = (ne + 127) / 128;
     double* cur = d_aa.p;
     double* trial = d_aan.p;
-    auto eval_cost = [&](const double* x, double* out) -> int {
-      k_rotavg_cost<<<eg, 128, 0, w.stream>>>(x, d_ab.p, d_R.p, ne, ha, d_cost.p);
-      k_rotavg_sum<<<1, kOThreads, 0, w.stream>>>(d_cost.p, ne, d_scal.p + 4);
-      R3D_CUDA_TRY(ctx, cudaGetLastError());
-      int r2;
-      if ((r2 = read_scal())) return r2;
-      *out = scal[4];
-      return R3D_OK;
-    };
-    bool have_scale = false;
-    double gmax = 0.0;
-    auto evaluate = [&]() -> int {  // residuals, Jacobians, the scale on the first call, g, diag and max |g / scale|
-      k_rotavg_eval<<<eg, 128, 0, w.stream>>>(cur, d_ab.p, d_R.p, ne, ha, d_res.p, d_jac.p);
-      if (!have_scale) {
-        k_rotavg_normal<<<m, 128, 0, w.stream>>>(0, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_res.p, d_jac.p, m, d_scale.p, d_g.p, d_diag.p, 0.0,
-                                                 nullptr);
-        have_scale = true;
-      }
-      k_rotavg_normal<<<m, 128, 0, w.stream>>>(1, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_res.p, d_jac.p, m, d_scale.p, d_g.p, d_diag.p, 0.0,
-                                               nullptr);
-      // the step kernel with a zero step and radius reports max |g / scale| in scal[3]
-      R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_x.p, 0, N * sizeof(double), w.stream));
-      k_avg_step<kOThreads><<<1, kOThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, (uint32_t)N, (uint32_t)N, 0.0, trial,
-                                                           d_scal.p);
-      R3D_CUDA_TRY(ctx, cudaGetLastError());
-      int r2;
-      if ((r2 = read_scal())) return r2;
-      gmax = scal[3];
-      return R3D_OK;
-    };
-    double cost = 0.0;
-    if ((rc = eval_cost(cur, &cost))) return rc;
-    S.lm_initial_cost = cost;
-    S.lm_iterations = 0;
-    S.lm_successful_steps = 0;
-    S.lm_termination = 0;
-    LmTrustRegion lm(lm_params(opt.lm));
-    if ((rc = evaluate())) return rc;
-    const bool stop = lm.start(gmax);
-    for (uint32_t iter = 1; !stop && iter <= lm.p.max_iterations; ++iter) {
-      lm.iterations = iter;
-      const double inv_radius = 1.0 / lm.radius;
-      R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_A.p, 0, (size_t)(N + 1) * N * sizeof(double), w.stream));
-      R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_scal.p + 7, 0, sizeof(double), w.stream));
-      k_rotavg_normal<<<m, 128, 0, w.stream>>>(2, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_res.p, d_jac.p, m, d_scale.p, d_g.p, d_diag.p,
-                                               inv_radius, d_A.p);
-      R3D_CUDA_TRY(ctx, cudaGetLastError());
-      if ((rc = dense_cholesky(ctx, w, d_A.p, d_L.p, d_Linv.p, N, d_scal.p + 7, d_x.p))) return rc;
-      k_avg_step<kOThreads><<<1, kOThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, (uint32_t)N, (uint32_t)N, inv_radius,
-                                                           trial, d_scal.p);
-      R3D_CUDA_TRY(ctx, cudaGetLastError());
-      if ((rc = read_scal())) return rc;
-      const double model_cost_change = scal[0];
-      bool accepted = false;
-      if (lm.step_usable(scal[7] == 0.0, model_cost_change)) {
-        if (lm.step_too_small(scal[1], scal[2])) break;
-        double new_cost = 0.0;
-        if ((rc = eval_cost(trial, &new_cost))) return rc;
-        if ((accepted = lm.accept(cost, new_cost, model_cost_change))) {
-          std::swap(cur, trial);
-          cost = new_cost;
-          if ((rc = evaluate())) return rc;
-          if (lm.converged(gmax)) break;
-        }
-      }
-      if (!accepted && lm.reject()) break;
-    }
-    S.lm_iterations = lm.iterations;
-    S.lm_successful_steps = lm.successful;
-    S.lm_termination = lm.termination;
-    S.lm_final_cost = cost;
+    const AvgBuffers B{d_iofs.p, d_iedge.p, d_ab.p, d_res.p, d_jac.p, d_cost.p, d_scale.p, d_g.p, d_diag.p,
+                       d_A.p, d_L.p, d_Linv.p, d_x.p, d_scal.p};
+    rc = averaging_lm<18>(
+        ctx, w, lm_params(opt.lm), B, ne, 0, (uint32_t)N, (uint32_t)N, cur, trial, S,
+        [&](const double* x) { k_rotavg_cost<<<eg, 128, 0, w.stream>>>(x, d_ab.p, d_R.p, ne, ha, d_cost.p); },
+        [&](const double* x) { k_rotavg_eval<<<eg, 128, 0, w.stream>>>(x, d_ab.p, d_R.p, ne, ha, d_res.p, d_jac.p); },
+        [](int) {},
+        [&](const double*, double inv_radius) {
+          k_rotavg_system<<<m, 128, 0, w.stream>>>(d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_jac.p, m, d_scale.p, d_g.p, d_diag.p,
+                                                   inv_radius, d_A.p);
+        },
+        [](const double*, double) {});
+    if (rc) return rc;
     R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[5], w.stream));
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(aa.data(), cur, N * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
     R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));

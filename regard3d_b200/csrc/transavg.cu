@@ -6,12 +6,12 @@
 // Replaces GlobalSfM_Translation_AveragingSolver::Translation_averaging (OpenMVG 1.4, SURVEY.md A.11) for
 // TRANSLATION_AVERAGING_L2_DISTANCE_CHORDAL and TRANSLATION_AVERAGING_SOFTL1, on the pairwise relative translations:
 //   1. host: the usable edges, the largest bi-edge-connected component (rotavg.cu's Tarjan), reindexing by view id.
-//   2. Levenberg-Marquardt (lm_trust_region.cuh's trust region), the lowest kept view held:
-//      k_ta_eval (one thread per edge, forward-mode duals: residual, 3 x 7 Jacobian, soft-L1 corrector),
-//      k_ta_view (one owner CTA per view block row: Jacobi scale, gradient, J^T J + D^2 with each edge's scale
-//      eliminated in the same pass -- no floating-point atomics), k_chol_fused (ba.cu) on the 3(m-1) reduced system,
-//      k_ta_back (the scale steps; a scale on its bound pushed outwards is held), k_avg_step (averaging.cuh; clamp
-//      s >= 1, model cost change, norms, projected gradient; fixed-order reductions).  Repeated calls are bit-identical.
+//   2. Levenberg-Marquardt (averaging.cuh's loop around lm_trust_region.cuh's trust region), the lowest kept view held:
+//      k_ta_eval (one thread per edge, forward-mode duals: residual, 3 x 7 Jacobian, soft-L1 corrector), k_ta_edge
+//      (the scale columns' Jacobi scale and gradient), k_ta_system (one owner CTA per view block row: J^T J + D^2 with
+//      each edge's scale eliminated in the same pass -- no floating-point atomics), k_chol_fused (ba.cu) on the 3(m-1)
+//      reduced system, k_ta_back (the scale steps; a scale on its bound pushed outwards is held); the step clamps
+//      s >= 1.  Fixed-order reductions: repeated calls are bit-identical.
 #include "r3d_internal.cuh"
 #include "averaging.cuh"
 #include "relpose_math.cuh"
@@ -25,26 +25,10 @@ namespace ta {
 
 constexpr int kChordal = 2;  // R3D_TRANSAVG_L2_CHORDAL
 constexpr int kSoftL1 = 3;   // R3D_TRANSAVG_SOFTL1
-constexpr int kRThreads = 256;
 
 // forward-mode dual: partials of (first view's 3 coordinates, second view's 3, the edge's scale)
-struct Dual {
-  double a;
-  double v[7];
-};
-__device__ __forceinline__ Dual dconst(double x) { Dual r; r.a = x; for (int i = 0; i < 7; ++i) r.v[i] = 0.0; return r; }
-__device__ __forceinline__ Dual operator+(const Dual& x, const Dual& y) { Dual r; r.a = x.a + y.a; for (int i = 0; i < 7; ++i) r.v[i] = x.v[i] + y.v[i]; return r; }
-__device__ __forceinline__ Dual operator-(const Dual& x, const Dual& y) { Dual r; r.a = x.a - y.a; for (int i = 0; i < 7; ++i) r.v[i] = x.v[i] - y.v[i]; return r; }
-__device__ __forceinline__ Dual operator*(const Dual& x, const Dual& y) { Dual r; r.a = x.a * y.a; for (int i = 0; i < 7; ++i) r.v[i] = x.a * y.v[i] + x.v[i] * y.a; return r; }
-__device__ __forceinline__ Dual operator/(const Dual& x, const Dual& y) {
-  Dual r; const double inv = 1.0 / y.a; r.a = x.a * inv;
-  for (int i = 0; i < 7; ++i) r.v[i] = (x.v[i] - r.a * y.v[i]) * inv;
-  return r;
-}
-__device__ __forceinline__ Dual operator-(const Dual& x, double s) { Dual r = x; r.a -= s; return r; }
-__device__ __forceinline__ Dual operator*(const Dual& x, double s) { Dual r; r.a = x.a * s; for (int i = 0; i < 7; ++i) r.v[i] = x.v[i] * s; return r; }
-__device__ __forceinline__ Dual sqrt(const Dual& x) { Dual r; r.a = ::sqrt(x.a); const double d = 0.5 / r.a; for (int i = 0; i < 7; ++i) r.v[i] = x.v[i] * d; return r; }
-__device__ __forceinline__ double sqrt(double x) { return ::sqrt(x); }
+using Dual = ra::Dual<7>;
+using ra::sqrt;
 
 // ChordFunctor (1DSfM): r = (x_J - x_I) / |x_J - x_I| - u, u = -R_J^T t_IJ / |t_IJ|
 template <class T>
@@ -97,16 +81,16 @@ __global__ void k_ta_eval(const double* __restrict__ x, const uint2* __restrict_
   const uint2 v = ab[e];
   Dual xi[3], xj[3], r[3];
   for (int k = 0; k < 3; ++k) {
-    xi[k] = dconst(view_coord(x, v.x, k));
+    xi[k] = ra::dconst<7>(view_coord(x, v.x, k));
     xi[k].v[k] = 1.0;
-    xj[k] = dconst(view_coord(x, v.y, k));
+    xj[k] = ra::dconst<7>(view_coord(x, v.y, k));
     xj[k].v[3 + k] = 1.0;
   }
   double sq = 1.0;
   if (M == kChordal) {
     chordal_residual(xi, xj, ed + 6 * (size_t)e, r);
   } else {
-    Dual s = dconst(x[N + e]);
+    Dual s = ra::dconst<7>(x[N + e]);
     s.v[6] = 1.0;
     softl1_residual(xi, xj, s, ed + 6 * (size_t)e, r);
     double rho1;
@@ -139,14 +123,6 @@ __global__ void k_ta_cost(const double* __restrict__ x, const uint2* __restrict_
     double rho1;
     cost[e] = 0.5 * softl1_rho(r[0] * r[0] + r[1] * r[1] + r[2] * r[2], loss_a, &rho1);
   }
-}
-
-__global__ void __launch_bounds__(kRThreads) k_ta_sum(const double* __restrict__ v, uint32_t n, double* __restrict__ out) {
-  __shared__ double red[kRThreads / 32];
-  double s = 0.0;
-  for (uint32_t i = threadIdx.x; i < n; i += kRThreads) s += v[i];
-  s = block_sum_fixed<kRThreads>(s, red);
-  if (threadIdx.x == 0) out[0] = s;
 }
 
 // the scale column of edge e: mode 0 its Jacobi scale; mode 1 its gradient and diag(J^T J) (scaled)
@@ -199,51 +175,19 @@ __device__ __forceinline__ void edge_blocks(const double* J, const double* scale
   }
 }
 
-// Owner per free view a = blockIdx.x + 1 (reduced block row a - 1), its incident edges in neighbour order.  mode 0: the
-// Jacobi scale 1 / (1 + ||column||) of its 3 columns; mode 1: gradient g = J^T r and diag(J^T J) (scaled); mode 2: its
-// block row of the reduced system (J^T J + D^2 with every free scale eliminated) into the zeroed (N + 1) x N matrix and the
-// reduced right-hand side into row N.  The held view 0 has no row or column.
-__global__ void __launch_bounds__(128) k_ta_view(int mode, int softl1, const uint32_t* __restrict__ inc_ofs,
-                                                 const uint32_t* __restrict__ inc_nbr, const uint32_t* __restrict__ inc_edge,
-                                                 const uint2* __restrict__ ab, const double* __restrict__ res,
-                                                 const double* __restrict__ jac, const double* __restrict__ x, uint32_t N,
-                                                 double* __restrict__ scale, double* __restrict__ g, double* __restrict__ diag,
-                                                 double inv_radius, double* __restrict__ A) {
+// Owner per free view a = blockIdx.x + 1 (reduced block row a - 1), its incident edges in neighbour order: its block row
+// of the reduced system (J^T J + D^2, scaled before the block products, with every free scale eliminated) into the zeroed
+// (N + 1) x N matrix and the reduced right-hand side into row N.  The held view 0 has no row or column.  Off-diagonal
+// blocks first, one per incident edge to a free view.
+__global__ void __launch_bounds__(128) k_ta_system(int softl1, const uint32_t* __restrict__ inc_ofs, const uint32_t* __restrict__ inc_nbr,
+                                                   const uint32_t* __restrict__ inc_edge, const uint2* __restrict__ ab,
+                                                   const double* __restrict__ jac, const double* __restrict__ x, uint32_t N,
+                                                   const double* __restrict__ scale, const double* __restrict__ g,
+                                                   const double* __restrict__ diag, double inv_radius, double* __restrict__ A) {
   const uint32_t a = blockIdx.x + 1, tid = threadIdx.x;
   const uint32_t ra_ = 3 * (a - 1);
   const uint32_t b0 = inc_ofs[a], b1 = inc_ofs[a + 1];
   auto col = [&](uint32_t e) -> int { return ab[e].x == a ? 0 : 3; };
-  if (mode == 0) {
-    if (tid < 3) {
-      double n2 = 0.0;
-      for (uint32_t p = b0; p < b1; ++p) {
-        const uint32_t e = inc_edge[p];
-        const int o = col(e) + (int)tid;
-        for (int i = 0; i < 3; ++i) n2 += jac[21 * (size_t)e + 7 * i + o] * jac[21 * (size_t)e + 7 * i + o];
-      }
-      scale[ra_ + tid] = 1.0 / (1.0 + ::sqrt(n2));
-    }
-    return;
-  }
-  if (mode == 1) {
-    if (tid < 6) {
-      const int k = (int)tid % 3;
-      const double sk = scale[ra_ + k];
-      double s = 0.0;
-      for (uint32_t p = b0; p < b1; ++p) {
-        const uint32_t e = inc_edge[p];
-        const int o = col(e) + k;
-        for (int i = 0; i < 3; ++i) {
-          const double j = jac[21 * (size_t)e + 7 * i + o] * sk;
-          s += tid < 3 ? j * res[3 * (size_t)e + i] : j * j;
-        }
-      }
-      if (tid < 3) g[ra_ + k] = s;
-      else diag[ra_ + k] = s;
-    }
-    return;
-  }
-  // mode 2: off-diagonal blocks, one per incident edge to a free view
   for (uint32_t p = b0 + tid; p < b1; p += blockDim.x) {
     const uint32_t e = inc_edge[p], b = inc_nbr[p];
     if (b == 0) continue;
@@ -394,16 +338,8 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
   S.n_kept_views = m;
   S.n_kept_edges = ne;
   for (uint32_t v : kview) view_kept[v] = 1;
-  // incidence lists in neighbour order (edges are sorted by (lo, hi): for view v the entries (lo < v) arrive in lo order
-  // first, then (v, hi > v) in hi order)
-  std::vector<uint32_t> inc_ofs(m + 1, 0), inc_nbr(2 * (size_t)ne), inc_edge(2 * (size_t)ne);
-  for (const uint2& e : kab) { inc_ofs[e.x + 1]++; inc_ofs[e.y + 1]++; }
-  for (uint32_t a = 0; a < m; ++a) inc_ofs[a + 1] += inc_ofs[a];
-  {
-    std::vector<uint32_t> pos(inc_ofs.begin(), inc_ofs.end() - 1);
-    for (uint32_t e = 0; e < ne; ++e) { inc_nbr[pos[kab[e].y]] = kab[e].x; inc_edge[pos[kab[e].y]++] = e; }
-    for (uint32_t e = 0; e < ne; ++e) { inc_nbr[pos[kab[e].x]] = kab[e].y; inc_edge[pos[kab[e].x]++] = e; }
-  }
+  std::vector<uint32_t> inc_ofs, inc_nbr, inc_edge;
+  ra::incidence_lists(m, kab, inc_ofs, inc_nbr, inc_edge);
   // ---- 2. Levenberg-Marquardt ----
   const int N = 3 * ((int)m - 1);            // free view coordinates (view 0 held)
   const uint32_t ns = softl1 ? ne : 0u;      // scales
@@ -431,12 +367,6 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
   Events<2> evt;
   R3D_CUDA_TRY(ctx, evt.create());
   R3D_CUDA_TRY(ctx, cudaEventRecord(evt.e[0], w.stream));
-  double scal[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-  auto read_scal = [&]() -> int {
-    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(scal, d_scal.p, sizeof(scal), cudaMemcpyDeviceToHost, w.stream));
-    R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-    return R3D_OK;
-  };
   LmParams prm = lm_params(opt.lm);
   if (prm.max_iterations == 0) prm.max_iterations = softl1 ? std::max<uint32_t>(50, 2 * ne) : 500u;
   if (!(prm.function_tolerance > 0.0)) prm.function_tolerance = softl1 ? 1e-6 : 1e-7;
@@ -444,80 +374,29 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
   const uint32_t eg = (ne + 127) / 128;
   double* cur = d_cur.p;
   double* trial = d_trial.p;
-  auto eval_cost = [&](const double* xx, double* out) -> int {
-    if (softl1) k_ta_cost<kSoftL1><<<eg, 128, 0, w.stream>>>(xx, d_ab.p, d_ed.p, ne, (uint32_t)N, la, d_cost.p);
-    else k_ta_cost<kChordal><<<eg, 128, 0, w.stream>>>(xx, d_ab.p, d_ed.p, ne, (uint32_t)N, la, d_cost.p);
-    k_ta_sum<<<1, kRThreads, 0, w.stream>>>(d_cost.p, ne, d_scal.p + 4);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    int r2;
-    if ((r2 = read_scal())) return r2;
-    *out = scal[4];
-    return R3D_OK;
-  };
-  bool have_scale = false;
-  double gmax = 0.0;
-  auto evaluate = [&]() -> int {  // residuals, Jacobians, the scale on the first call, g, diag and the projected gradient
-    if (softl1) k_ta_eval<kSoftL1><<<eg, 128, 0, w.stream>>>(cur, d_ab.p, d_ed.p, ne, (uint32_t)N, la, d_res.p, d_jac.p);
-    else k_ta_eval<kChordal><<<eg, 128, 0, w.stream>>>(cur, d_ab.p, d_ed.p, ne, (uint32_t)N, la, d_res.p, d_jac.p);
-    if (!have_scale) {
-      k_ta_view<<<m - 1, 128, 0, w.stream>>>(0, softl1, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_res.p, d_jac.p, cur, (uint32_t)N, d_scale.p,
-                                              d_g.p, d_diag.p, 0.0, nullptr);
-      if (softl1) k_ta_edge<<<eg, 128, 0, w.stream>>>(0, d_res.p, d_jac.p, ne, (uint32_t)N, d_scale.p, d_g.p, d_diag.p);
-      have_scale = true;
-    }
-    k_ta_view<<<m - 1, 128, 0, w.stream>>>(1, softl1, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_res.p, d_jac.p, cur, (uint32_t)N, d_scale.p,
-                                            d_g.p, d_diag.p, 0.0, nullptr);
-    if (softl1) k_ta_edge<<<eg, 128, 0, w.stream>>>(1, d_res.p, d_jac.p, ne, (uint32_t)N, d_scale.p, d_g.p, d_diag.p);
-    // the step kernel with a zero step and radius reports the projected gradient in scal[3]
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_x.p, 0, Nv * sizeof(double), w.stream));
-    ra::k_avg_step<kRThreads><<<1, kRThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, Nv, (uint32_t)N, 0.0, trial,
-                                                            d_scal.p);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    int r2;
-    if ((r2 = read_scal())) return r2;
-    gmax = scal[3];
-    return R3D_OK;
-  };
-  int rc;
-  double cost = 0.0;
-  if ((rc = eval_cost(cur, &cost))) return rc;
-  S.lm_initial_cost = cost;
-  LmTrustRegion lm(prm);
-  if ((rc = evaluate())) return rc;
-  const bool stop = lm.start(gmax);
-  for (uint32_t iter = 1; !stop && iter <= prm.max_iterations; ++iter) {
-    lm.iterations = iter;
-    const double inv_radius = 1.0 / lm.radius;
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_A.p, 0, (size_t)(N + 1) * N * sizeof(double), w.stream));
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_scal.p + 7, 0, sizeof(double), w.stream));
-    k_ta_view<<<m - 1, 128, 0, w.stream>>>(2, softl1, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_res.p, d_jac.p, cur, (uint32_t)N, d_scale.p,
-                                            d_g.p, d_diag.p, inv_radius, d_A.p);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    if ((rc = dense_cholesky(ctx, w, d_A.p, d_L.p, d_Linv.p, N, d_scal.p + 7, d_x.p))) return rc;
-    if (softl1) k_ta_back<<<eg, 128, 0, w.stream>>>(d_ab.p, d_jac.p, cur, d_scale.p, d_g.p, ne, (uint32_t)N, inv_radius, d_x.p);
-    ra::k_avg_step<kRThreads><<<1, kRThreads, 0, w.stream>>>(d_x.p, d_g.p, d_diag.p, d_scale.p, cur, Nv, (uint32_t)N, inv_radius, trial,
-                                                            d_scal.p);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    if ((rc = read_scal())) return rc;
-    const double model_cost_change = scal[0];
-    bool accepted = false;
-    if (lm.step_usable(scal[7] == 0.0, model_cost_change)) {
-      if (lm.step_too_small(scal[1], scal[2])) break;
-      double new_cost = 0.0;
-      if ((rc = eval_cost(trial, &new_cost))) return rc;
-      if ((accepted = lm.accept(cost, new_cost, model_cost_change))) {
-        std::swap(cur, trial);
-        cost = new_cost;
-        if ((rc = evaluate())) return rc;
-        if (lm.converged(gmax)) break;
-      }
-    }
-    if (!accepted && lm.reject()) break;
-  }
-  S.lm_iterations = lm.iterations;
-  S.lm_successful_steps = lm.successful;
-  S.lm_termination = lm.termination;
-  S.lm_final_cost = cost;
+  const ra::AvgBuffers B{d_iofs.p, d_iedge.p, d_ab.p, d_res.p, d_jac.p, d_cost.p, d_scale.p, d_g.p, d_diag.p,
+                         d_A.p, d_L.p, d_Linv.p, d_x.p, d_scal.p};
+  const int rc = ra::averaging_lm<21>(
+      ctx, w, prm, B, ne, 1, Nv, (uint32_t)N, cur, trial, S,
+      [&](const double* xx) {
+        if (softl1) k_ta_cost<kSoftL1><<<eg, 128, 0, w.stream>>>(xx, d_ab.p, d_ed.p, ne, (uint32_t)N, la, d_cost.p);
+        else k_ta_cost<kChordal><<<eg, 128, 0, w.stream>>>(xx, d_ab.p, d_ed.p, ne, (uint32_t)N, la, d_cost.p);
+      },
+      [&](const double* xx) {
+        if (softl1) k_ta_eval<kSoftL1><<<eg, 128, 0, w.stream>>>(xx, d_ab.p, d_ed.p, ne, (uint32_t)N, la, d_res.p, d_jac.p);
+        else k_ta_eval<kChordal><<<eg, 128, 0, w.stream>>>(xx, d_ab.p, d_ed.p, ne, (uint32_t)N, la, d_res.p, d_jac.p);
+      },
+      [&](int mode) {
+        if (softl1) k_ta_edge<<<eg, 128, 0, w.stream>>>(mode, d_res.p, d_jac.p, ne, (uint32_t)N, d_scale.p, d_g.p, d_diag.p);
+      },
+      [&](const double* xx, double inv_radius) {
+        k_ta_system<<<m - 1, 128, 0, w.stream>>>(softl1, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_jac.p, xx, (uint32_t)N, d_scale.p,
+                                                 d_g.p, d_diag.p, inv_radius, d_A.p);
+      },
+      [&](const double* xx, double inv_radius) {
+        if (softl1) k_ta_back<<<eg, 128, 0, w.stream>>>(d_ab.p, d_jac.p, xx, d_scale.p, d_g.p, ne, (uint32_t)N, inv_radius, d_x.p);
+      });
+  if (rc) return rc;
   R3D_CUDA_TRY(ctx, cudaEventRecord(evt.e[1], w.stream));
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(x.data(), cur, Nv * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
