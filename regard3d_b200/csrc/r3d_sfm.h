@@ -1,4 +1,4 @@
-// r3d_sfm.h -- openMVG::sfm::SfM_Data as the library holds it (shared by sfm_data_io.cpp and sfm_ba.cpp).
+// r3d_sfm.h -- openMVG::sfm::SfM_Data as the library holds it, and its flat form for the device code (sfm_scene.cpp).
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -35,40 +35,6 @@ struct r3d_sfm_data {
 
 namespace r3d_sfm {
 
-// ceres::RotationMatrixToAngleAxis (via the quaternion, robust near pi)
-inline void rotation_to_angle_axis(const double* R, double* aa) {
-  double q[4];
-  const double tr = R[0] + R[4] + R[8];
-  if (tr >= 0.0) {
-    double t = std::sqrt(tr + 1.0);
-    q[0] = 0.5 * t;
-    t = 0.5 / t;
-    q[1] = (R[7] - R[5]) * t;
-    q[2] = (R[2] - R[6]) * t;
-    q[3] = (R[3] - R[1]) * t;
-  } else {
-    int i = 0;
-    if (R[4] > R[0]) i = 1;
-    if (R[8] > R[4 * i]) i = 2;
-    const int j = (i + 1) % 3, k = (j + 1) % 3;
-    double t = std::sqrt(R[4 * i] - R[4 * j] - R[4 * k] + 1.0);
-    q[i + 1] = 0.5 * t;
-    t = 0.5 / t;
-    q[0] = (R[3 * k + j] - R[3 * j + k]) * t;
-    q[j + 1] = (R[3 * j + i] + R[3 * i + j]) * t;
-    q[k + 1] = (R[3 * k + i] + R[3 * i + k]) * t;
-  }
-  const double s2 = q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
-  if (s2 > 0.0) {
-    const double s = std::sqrt(s2), c = q[0];
-    const double two_theta = 2.0 * (c < 0.0 ? std::atan2(-s, -c) : std::atan2(s, c));
-    const double k = two_theta / s;
-    aa[0] = q[1] * k; aa[1] = q[2] * k; aa[2] = q[3] * k;
-  } else {
-    aa[0] = q[1] * 2.0; aa[1] = q[2] * 2.0; aa[2] = q[3] * 2.0;
-  }
-}
-
 inline void angle_axis_to_rotation(const double* aa, double* R) {  // Rodrigues, row-major
   const double th2 = aa[0] * aa[0] + aa[1] * aa[1] + aa[2] * aa[2];
   double A, B;
@@ -85,6 +51,39 @@ inline void angle_axis_to_rotation(const double* aa, double* R) {  // Rodrigues,
   const double K2[9] = {x * x - th2, x * y, x * z, x * y, y * y - th2, y * z, x * z, y * z, z * z - th2};
   for (int i = 0; i < 9; ++i) R[i] = ((i == 0 || i == 4 || i == 8) ? 1.0 : 0.0) + A * K[i] + B * K2[i];
 }
+
+// the centre C = -R^T t of the camera [R | t], R row-major
+inline void center_of(const double* R, const double* t, double* C) {
+  for (int i = 0; i < 3; ++i) C[i] = -(R[i] * t[0] + R[3 + i] * t[1] + R[6 + i] * t[2]);
+}
+
+// an intrinsic as the C ABI returns it, disto padded with zeros to 5
+inline void to_c_intrinsic(uint32_t id, const r3d_sfm_data::Intrinsic& in, r3d_sfm_intrinsic* out) {
+  out->id = id; out->model = in.model; out->width = in.width; out->height = in.height;
+  out->focal = in.focal; out->ppx = in.ppx; out->ppy = in.ppy;
+  for (int i = 0; i < 5; ++i) out->disto[i] = i < (int)in.disto.size() ? in.disto[i] : 0.0;
+}
+
+// The scene as bundle adjustment, triangulation and the outlier filters read it, with OpenMVG's BA parameterisation
+// (SURVEY.md A.7): poses and intrinsics in id order, one landmark per structure entry, its observations in view order.
+struct Flat {
+  std::map<uint32_t, uint32_t> pose_index, intr_index;  // id -> index
+  std::vector<double> poses;                            // 6 per pose: angle-axis(R) | t = -R C
+  std::vector<double> intr, ext;                        // 6 | 2 per intrinsic: f ppx ppy disto[0..2] | disto[3..4]
+  std::vector<uint8_t> model;                           // R3D_CAM_* per intrinsic
+  std::vector<uint32_t> cam_intr;                       // intrinsic index per pose (0 for a pose nobody observes)
+  std::vector<uint32_t> lm_ids;                         // landmark id per index
+  std::vector<double> X;                                // 3 per landmark
+  std::vector<uint64_t> obs_ofs;                        // observations of landmark l: [obs_ofs[l], obs_ofs[l + 1])
+  std::vector<uint32_t> obs_cam, obs_view;              // pose index, view id per observation
+  std::vector<double> obs_xy;                           // 2 per observation
+};
+
+// sd -> F (empty).  An observation of an unknown view, or of a view whose pose or intrinsic is undefined, is left out
+// when skip_undefined (IsPoseAndIntrinsicDefined) and is R3D_ERR_INVALID otherwise.  The solvers keep one intrinsic
+// group per pose (id_pose = id_view in every sfm_data the reference writes): a pose observed through two intrinsics
+// is R3D_ERR_UNSUPPORTED.  The first of these defects in (landmark, view) order decides the code.
+int flatten(const r3d_sfm_data& sd, bool skip_undefined, Flat& F);
 
 }  // namespace r3d_sfm
 

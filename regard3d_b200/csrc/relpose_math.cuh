@@ -178,7 +178,7 @@ R3D_RP_HD void projective(const double* K, const double* R, const double* t, dou
 
 // ceres::RotationMatrixToAngleAxis (RotationMatrixToQuaternion + QuaternionToAngleAxis), R row-major.  The two-view
 // BA's initial pose is converted on the host, where the oracle converts it, with the same libm; the pose refinement
-// of resection.cu converts on the device.
+// of resection.cu converts on the device, r3d_sfm::flatten (sfm_scene.cpp) the SfM_Data poses on the host.
 R3D_RP_HD void rotation_to_angle_axis(const double* R, double* aa) {
   double q[4];
   const double trace = R[0] + R[4] + R[8];

@@ -275,12 +275,10 @@ __global__ void __launch_bounds__(kRThreads) k_resect_refine(const RsView* __res
   }
 }
 
-void angle_axis_to_rotation(const double* aa, double* R) { r3d_sfm::angle_axis_to_rotation(aa, R); }
-
 void set_pose(r3d_resection& o, const double* R, const double* t) {
   std::memcpy(o.rotation, R, sizeof(o.rotation));
   std::memcpy(o.translation, t, sizeof(o.translation));
-  for (int i = 0; i < 3; ++i) o.center[i] = -(R[i] * t[0] + R[3 + i] * t[1] + R[6 + i] * t[2]);  // C = -R^T t
+  r3d_sfm::center_of(R, t, o.center);
 }
 
 // views [v0, v1) on worker w; inl[v]: the view's AC-RANSAC inliers (residual order)
@@ -427,7 +425,7 @@ int resect_range(r3d_ctx* ctx, DeviceWorker& w, const r3d_resection_view* views,
     T.lm_iterations += l.iterations;
     if (l.termination == 4) continue;  // the solve failed: the AC-RANSAC pose stays
     double R[9];
-    angle_axis_to_rotation(l.pose, R);
+    r3d_sfm::angle_axis_to_rotation(l.pose, R);
     set_pose(o, R, l.pose + 3);
   }
   T.ms_host = now_ms() - t0 - T.ms_device_total;
@@ -534,14 +532,7 @@ extern "C" int r3d_sfm_resect_views(r3d_ctx* ctx, r3d_sfm_data* sd, const uint32
     r.view_id = ids[k];
     r.width = vit->second.width;
     r.height = vit->second.height;
-    r.intrinsic.id = iit->first;
-    r.intrinsic.model = iit->second.model;
-    r.intrinsic.width = iit->second.width;
-    r.intrinsic.height = iit->second.height;
-    r.intrinsic.focal = iit->second.focal;
-    r.intrinsic.ppx = iit->second.ppx;
-    r.intrinsic.ppy = iit->second.ppy;
-    for (size_t i = 0; i < iit->second.disto.size() && i < 5; ++i) r.intrinsic.disto[i] = iit->second.disto[i];
+    r3d_sfm::to_c_intrinsic(iit->first, iit->second, &r.intrinsic);
   }
   // the 2D-3D correspondences of a view: every landmark that holds an observation of it, in landmark-id order
   std::vector<std::vector<double>> Xs(ids.size()), xs(ids.size());

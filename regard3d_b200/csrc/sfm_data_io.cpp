@@ -397,10 +397,7 @@ int r3d_sfm_get_intrinsic(const r3d_sfm_data* sd, uint32_t k, r3d_sfm_intrinsic*
   if (!sd || !out || k >= sd->intrinsics.size()) return R3D_ERR_INVALID;
   auto it = sd->intrinsics.begin();
   std::advance(it, k);
-  const r3d_sfm_data::Intrinsic& w = it->second;
-  out->id = it->first; out->model = w.model; out->width = w.width; out->height = w.height;
-  out->focal = w.focal; out->ppx = w.ppx; out->ppy = w.ppy;
-  for (int i = 0; i < 5; ++i) out->disto[i] = i < (int)w.disto.size() ? w.disto[i] : 0.0;
+  r3d_sfm::to_c_intrinsic(it->first, it->second, out);
   return R3D_OK;
 }
 

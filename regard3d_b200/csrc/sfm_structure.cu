@@ -14,7 +14,6 @@
 #include "p3p.cuh"
 
 #include <cstring>
-#include <map>
 
 struct r3d_tracks {  // tracks.cpp
   std::vector<uint32_t> ids;
@@ -174,63 +173,6 @@ using namespace r3d;
 
 namespace {
 
-struct Flat {  // the SfM_Data scene as the kernels read it
-  std::map<uint32_t, uint32_t> pose_index, intr_index;
-  std::vector<double> poses, intr, ext, obs_xy, X;
-  std::vector<uint8_t> model;
-  std::vector<uint32_t> cam_intr, obs_cam, lm_ids, obs_view;
-  std::vector<uint64_t> obs_ofs;
-};
-
-// poses / intrinsics as in r3d_sfm_bundle_adjust; landmarks = sd->structure, observations of views whose pose and
-// intrinsic are defined (IsPoseAndIntrinsicDefined)
-int flatten(const r3d_sfm_data* sd, Flat& F) {
-  for (const auto& kv : sd->poses) {
-    F.pose_index[kv.first] = (uint32_t)F.pose_index.size();
-    double aa[3];
-    r3d_sfm::rotation_to_angle_axis(kv.second.R, aa);
-    const double* R = kv.second.R;
-    const double* C = kv.second.C;
-    F.poses.insert(F.poses.end(), {aa[0], aa[1], aa[2], -(R[0] * C[0] + R[1] * C[1] + R[2] * C[2]),
-                                   -(R[3] * C[0] + R[4] * C[1] + R[5] * C[2]), -(R[6] * C[0] + R[7] * C[1] + R[8] * C[2])});
-  }
-  for (const auto& kv : sd->intrinsics) {
-    F.intr_index[kv.first] = (uint32_t)F.intr_index.size();
-    const r3d_sfm_data::Intrinsic& in = kv.second;
-    double p6[6] = {in.focal, in.ppx, in.ppy, 0, 0, 0}, e2[2] = {0, 0};
-    for (size_t k = 0; k < in.disto.size(); ++k) {
-      if (k < 3) p6[3 + k] = in.disto[k];
-      else e2[k - 3] = in.disto[k];
-    }
-    F.intr.insert(F.intr.end(), p6, p6 + 6);
-    F.ext.insert(F.ext.end(), e2, e2 + 2);
-    F.model.push_back((uint8_t)in.model);
-  }
-  F.cam_intr.assign(F.pose_index.size(), 0u);
-  std::vector<uint8_t> cam_set(F.pose_index.size(), 0);
-  F.obs_ofs.push_back(0);
-  for (const auto& kv : sd->structure) {
-    F.lm_ids.push_back(kv.first);
-    F.X.insert(F.X.end(), kv.second.X, kv.second.X + 3);
-    for (const auto& ob : kv.second.obs) {
-      auto vit = sd->views.find(ob.first);
-      if (vit == sd->views.end()) continue;
-      auto pit = F.pose_index.find(vit->second.id_pose);
-      auto iit = F.intr_index.find(vit->second.id_intrinsic);
-      if (pit == F.pose_index.end() || iit == F.intr_index.end()) continue;
-      if (cam_set[pit->second] && F.cam_intr[pit->second] != iit->second) return R3D_ERR_UNSUPPORTED;
-      cam_set[pit->second] = 1;
-      F.cam_intr[pit->second] = iit->second;
-      F.obs_cam.push_back(pit->second);
-      F.obs_view.push_back(ob.first);
-      F.obs_xy.push_back(ob.second.x[0]);
-      F.obs_xy.push_back(ob.second.x[1]);
-    }
-    F.obs_ofs.push_back(F.obs_cam.size());
-  }
-  return R3D_OK;
-}
-
 struct DevScene {
   DeviceWorker* w;
   std::vector<void*> blocks;
@@ -249,7 +191,7 @@ struct DevScene {
   }
 };
 
-int upload(r3d_ctx* ctx, const Flat& F, DevScene& D) {
+int upload(r3d_ctx* ctx, const r3d_sfm::Flat& F, DevScene& D) {
   const size_t n_lm = F.lm_ids.size(), n_obs = F.obs_cam.size(), n_cams = F.pose_index.size();
   bool ok = D.up(&D.poses, F.poses.data(), F.poses.size()) && D.up(&D.intr, F.intr.data(), F.intr.size()) &&
             D.up(&D.ext, F.ext.data(), F.ext.size()) && D.up(&D.X, F.X.data(), F.X.size()) && D.up(&D.model, F.model.data(), F.model.size()) &&
@@ -284,8 +226,8 @@ extern "C" int r3d_sfm_structure_from_tracks(r3d_ctx* ctx, r3d_sfm_data* sd, con
     }
     sd->structure[tracks->ids[k]] = std::move(lm);
   }
-  Flat F;
-  int rc = flatten(sd, F);
+  r3d_sfm::Flat F;
+  int rc = r3d_sfm::flatten(*sd, /*skip_undefined=*/true, F);
   if (rc) return fail(ctx, rc, "r3d_sfm_structure_from_tracks: a pose is shared by views with different intrinsics");
   uint32_t rejected = 0;
   const uint32_t n_lm = (uint32_t)F.lm_ids.size();
@@ -318,8 +260,8 @@ extern "C" int r3d_sfm_remove_outliers(r3d_ctx* ctx, r3d_sfm_data* sd, double ma
   if (!ctx || !sd) return fail(ctx, R3D_ERR_INVALID, "r3d_sfm_remove_outliers: bad arguments");
   DeviceWorker& w = ctx->workers[0];
   R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
-  Flat F;
-  int rc = flatten(sd, F);
+  r3d_sfm::Flat F;
+  int rc = r3d_sfm::flatten(*sd, /*skip_undefined=*/true, F);
   if (rc) return fail(ctx, rc, "r3d_sfm_remove_outliers: a pose is shared by views with different intrinsics");
   uint32_t rm_obs = 0, rm_lm = 0;
   const uint32_t n_lm = (uint32_t)F.lm_ids.size();

@@ -227,6 +227,9 @@ def test_structure_from_tracks_mixed_models(gpu_ctx, r3dlib):
 
 
 def test_pose_shared_by_two_intrinsics_is_unsupported(gpu_ctx, r3dlib):
+    """A pose observed through two intrinsics is R3D_ERR_UNSUPPORTED for triangulation, the outlier filters and bundle
+    adjustment.  An observation of an unknown view, or of a view without a pose, is skipped by the first two and
+    R3D_ERR_INVALID for bundle adjustment, which reports the first defect in (landmark, view) order."""
     rng, views, cams, cam_of, L, tf, xy, _ = _mixed_scene(n_random=200, n_ab=100)
     _upload(gpu_ctx, xy)
     tracks = _tracks(r3dlib, [t[0] for t in L], tf)
@@ -234,6 +237,49 @@ def test_pose_shared_by_two_intrinsics_is_unsupported(gpu_ctx, r3dlib):
     with pytest.raises(r3dlib.R3DError) as e:
         gpu_ctx.structure_from_tracks(sd, tracks)
     assert e.value.code == R3D_ERR_UNSUPPORTED
+    # views 0 .. 3: intrinsic 0, pose v; view 4: a pose id that is never defined; view 5: pose 0 with intrinsic 1;
+    # view 9: not in the scene.  Landmark l < 20 is seen by views 0 .. 3, the extra ones by the views listed.
+    rng = np.random.default_rng(31)
+    base = [sr.look_at(C) for C in sr.sphere_centres(rng, 4, 8.0)]
+    X = rng.uniform(-1.0, 1.0, (22, 3))
+    xy = {v: project(MODELS[2], FOCAL, *_ppx(0), DISTO[MODELS[2]], *base[v if v < 4 else 0], X).astype(np.float32)
+          for v in (0, 1, 2, 3, 4, 5, 9)}
+    _upload(gpu_ctx, xy)
+
+    def scene(lms):
+        sd = r3dlib.SfmData()
+        for g in (0, 1):
+            sd.add_intrinsic(g, MODELS[2 - 2 * g], W, H, FOCAL, *_ppx(g), disto=list(DISTO[MODELS[2 - 2 * g]]))
+        for v, (gi, pid) in {0: (0, 0), 1: (0, 1), 2: (0, 2), 3: (0, 3), 4: (0, 99), 5: (1, 0)}.items():
+            sd.add_view(v, "image%06d.jpg" % v, W, H, id_intrinsic=gi, id_pose=pid)
+        for v in range(4):
+            sd.add_pose(v, base[v][0], -base[v][0].T @ base[v][1])
+        for l, vs in enumerate(lms):
+            sd.add_landmark(l, X[l], [(v, l, float(xy[v][l, 0]), float(xy[v][l, 1])) for v in vs])
+        return sd
+
+    def code(call, *args, **kw):
+        try:
+            call(*args, **kw)
+            return 0
+        except r3dlib.R3DError as e:
+            return e.code
+
+    INV, UNS = -1, R3D_ERR_UNSUPPORTED
+    # extra landmarks -> code of bundle adjustment, code of triangulation and the outlier filters
+    for extra, ba, others in (([], 0, 0), ([[1, 9]], INV, 0), ([[1, 4]], INV, 0), ([[1, 5]], UNS, UNS),
+                              ([[1, 4], [1, 5]], INV, UNS), ([[1, 5], [1, 4]], UNS, UNS), ([[4, 5]], INV, UNS),
+                              ([[5, 9]], UNS, UNS)):
+        lms = [[0, 1, 2, 3]] * 20 + extra
+        tracks = _tracks(r3dlib, lms, [[l] * len(vs) for l, vs in enumerate(lms)])
+        assert code(gpu_ctx.structure_from_tracks, scene([]), tracks) == others, extra
+        assert code(gpu_ctx.remove_outliers, scene(lms)) == others, extra
+        assert code(gpu_ctx.sfm_bundle_adjust, scene(lms), max_iterations=5) == ba, extra
+    # an empty scene: nothing to triangulate or filter, nothing to adjust
+    empty = r3dlib.Tracks.build(r3dlib.Matches.from_csr(np.zeros((0, 2)), np.zeros(1), np.zeros(0, r3dlib.indmatch_dtype)), 2)
+    assert gpu_ctx.structure_from_tracks(scene([]), empty) == 0
+    assert gpu_ctx.remove_outliers(scene([])) == (0, 0)
+    assert code(gpu_ctx.sfm_bundle_adjust, scene([])) == INV
 
 
 # ---- 3. outlier filters on landmarks set directly ------------------------------------------------------------------------
