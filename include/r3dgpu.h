@@ -417,7 +417,8 @@ int r3d_rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t 
 int r3d_matches_keep_largest_biedge_component(const r3d_matches* m, r3d_matches** out);
 
 /* ---- global translations from the relative motions and the global rotations (global SfM, third step) ----------- */
-#define R3D_TRANSAVG_L1 1            /* TRANSLATION_AVERAGING_L1 (the linear program): not implemented, R3D_ERR_UNSUPPORTED */
+#define R3D_TRANSAVG_L1 1            /* TRANSLATION_AVERAGING_L1 (the linear program): R3D_ERR_UNSUPPORTED here, solved by
+                                      * r3d_translation_averaging_l1 */
 #define R3D_TRANSAVG_L2_CHORDAL 2    /* TRANSLATION_AVERAGING_L2_DISTANCE_CHORDAL: 1DSfM chordal distance on the centres */
 #define R3D_TRANSAVG_SOFTL1 3        /* TRANSLATION_AVERAGING_SOFTL1: soft-L1 on t_j - (R_ij t_i + s_ij t_ij), s_ij >= 1 */
 /* The method values are Regard3D's transAveraging_ (src/threads/R3DTriangulationThread.cpp:204-208). */
@@ -458,6 +459,42 @@ int r3d_translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64
                               const double* rotations, const uint8_t* rot_kept, uint32_t n_views,
                               const r3d_transavg_options* opt, double* centers, double* translations, uint8_t* view_kept,
                               uint8_t* edge_kept, r3d_transavg_summary* summary);
+
+/* ---- global translations by Regard3D's default method, TRANSLATION_AVERAGING_L1 ----------------------------------- */
+typedef struct {
+  int max_iterations;                /* 100: interior-point iterations (>= 1) */
+  double tolerance;                  /* 1e-9: stop when max |G y + s - h| <= tol (1 + |h|_inf), max |G^T z + c| <= tol and
+                                      * |gamma - dual objective| <= tol (1 + |gamma|) (> 0) */
+} r3d_transavg_l1_options;
+void r3d_transavg_l1_default_options(r3d_transavg_l1_options* o);  /* 100, 1e-9 */
+typedef struct {
+  int success;                       /* as r3d_transavg_summary */
+  uint64_t n_edges, n_kept_edges;
+  uint32_t n_kept_views;
+  uint32_t iterations;               /* predictor-corrector iterations */
+  uint32_t regularized_factorizations;  /* retries of a factorisation that was not positive definite, each with
+                                      * 1e-18, 1e-16, ... (x 100, at most 5) times the largest diagonal entry added */
+  int termination;                   /* 0 converged, 1 iteration cap, 2 factorisation failed, -1 not run */
+  double gamma;                      /* the L-infinity bound of the returned point (the LP's objective) */
+  double dual_objective;
+  double max_primal_violation;       /* largest violation of a constraint by the returned point (>= 0) */
+  double max_dual_violation;         /* max |G^T z + c| */
+  double ms_solve, ms_device_total, ms_host;
+} r3d_transavg_l1_summary;
+/* Replaces GlobalSfM_Translation_AveragingSolver::Translation_averaging for TRANSLATION_AVERAGING_L1 (OpenMVG 1.4,
+ * Tifromtij_ConstraintBuilder + the CLP solver; Regard3D's default, src/threads/R3DTriangulationThread.cpp:204): the
+ * L-infinity translation registration of Moulon et al. (ICCV 2013) on the pairwise relative translations, one scale per
+ * edge:  minimise gamma  s.t.  |(T_J - R_J R_I^T T_I - lambda_IJ t_IJ / |t_IJ|)_k| <= gamma,  lambda_IJ >= 1, by a
+ * primal-dual interior-point method (Mehrotra predictor-corrector) on the first device.  Inputs, edge rules, the kept
+ * component, the gauge (the lowest kept view id gets T = 0) and the outputs centers / translations / view_kept /
+ * edge_kept as r3d_translation_averaging's soft-L1 method; edge_scale (n_rel, may be NULL): lambda of the kept edges,
+ * 0 elsewhere.  The optimal value gamma is unique, the optimal point in general is not: the method returns a point near
+ * the centre of the optimal face, not a vertex.  Errors as r3d_translation_averaging, and R3D_ERR_INVALID for
+ * max_iterations < 1 or tolerance <= 0. */
+int r3d_translation_averaging_l1(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use,
+                                 const double* rotations, const uint8_t* rot_kept, uint32_t n_views,
+                                 const r3d_transavg_l1_options* opt, double* centers, double* translations, uint8_t* view_kept,
+                                 uint8_t* edge_kept, double* edge_scale, r3d_transavg_l1_summary* summary);
 
 /* ---- the steps either side of bundle adjustment (SURVEY.md 8f-3) -------------------------------------------------
  * openMVG::tracks::TracksBuilder Build + Filter(min_length) + ExportToSTL, as Regard3D calls them itself

@@ -37,7 +37,8 @@ EXPORTS = [
     "r3d_relpose_default_options", "r3d_relative_poses", "r3d_get_relpose_timing",
     "r3d_resection_default_options", "r3d_resect_views", "r3d_sfm_resect_views", "r3d_get_resection_timing",
     "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_matches_keep_largest_biedge_component",
-    "r3d_transavg_default_options", "r3d_translation_averaging", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
+    "r3d_transavg_default_options", "r3d_translation_averaging", "r3d_transavg_l1_default_options",
+    "r3d_translation_averaging_l1", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
     "r3d_debug_acransac_score", "r3d_debug_detmath", "r3d_debug_ba_step",
     "r3d_akaze_default_options", "r3d_akaze_levels", "r3d_akaze_detect", "r3d_features_num_images", "r3d_features_count",
     "r3d_features_get", "r3d_free_features", "r3d_get_akaze_timing", "r3d_debug_akaze_levels",
@@ -234,6 +235,18 @@ class TransavgSummary(C.Structure):
                 ("lm_iterations", C.c_uint32), ("lm_successful_steps", C.c_uint32), ("lm_termination", C.c_int),
                 ("lm_initial_cost", C.c_double), ("lm_final_cost", C.c_double), ("ms_solve", C.c_double),
                 ("ms_device_total", C.c_double), ("ms_host", C.c_double)]
+
+
+class TransavgL1Options(C.Structure):
+    _fields_ = [("max_iterations", C.c_int), ("tolerance", C.c_double)]
+
+
+class TransavgL1Summary(C.Structure):
+    _fields_ = [("success", C.c_int), ("n_edges", C.c_uint64), ("n_kept_edges", C.c_uint64), ("n_kept_views", C.c_uint32),
+                ("iterations", C.c_uint32), ("regularized_factorizations", C.c_uint32), ("termination", C.c_int),
+                ("gamma", C.c_double), ("dual_objective", C.c_double), ("max_primal_violation", C.c_double),
+                ("max_dual_violation", C.c_double), ("ms_solve", C.c_double), ("ms_device_total", C.c_double),
+                ("ms_host", C.c_double)]
 
 
 def relative_pose_records(I, J, R, status=None):
@@ -1145,6 +1158,36 @@ class Context:
                                                     C.byref(s)))
         summ = {k: getattr(s, k) for k, _ in TransavgSummary._fields_}
         return cen[:n_views], tra[:n_views], vk[:n_views].astype(bool), ek[:len(rel)].astype(bool), summ
+
+    def translation_averaging_l1(self, rel, rotations, rot_kept, n_views, edge_use=None, max_iterations=100, tolerance=1e-9):
+        """r3d_translation_averaging_l1: the L-infinity translation LP (Regard3D's default L1 method) on the same edges as
+        translation_averaging.  Returns (centers (n_views, 3), translations (n_views, 3), view_kept (n_views,) bool,
+        edge_kept (len(rel),) bool, edge_scale (len(rel),) (lambda of the kept edges, 0 elsewhere), summary dict)."""
+        rel = np.ascontiguousarray(rel, relpose_dtype)
+        rot = np.ascontiguousarray(np.asarray(rotations, np.float64).reshape(-1, 3, 3))
+        rk = np.ascontiguousarray(np.asarray(rot_kept).astype(np.uint8).ravel())
+        if len(rot) < n_views or len(rk) < n_views:
+            raise ValueError("rotations / rot_kept hold fewer than n_views views")
+        use = None
+        if edge_use is not None:
+            use = np.ascontiguousarray(np.asarray(edge_use).astype(np.uint8).ravel())
+            if len(use) != len(rel):
+                raise ValueError("edge_use must have one entry per record")
+        o = TransavgL1Options()
+        lib().r3d_transavg_l1_default_options(C.byref(o))
+        o.max_iterations = max_iterations
+        o.tolerance = tolerance
+        cen = np.zeros((max(n_views, 1), 3))
+        tra = np.zeros((max(n_views, 1), 3))
+        vk = np.zeros(max(n_views, 1), np.uint8)
+        ek = np.zeros(max(len(rel), 1), np.uint8)
+        lam = np.zeros(max(len(rel), 1))
+        s = TransavgL1Summary()
+        self._check(lib().r3d_translation_averaging_l1(self._h, _p(rel), C.c_uint64(len(rel)), None if use is None else _p(use),
+                                                       _p(rot), _p(rk), C.c_uint32(n_views), C.byref(o), _p(cen), _p(tra), _p(vk),
+                                                       _p(ek), _p(lam), C.byref(s)))
+        summ = {k: getattr(s, k) for k, _ in TransavgL1Summary._fields_}
+        return cen[:n_views], tra[:n_views], vk[:n_views].astype(bool), ek[:len(rel)].astype(bool), lam[:len(rel)].copy(), summ
 
     def relpose_timing(self):
         t = RelposeTiming()

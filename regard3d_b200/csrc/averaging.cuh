@@ -1,7 +1,9 @@
 // averaging.cuh -- the Levenberg-Marquardt refinement shared by the global-SfM averaging steps, rotations (rotavg.cu) and
 // translations (transavg.cu): forward-mode duals, the per-view Jacobi scale and gradient, the step and sum kernels, the
 // incidence lists and the host loop around lm_trust_region.cuh's trust region.  Each step keeps its own residuals and
-// its own system assembly.  Only for translation units compiled with --fmad=false (regard3d_b200/build.py).
+// its own system assembly.  Also the translation steps' shared edge selection (ta::select_edges, transavg.cu) and
+// rotavg.cu's 3-column triangular solve (trsm3), which the L1 translation solver (transavg_l1.cu) reuses.  Only for
+// translation units compiled with --fmad=false (regard3d_b200/build.py).
 #pragma once
 #include "r3d_internal.cuh"
 #include "lm_trust_region.cuh"
@@ -157,6 +159,11 @@ __global__ void __launch_bounds__(128, 9) k_avg_grad(int mode, const uint32_t* _
 // -1; comp[v] = component of v, -1 for nodes without edges.
 int largest_biedge_component(uint32_t n, const std::vector<uint32_t>& eu, const std::vector<uint32_t>& ev, std::vector<int>& comp);
 
+// rotavg.cu: L Lt X = Y in place of Y (n x 3 row-major), Z: n x 3 scratch, with the factor L, Linv of dense_cholesky
+// (one cooperative launch); trsm3_grid resolves grid 0 and checks that the grid can be co-resident.
+int trsm3_grid(r3d_ctx* ctx, DeviceWorker& w, int* grid);
+int trsm3(r3d_ctx* ctx, DeviceWorker& w, const double* L, const double* Linv, int n, double* Y, double* Z, int grid);
+
 // Incidence lists of m views over edges given as (lo < hi) and sorted by (lo, hi), in neighbour order: view v's entries
 // (lo < v) come first in lo order, then (v, hi > v) in hi order.  ofs: m + 1 offsets; nbr, edge: the neighbour and the
 // edge index of each entry.
@@ -268,4 +275,24 @@ int averaging_lm(r3d_ctx* ctx, DeviceWorker& w, const LmParams& prm, const AvgBu
 }
 
 }  // namespace ra
+
+namespace ta {
+
+// The edges of a translation-averaging call (transavg.cu), shared by r3d_translation_averaging and
+// r3d_translation_averaging_l1: the OK records with edge_use set, checked (I != J, ids < n_views, a non-zero finite
+// translation, no unordered pair twice), in canonical (min, max) order, both views rotation-kept; the largest
+// bi-edge-connected component of them, local ids in view id order (local 0 = the lowest kept view id, the gauge).
+struct KeptEdges {
+  uint64_t n_edges = 0;          // usable edges before the component
+  std::vector<uint32_t> kview;   // kept view ids by local id; empty: no component
+  std::vector<uint2> kab, ab;    // per kept edge: canonical (lo < hi) and record-oriented (I, J) local ids
+  std::vector<uint64_t> src;     // per kept edge: its record
+  std::vector<double> Rij, u;    // per kept edge: R_J R_I^T (9, row-major) and t_IJ / |t_IJ| (3)
+};
+// R3D_OK (K.kview empty when no component survives), R3D_ERR_INVALID for a bad record, R3D_ERR_UNSUPPORTED for more
+// than R3D_ROTAVG_MAX_VIEWS kept views; fn prefixes the error messages.
+int select_edges(r3d_ctx* ctx, const char* fn, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use,
+                 const double* rot, const uint8_t* rot_kept, uint32_t n_views, KeptEdges& K);
+
+}  // namespace ta
 }  // namespace r3d

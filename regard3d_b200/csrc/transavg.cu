@@ -5,7 +5,8 @@
 //
 // Replaces GlobalSfM_Translation_AveragingSolver::Translation_averaging (OpenMVG 1.4, SURVEY.md A.11) for
 // TRANSLATION_AVERAGING_L2_DISTANCE_CHORDAL and TRANSLATION_AVERAGING_SOFTL1, on the pairwise relative translations:
-//   1. host: the usable edges, the largest bi-edge-connected component (rotavg.cu's Tarjan), reindexing by view id.
+//   1. host (select_edges, shared with transavg_l1.cu): the usable edges, the largest bi-edge-connected component
+//      (rotavg.cu's Tarjan), reindexing by view id.
 //   2. Levenberg-Marquardt (averaging.cuh's loop around lm_trust_region.cuh's trust region), the lowest kept view held:
 //      k_ta_eval (one thread per edge, forward-mode duals: residual, 3 x 7 Jacobian, soft-L1 corrector), k_ta_edge
 //      (the scale columns' Jacobi scale and gradient), k_ta_system (one owner CTA per view block row: J^T J + D^2 with
@@ -262,18 +263,9 @@ double start_value(uint64_t k) {
   return (double)(z >> 11) * (1.0 / 9007199254740992.0);
 }
 
-int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use, const double* rot,
-                          const uint8_t* rot_kept, uint32_t n_views, const r3d_transavg_options& opt, double* centers,
-                          double* translations, uint8_t* view_kept, uint8_t* edge_kept, r3d_transavg_summary& S) {
-  const double t0 = now_ms();
-  const char* fn = "r3d_translation_averaging: ";
-  DeviceWorker& w = ctx->workers[0];
-  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
-  std::memset(centers, 0, (size_t)n_views * 3 * sizeof(double));
-  std::memset(translations, 0, (size_t)n_views * 3 * sizeof(double));
-  std::memset(view_kept, 0, n_views);
-  if (edge_kept) std::memset(edge_kept, 0, n_rel);
-  // ---- 1. edges: checked, canonical order (min, max); the record's orientation is kept ----
+int select_edges(r3d_ctx* ctx, const char* fn, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use,
+                 const double* rot, const uint8_t* rot_kept, uint32_t n_views, KeptEdges& K) {
+  // edges: checked, canonical order (min, max); the record's orientation is kept
   struct Edge { uint32_t lo, hi; uint64_t src; };
   std::vector<Edge> edges;
   for (uint64_t k = 0; k < n_rel; ++k) {
@@ -291,47 +283,78 @@ int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
     if (edges[k].lo == edges[k - 1].lo && edges[k].hi == edges[k - 1].hi)
       return fail(ctx, R3D_ERR_INVALID, std::string(fn) + "the same pair of views is given twice");
   edges.erase(std::remove_if(edges.begin(), edges.end(), [&](const Edge& e) { return !rot_kept[e.lo] || !rot_kept[e.hi]; }), edges.end());
-  S.n_edges = edges.size();
-  // ---- the largest bi-edge-connected component, local ids in view id order ----
+  K.n_edges = edges.size();
+  // the largest bi-edge-connected component, local ids in view id order
   std::vector<uint32_t> eu(edges.size()), ev(edges.size());
   for (size_t k = 0; k < edges.size(); ++k) { eu[k] = edges[k].lo; ev[k] = edges[k].hi; }
   std::vector<int> comp;
   const int best = ra::largest_biedge_component(n_views, eu, ev, comp);
-  if (best < 0) {
-    S.ms_host = now_ms() - t0;
-    return R3D_OK;
-  }
-  std::vector<uint32_t> local(n_views, UINT32_MAX), kview;
+  if (best < 0) return R3D_OK;
+  std::vector<uint32_t> local(n_views, UINT32_MAX);
   for (uint32_t v = 0; v < n_views; ++v)
-    if (comp[v] == best) { local[v] = (uint32_t)kview.size(); kview.push_back(v); }
-  const uint32_t m = (uint32_t)kview.size();
-  if (m > R3D_ROTAVG_MAX_VIEWS)
+    if (comp[v] == best) { local[v] = (uint32_t)K.kview.size(); K.kview.push_back(v); }
+  if (K.kview.size() > R3D_ROTAVG_MAX_VIEWS) {
+    K.kview.clear();
     return fail(ctx, R3D_ERR_UNSUPPORTED, std::string(fn) + "more than R3D_ROTAVG_MAX_VIEWS views in the component");
-  const bool softl1 = opt.method == kSoftL1;
-  std::vector<uint2> kab, ab;  // canonical (lo < hi) and record-oriented (I, J) local ids of the kept edges
-  std::vector<double> ed;      // per kept edge: chordal u (3, 3 unused); soft-L1 the angle-axis of R_J R_I^T (3), t_IJ / |t_IJ| (3)
+  }
   for (const Edge& e : edges) {
     if (local[e.lo] == UINT32_MAX || local[e.hi] == UINT32_MAX) continue;
     const r3d_relative_pose& r = rel[e.src];
-    kab.push_back(make_uint2(local[e.lo], local[e.hi]));
-    ab.push_back(make_uint2(local[r.I], local[r.J]));
+    K.kab.push_back(make_uint2(local[e.lo], local[e.hi]));
+    K.ab.push_back(make_uint2(local[r.I], local[r.J]));
+    K.src.push_back(e.src);
     const double* t = r.translation;
     const double tn = std::sqrt(t[0] * t[0] + t[1] * t[1] + t[2] * t[2]);
     const double u[3] = {t[0] / tn, t[1] / tn, t[2] / tn};
     const double* RI = rot + 9 * (size_t)r.I;
     const double* RJ = rot + 9 * (size_t)r.J;
+    double Rij[9];
+    for (int a = 0; a < 3; ++a)
+      for (int b = 0; b < 3; ++b) Rij[3 * a + b] = RJ[3 * a] * RI[3 * b] + RJ[3 * a + 1] * RI[3 * b + 1] + RJ[3 * a + 2] * RI[3 * b + 2];
+    K.Rij.insert(K.Rij.end(), Rij, Rij + 9);
+    K.u.insert(K.u.end(), u, u + 3);
+  }
+  return R3D_OK;
+}
+
+int translation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use, const double* rot,
+                          const uint8_t* rot_kept, uint32_t n_views, const r3d_transavg_options& opt, double* centers,
+                          double* translations, uint8_t* view_kept, uint8_t* edge_kept, r3d_transavg_summary& S) {
+  const double t0 = now_ms();
+  DeviceWorker& w = ctx->workers[0];
+  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
+  std::memset(centers, 0, (size_t)n_views * 3 * sizeof(double));
+  std::memset(translations, 0, (size_t)n_views * 3 * sizeof(double));
+  std::memset(view_kept, 0, n_views);
+  if (edge_kept) std::memset(edge_kept, 0, n_rel);
+  // ---- 1. the kept edges (select_edges) ----
+  const char* fn = "r3d_translation_averaging: ";
+  KeptEdges K;
+  const int rc0 = select_edges(ctx, fn, rel, n_rel, edge_use, rot, rot_kept, n_views, K);
+  S.n_edges = K.n_edges;
+  if (rc0) return rc0;
+  if (K.kview.empty()) {
+    S.ms_host = now_ms() - t0;
+    return R3D_OK;
+  }
+  const std::vector<uint32_t>& kview = K.kview;
+  const std::vector<uint2>& kab = K.kab;
+  const std::vector<uint2>& ab = K.ab;
+  const uint32_t m = (uint32_t)kview.size();
+  const bool softl1 = opt.method == kSoftL1;
+  std::vector<double> ed;  // per kept edge: chordal u (3, 3 unused); soft-L1 the angle-axis of R_J R_I^T (3), t_IJ / |t_IJ| (3)
+  for (size_t k = 0; k < kab.size(); ++k) {
+    const double* u = &K.u[3 * k];
+    const double* RJ = rot + 9 * (size_t)rel[K.src[k]].J;
     double q[6] = {0, 0, 0, 0, 0, 0};
     if (!softl1) {
-      for (int k = 0; k < 3; ++k) q[k] = -(RJ[k] * u[0] + RJ[3 + k] * u[1] + RJ[6 + k] * u[2]);
+      for (int c = 0; c < 3; ++c) q[c] = -(RJ[c] * u[0] + RJ[3 + c] * u[1] + RJ[6 + c] * u[2]);
     } else {
-      double Rij[9];
-      for (int a = 0; a < 3; ++a)
-        for (int b = 0; b < 3; ++b) Rij[3 * a + b] = RJ[3 * a] * RI[3 * b] + RJ[3 * a + 1] * RI[3 * b + 1] + RJ[3 * a + 2] * RI[3 * b + 2];
-      rp::rotation_to_angle_axis(Rij, q);
-      for (int k = 0; k < 3; ++k) q[3 + k] = u[k];
+      rp::rotation_to_angle_axis(&K.Rij[9 * k], q);
+      for (int c = 0; c < 3; ++c) q[3 + c] = u[c];
     }
     ed.insert(ed.end(), q, q + 6);
-    if (edge_kept) edge_kept[e.src] = 1;
+    if (edge_kept) edge_kept[K.src[k]] = 1;
   }
   const uint32_t ne = (uint32_t)kab.size();
   S.success = 1;
