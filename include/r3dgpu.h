@@ -706,6 +706,42 @@ typedef struct {
 int r3d_debug_ba_step(r3d_ctx* ctx, const r3d_ba_problem* p, const r3d_ba_options* opt, double radius, int schur_route,
                       int chol_method, r3d_ba_step_out* out);
 
+/* Diagnostics (device): one predictor-corrector iteration of r3d_translation_averaging_l1, through the code that
+ * function runs per iteration, on the same kept edges.  A state is packed as y (N = 3 (m - 1) + 1: T of the free kept
+ * views in local order, then gamma), lambda (ne), s (7 ne), z (7 ne), the last three in kept-edge order and the 7 rows
+ * of an edge as the LP's (r_k - gamma, -r_k - gamma for k = 0..2, -lambda).  Array outputs are caller-allocated for at
+ * most m = n_views kept views and ne = n_rel kept edges, NULL ones are skipped; the scalars are always filled. */
+typedef struct {
+  uint32_t n_kept_views, n_kept_edges, n;  /* m, ne, N; 0: no component, nothing else written */
+  uint32_t* view_ids;       /* m: the kept view ids by local id (local 0: the gauge) */
+  uint64_t* edge_record;    /* ne: each kept edge's record */
+  uint32_t* edge_ij;        /* ne x 2: its record-oriented local (I, J) */
+  double* Rij;              /* ne x 9: R_J R_I^T (row-major) as the kernels use it */
+  double* u;                /* ne x 3: t_IJ / |t_IJ| as the kernels use it */
+  double* state0;           /* N + 15 ne: the state the iteration started from */
+  double norms[5];          /* k_tl_norms: max |G y + s - h|, max(0, G y - h), max |G^T z + c|, s^T z, -h^T z */
+  double* A;                /* (N + 1) x N: the reduced (T, gamma) system as assembled, before scaling (rows 0..N-1;
+                             * the T block in full, the gamma row N - 1, the gamma column above it not written: 0),
+                             * row N: the predictor's right-hand side */
+  double* sc;               /* N: the Jacobi scale, 1 / sqrt(A_ii) (1 where A_ii <= 0) */
+  int not_pd[6];            /* per factorisation attempt of the predictor: it met a pivot that is not > 0 */
+  uint32_t retries;         /* attempts after the first (each with the diagonal raised) */
+  double *pred_dy, *pred_dlam, *pred_ds, *pred_dz;  /* N, ne, 7 ne, 7 ne: the predictor's step (dy refined, unscaled) */
+  double pred_alpha_p, pred_alpha_d, pred_complementarity;  /* its step lengths (eta = 1), (s + a_p ds)^T (z + a_d dz) */
+  double sigma;             /* the centring (mu_aff / mu)^3 */
+  double* corr_rhs;         /* N: the corrector's right-hand side, scaled by sc */
+  double *corr_dy, *corr_dlam, *corr_ds, *corr_dz;  /* the corrector's step */
+  double alpha_p, alpha_d;  /* its step lengths (eta = 0.99) */
+  double* state;            /* N + 15 ne: the state after the step */
+  int converged;            /* the stopping test held at the start: nothing after the norms and A ran */
+  int failed;               /* every factorisation attempt failed: nothing after the predictor ran */
+} r3d_transavg_l1_step_out;
+/* state: NULL for the solver's start point, else N + 15 ne values (n_state), finite, s > 0 and z >= 0, or
+ * R3D_ERR_INVALID.  tolerance: the stopping test's (r3d_transavg_l1_options). */
+int r3d_debug_transavg_l1_step(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use,
+                               const double* rotations, const uint8_t* rot_kept, uint32_t n_views, const double* state,
+                               uint64_t n_state, double tolerance, r3d_transavg_l1_step_out* out);
+
 /* ---- keypoints (SURVEY.md 3: the feature stage's detector) ------------------------------------------------------ */
 /* Fast-AKAZE, Regard3D's default detector: Regard3DFeatures::detectKeypoints' "Fast-AKAZE" branch
  * (src/Regard3DFeatures.cpp:590-614) with cv::AKAZE2 of src/thirdparty/fast-akaze.  Input: float gray images in

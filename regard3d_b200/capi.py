@@ -38,7 +38,7 @@ EXPORTS = [
     "r3d_resection_default_options", "r3d_resect_views", "r3d_sfm_resect_views", "r3d_get_resection_timing",
     "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_matches_keep_largest_biedge_component",
     "r3d_transavg_default_options", "r3d_translation_averaging", "r3d_transavg_l1_default_options",
-    "r3d_translation_averaging_l1", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
+    "r3d_translation_averaging_l1", "r3d_debug_transavg_l1_step", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
     "r3d_debug_acransac_score", "r3d_debug_detmath", "r3d_debug_ba_step",
     "r3d_akaze_default_options", "r3d_akaze_levels", "r3d_akaze_detect", "r3d_features_num_images", "r3d_features_count",
     "r3d_features_get", "r3d_free_features", "r3d_get_akaze_timing", "r3d_debug_akaze_levels",
@@ -247,6 +247,18 @@ class TransavgL1Summary(C.Structure):
                 ("gamma", C.c_double), ("dual_objective", C.c_double), ("max_primal_violation", C.c_double),
                 ("max_dual_violation", C.c_double), ("ms_solve", C.c_double), ("ms_device_total", C.c_double),
                 ("ms_host", C.c_double)]
+
+
+class TransavgL1StepOut(C.Structure):
+    _fields_ = [("n_kept_views", C.c_uint32), ("n_kept_edges", C.c_uint32), ("n", C.c_uint32), ("view_ids", C.c_void_p),
+                ("edge_record", C.c_void_p), ("edge_ij", C.c_void_p), ("Rij", C.c_void_p), ("u", C.c_void_p),
+                ("state0", C.c_void_p), ("norms", C.c_double * 5), ("A", C.c_void_p), ("sc", C.c_void_p),
+                ("not_pd", C.c_int * 6), ("retries", C.c_uint32), ("pred_dy", C.c_void_p), ("pred_dlam", C.c_void_p),
+                ("pred_ds", C.c_void_p), ("pred_dz", C.c_void_p), ("pred_alpha_p", C.c_double), ("pred_alpha_d", C.c_double),
+                ("pred_complementarity", C.c_double), ("sigma", C.c_double), ("corr_rhs", C.c_void_p),
+                ("corr_dy", C.c_void_p), ("corr_dlam", C.c_void_p), ("corr_ds", C.c_void_p), ("corr_dz", C.c_void_p),
+                ("alpha_p", C.c_double), ("alpha_d", C.c_double), ("state", C.c_void_p), ("converged", C.c_int),
+                ("failed", C.c_int)]
 
 
 def relative_pose_records(I, J, R, status=None):
@@ -1188,6 +1200,55 @@ class Context:
                                                        _p(ek), _p(lam), C.byref(s)))
         summ = {k: getattr(s, k) for k, _ in TransavgL1Summary._fields_}
         return cen[:n_views], tra[:n_views], vk[:n_views].astype(bool), ek[:len(rel)].astype(bool), lam[:len(rel)].copy(), summ
+
+    def debug_transavg_l1_step(self, rel, rotations, rot_kept, n_views, edge_use=None, state=None, tolerance=1e-9):
+        """r3d_debug_transavg_l1_step: one iteration of translation_averaging_l1 on the same kept edges, from state =
+        (y, lam, s, z) (y: T of the free kept views then gamma; lam, s, z in kept-edge order) or, with None, the
+        solver's start point.  Returns a dict: m, ne, N, view_ids, edge_record, edge_ij (ne, 2), Rij (ne, 3, 3), u (ne, 3),
+        state0 and state (each a (y, lam, s, z) tuple), norms (5), A ((N + 1) x N: the unscaled reduced matrix, row N
+        the predictor's right-hand side), sc, not_pd (per attempt), retries, pred / corr dicts of dy, dlam, ds, dz,
+        alpha_p, alpha_d (pred also complementarity, corr also rhs, scaled), sigma, converged, failed."""
+        rel = np.ascontiguousarray(rel, relpose_dtype)
+        rot = np.ascontiguousarray(np.asarray(rotations, np.float64).reshape(-1, 3, 3))
+        rk = np.ascontiguousarray(np.asarray(rot_kept).astype(np.uint8).ravel())
+        if len(rot) < n_views or len(rk) < n_views:
+            raise ValueError("rotations / rot_kept hold fewer than n_views views")
+        use = None
+        if edge_use is not None:
+            use = np.ascontiguousarray(np.asarray(edge_use).astype(np.uint8).ravel())
+            if len(use) != len(rel):
+                raise ValueError("edge_use must have one entry per record")
+        x = None if state is None else np.ascontiguousarray(np.concatenate([np.asarray(a, np.float64).ravel() for a in state]))
+        mc, ec = max(n_views, 1), max(len(rel), 1)
+        nc = 3 * mc + 1
+        nx = nc + 15 * ec
+        r = {"view_ids": np.zeros(mc, np.uint32), "edge_record": np.zeros(ec, np.uint64), "edge_ij": np.zeros(2 * ec, np.uint32),
+             "Rij": np.zeros(9 * ec), "u": np.zeros(3 * ec), "state0": np.zeros(nx), "A": np.zeros((nc + 1) * nc), "sc": np.zeros(nc),
+             "corr_rhs": np.zeros(nc), "state": np.zeros(nx)}
+        for ph in ("pred", "corr"):
+            r.update({ph + "_dy": np.zeros(nc), ph + "_dlam": np.zeros(ec), ph + "_ds": np.zeros(7 * ec), ph + "_dz": np.zeros(7 * ec)})
+        out = TransavgL1StepOut(**{k: v.ctypes.data for k, v in r.items()})
+        self._check(lib().r3d_debug_transavg_l1_step(self._h, _p(rel), C.c_uint64(len(rel)), None if use is None else _p(use),
+                                                     _p(rot), _p(rk), C.c_uint32(n_views), None if x is None else _p(x),
+                                                     C.c_uint64(0 if x is None else len(x)), C.c_double(tolerance), C.byref(out)))
+        m, ne, N = out.n_kept_views, out.n_kept_edges, out.n
+        nr = 7 * ne
+
+        def unpack(v):
+            return v[:N].copy(), v[N:N + ne].copy(), v[N + ne:N + ne + nr].copy(), v[N + ne + nr:N + ne + 2 * nr].copy()
+
+        d = {"m": m, "ne": ne, "N": N, "view_ids": r["view_ids"][:m].copy(), "edge_record": r["edge_record"][:ne].copy(),
+             "edge_ij": r["edge_ij"][:2 * ne].reshape(ne, 2).copy(), "Rij": r["Rij"][:9 * ne].reshape(ne, 3, 3).copy(),
+             "u": r["u"][:3 * ne].reshape(ne, 3).copy(), "state0": unpack(r["state0"]), "state": unpack(r["state"]),
+             "norms": np.array(out.norms[:]), "A": r["A"][:(N + 1) * N].reshape(N + 1, N).copy(), "sc": r["sc"][:N].copy(),
+             "not_pd": [bool(v) for v in out.not_pd], "retries": out.retries, "sigma": out.sigma,
+             "converged": bool(out.converged), "failed": bool(out.failed)}
+        for ph in ("pred", "corr"):
+            d[ph] = {"dy": r[ph + "_dy"][:N].copy(), "dlam": r[ph + "_dlam"][:ne].copy(), "ds": r[ph + "_ds"][:nr].copy(),
+                     "dz": r[ph + "_dz"][:nr].copy()}
+        d["pred"].update(alpha_p=out.pred_alpha_p, alpha_d=out.pred_alpha_d, complementarity=out.pred_complementarity)
+        d["corr"].update(alpha_p=out.alpha_p, alpha_d=out.alpha_d, rhs=r["corr_rhs"][:N].copy())
+        return d
 
     def relpose_timing(self):
         t = RelposeTiming()

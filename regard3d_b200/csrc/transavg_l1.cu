@@ -412,6 +412,197 @@ __global__ void k_tl_vec(int mode, uint32_t N, const double* __restrict__ sc, do
   }
 }
 
+// The start point, packed as a state (y: T of the free views then gamma, lambda, s, z; the last three in kept-edge
+// order): T = 0, lambda = 2, gamma = 3 (strictly feasible: |u| = 1), s = h - G y, z = 1
+std::vector<double> start_point(const ta::KeptEdges& K, uint32_t N) {
+  const uint32_t ne = (uint32_t)K.kab.size();
+  const size_t nr = (size_t)kRows * ne;
+  std::vector<double> x(N + ne + 2 * nr, 0.0);
+  x[N - 1] = 3.0;
+  double* lam = x.data() + N;
+  double* s = lam + ne;
+  double* z = s + nr;
+  for (uint32_t e = 0; e < ne; ++e) {
+    lam[e] = 2.0;
+    for (int k = 0; k < 3; ++k) {
+      const double r = -2.0 * K.u[3 * (size_t)e + k];
+      s[kRows * (size_t)e + k] = -(r - 3.0);
+      s[kRows * (size_t)e + 3 + k] = -(-r - 3.0);
+    }
+    s[kRows * (size_t)e + 6] = 1.0;
+  }
+  for (size_t i = 0; i < nr; ++i) z[i] = 1.0;
+  return x;
+}
+
+// The device side of one interior-point solve on the kept edges: its buffers and the four phases of an iteration.
+// translation_averaging_l1 runs the phases back to back; r3d_debug_transavg_l1_step runs them once and reads the
+// buffers back between them.
+struct Ipm {
+  r3d_ctx* ctx;
+  DeviceWorker& w;
+  const uint32_t m, ne, N;
+  const size_t nr;
+  const uint32_t eg, ug, vg;
+  DevArr<uint32_t> d_iofs, d_inbr, d_iedge;
+  DevArr<uint2> d_ab;
+  DevArr<double> d_R, d_u, d_y, d_lam, d_s, d_z, d_ds, d_dz, d_dlam, d_ew, d_gg, d_gr, d_nrm, d_ratio, d_rdT, d_A, d_M, d_b, d_sc,
+      d_L, d_Linv, d_x, d_Y, d_Z, d_scal;
+  int trsm_grid = 0;
+  // 0..4 k_tl_norms, 5 not-positive-definite flag, 8..10 k_tl_ratio, 15 gamma
+  double h_scal[16] = {};
+  int not_pd[kRegTries + 1] = {};  // the predictor's factorisation attempts
+  uint32_t retries = 0;
+  double sigma = 0.0;
+
+  Ipm(r3d_ctx* c, DeviceWorker& wk, const ta::KeptEdges& K)
+      : ctx(c), w(wk), m((uint32_t)K.kview.size()), ne((uint32_t)K.kab.size()), N(3 * (m - 1) + 1), nr((size_t)kRows * ne),
+        eg((ne + 127) / 128), ug((std::max(ne, N) + 127) / 128), vg((N + 127) / 128), d_iofs(wk), d_inbr(wk), d_iedge(wk), d_ab(wk),
+        d_R(wk), d_u(wk), d_y(wk), d_lam(wk), d_s(wk), d_z(wk), d_ds(wk), d_dz(wk), d_dlam(wk), d_ew(wk), d_gg(wk), d_gr(wk), d_nrm(wk),
+        d_ratio(wk), d_rdT(wk), d_A(wk), d_M(wk), d_b(wk), d_sc(wk), d_L(wk), d_Linv(wk), d_x(wk), d_Y(wk), d_Z(wk), d_scal(wk) {}
+
+  // the scratch, the kept edges and their incidence lists on the device, the state x (packed as start_point's)
+  int init(const char* fn, const ta::KeptEdges& K, const std::vector<double>& x) {
+    std::vector<uint32_t> inc_ofs, inc_nbr, inc_edge;
+    ra::incidence_lists(m, K.kab, inc_ofs, inc_nbr, inc_edge);
+    const int nblk = ((int)N + kCholNB - 1) / kCholNB;
+    if (!d_iofs.alloc(m + 1) || !d_inbr.alloc(2 * (size_t)ne) || !d_iedge.alloc(2 * (size_t)ne) || !d_ab.alloc(ne) || !d_R.alloc(9 * (size_t)ne) ||
+        !d_u.alloc(3 * (size_t)ne) || !d_y.alloc(N) || !d_lam.alloc(ne) || !d_s.alloc(nr) || !d_z.alloc(nr) || !d_ds.alloc(nr) ||
+        !d_dz.alloc(nr) || !d_dlam.alloc(ne) || !d_ew.alloc((size_t)kEW * ne) || !d_gg.alloc(ne) || !d_gr.alloc(ne) ||
+        !d_nrm.alloc((size_t)kNrm * ne) || !d_ratio.alloc(2 * (size_t)ne) || !d_rdT.alloc(m - 1) || !d_A.alloc((size_t)(N + 1) * N) ||
+        !d_L.alloc((size_t)(N + 1) * N + 64) || !d_Linv.alloc((size_t)nblk * kCholNB * kCholNB) || !d_x.alloc(N) ||
+        !d_Y.alloc(3 * (size_t)N) || !d_Z.alloc(3 * (size_t)N) || !d_M.alloc((size_t)N * N) || !d_b.alloc(N) || !d_sc.alloc(N) ||
+        !d_scal.alloc(16))
+      return fail(ctx, R3D_ERR_NOMEM, std::string(fn) + "device scratch");
+    R3D_CUDA_TRY(ctx, h2d(d_iofs.p, inc_ofs.data(), (m + 1) * sizeof(uint32_t)));
+    R3D_CUDA_TRY(ctx, h2d(d_inbr.p, inc_nbr.data(), inc_nbr.size() * sizeof(uint32_t)));
+    R3D_CUDA_TRY(ctx, h2d(d_iedge.p, inc_edge.data(), inc_edge.size() * sizeof(uint32_t)));
+    R3D_CUDA_TRY(ctx, h2d(d_ab.p, K.ab.data(), ne * sizeof(uint2)));
+    R3D_CUDA_TRY(ctx, h2d(d_R.p, K.Rij.data(), K.Rij.size() * sizeof(double)));
+    R3D_CUDA_TRY(ctx, h2d(d_u.p, K.u.data(), K.u.size() * sizeof(double)));
+    R3D_CUDA_TRY(ctx, h2d(d_y.p, x.data(), N * sizeof(double)));
+    R3D_CUDA_TRY(ctx, h2d(d_lam.p, x.data() + N, ne * sizeof(double)));
+    R3D_CUDA_TRY(ctx, h2d(d_s.p, x.data() + N + ne, nr * sizeof(double)));
+    R3D_CUDA_TRY(ctx, h2d(d_z.p, x.data() + N + ne + nr, nr * sizeof(double)));
+    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_scal.p, 0, 16 * sizeof(double), w.stream));
+    return ra::trsm3_grid(ctx, w, &trsm_grid);
+  }
+
+  cudaError_t h2d(void* dst, const void* src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, w.stream); }
+
+  int read_scal() {
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(h_scal, d_scal.p, sizeof(h_scal), cudaMemcpyDeviceToHost, w.stream));
+    R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+    return R3D_OK;
+  }
+
+  // one step of iterative refinement of the scaled solution in d_x against the unregularised M, b, then unscaled:
+  // x <- sc (x + (L L^T)^-1 (b - M x))
+  int refine() {
+    k_tl_resid<<<(N + 3) / 4, 128, 0, w.stream>>>(d_M.p, d_b.p, d_x.p, N, d_Y.p);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    int rc;
+    if ((rc = ra::trsm3(ctx, w, d_L.p, d_Linv.p, (int)N, d_Y.p, d_Z.p, trsm_grid))) return rc;
+    k_tl_vec<<<vg, 128, 0, w.stream>>>(2, N, d_sc.p, d_Y.p, d_x.p, d_b.p);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    return R3D_OK;
+  }
+
+  // phase 1: the residuals, the reduced system of the current point (the matrix and the predictor's right-hand side
+  // into d_A, unscaled) and the norms (h_scal 0..4, gamma in h_scal 15)
+  int assemble() {
+    k_tl_rows<<<eg, 128, 0, w.stream>>>(0, d_ab.p, d_R.p, d_u.p, d_y.p, d_lam.p, d_s.p, d_z.p, d_ds.p, d_dz.p, 0.0, ne, N, d_ew.p,
+                                        d_gg.p, d_gr.p, d_nrm.p);
+    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_A.p, 0, (size_t)(N + 1) * N * sizeof(double), w.stream));
+    k_tl_system<<<m - 1, 128, 0, w.stream>>>(0, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_R.p, d_ew.p, d_z.p, N, d_A.p,
+                                             d_A.p + (size_t)N * N, 1, d_rdT.p);
+    ra::k_avg_sum<ra::kAvgThreads><<<1, ra::kAvgThreads, 0, w.stream>>>(d_gg.p, ne, d_A.p + (size_t)(N - 1) * N + (N - 1));
+    ra::k_avg_sum<ra::kAvgThreads><<<1, ra::kAvgThreads, 0, w.stream>>>(d_gr.p, ne, d_A.p + (size_t)N * N + (N - 1));
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    k_tl_norms<ra::kAvgThreads><<<1, ra::kAvgThreads, 0, w.stream>>>(d_nrm.p, d_rdT.p, ne, m - 1, d_scal.p);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_scal.p + 15, d_y.p + (N - 1), sizeof(double), cudaMemcpyDeviceToDevice, w.stream));
+    return read_scal();
+  }
+
+  // the stopping test on phase 1's norms (|h|_inf = 1)
+  bool converged(double tol) const {
+    const double pres = h_scal[0], dres = h_scal[2], dobj = h_scal[4], gam = h_scal[15];
+    return pres <= tol * 2.0 && dres <= tol && std::fabs(gam - dobj) <= tol * (1.0 + std::fabs(gam));
+  }
+
+  // one factorisation attempt (reg > 0: of M + reg max(diag) I, from the copy), its solve refined against M, the step
+  // lengths and the complementarity they reach
+  int predictor_attempt(double reg) {
+    if (reg > 0.0) {
+      R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_A.p, d_M.p, (size_t)N * N * sizeof(double), cudaMemcpyDeviceToDevice, w.stream));
+      R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_A.p + (size_t)N * N, d_b.p, N * sizeof(double), cudaMemcpyDeviceToDevice, w.stream));
+      k_tl_regularize<kRThreads><<<1, kRThreads, 0, w.stream>>>(d_A.p, N, reg);
+    }
+    double* scal = d_scal.p;
+    R3D_CUDA_TRY(ctx, cudaMemsetAsync(scal + 5, 0, sizeof(double), w.stream));
+    int rc;
+    if ((rc = dense_cholesky(ctx, w, d_A.p, d_L.p, d_Linv.p, (int)N, scal + 5, d_x.p))) return rc;
+    if ((rc = refine())) return rc;
+    k_tl_back<<<eg, 128, 0, w.stream>>>(d_ab.p, d_R.p, d_u.p, d_ew.p, d_s.p, d_z.p, d_x.p, 1, ne, N, d_dlam.p, d_ds.p, d_dz.p, d_ratio.p);
+    k_tl_ratio<kRThreads><<<1, kRThreads, 0, w.stream>>>(0, d_ratio.p, d_s.p, d_z.p, d_ds.p, d_dz.p, ne, 1.0, scal + 8);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    return read_scal();
+  }
+
+  // phase 2: the system scaled to a unit diagonal (M, b: the unregularised copy), the predictor, and while its
+  // factorisation is not positive definite, again with the diagonal raised.  *failed: every attempt failed.
+  int predictor(bool* failed) {
+    k_tl_jacobi_sc<<<(N + 127) / 128, 128, 0, w.stream>>>(d_A.p, N, d_sc.p);
+    k_tl_jacobi<<<N, 128, 0, w.stream>>>(d_A.p, N, d_sc.p, d_M.p, d_b.p);
+    std::fill(not_pd, not_pd + kRegTries + 1, 0);
+    retries = 0;
+    int rc;
+    if ((rc = predictor_attempt(0.0))) return rc;
+    not_pd[0] = h_scal[5] != 0.0;
+    double reg = kRegRel;
+    for (int k = 0; k < kRegTries && h_scal[5] != 0.0; ++k, reg *= kRegGrowth) {
+      ++retries;
+      if ((rc = predictor_attempt(reg))) return rc;
+      not_pd[k + 1] = h_scal[5] != 0.0;
+    }
+    *failed = h_scal[5] != 0.0;
+    return R3D_OK;
+  }
+
+  // phase 3: sigma = (mu_aff / mu)^3, the corrector through the predictor's factor: the right-hand side with the
+  // predictor's second-order term and sigma mu, its solve refined against M, the step lengths (h_scal 8, 9 after the
+  // next read)
+  int corrector() {
+    const double nrows = (double)nr;
+    const double mu = h_scal[3] / nrows, ratio_mu = (h_scal[10] / nrows) / mu;
+    sigma = (ratio_mu * ratio_mu) * ratio_mu;
+    k_tl_rows<<<eg, 128, 0, w.stream>>>(1, d_ab.p, d_R.p, d_u.p, d_y.p, d_lam.p, d_s.p, d_z.p, d_ds.p, d_dz.p, sigma * mu, ne, N,
+                                        d_ew.p, d_gg.p, d_gr.p, d_nrm.p);
+    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_Y.p, 0, 3 * (size_t)N * sizeof(double), w.stream));
+    k_tl_system<<<m - 1, 128, 0, w.stream>>>(1, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_R.p, d_ew.p, d_z.p, N, d_A.p, d_Y.p, 3,
+                                             d_rdT.p);
+    ra::k_avg_sum<ra::kAvgThreads><<<1, ra::kAvgThreads, 0, w.stream>>>(d_gr.p, ne, d_Y.p + 3 * (size_t)(N - 1));
+    k_tl_vec<<<vg, 128, 0, w.stream>>>(0, N, d_sc.p, d_Y.p, d_x.p, d_b.p);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    int rc;
+    if ((rc = ra::trsm3(ctx, w, d_L.p, d_Linv.p, (int)N, d_Y.p, d_Z.p, trsm_grid))) return rc;
+    k_tl_vec<<<vg, 128, 0, w.stream>>>(1, N, d_sc.p, d_Y.p, d_x.p, d_b.p);
+    if ((rc = refine())) return rc;
+    k_tl_back<<<eg, 128, 0, w.stream>>>(d_ab.p, d_R.p, d_u.p, d_ew.p, d_s.p, d_z.p, d_x.p, 1, ne, N, d_dlam.p, d_ds.p, d_dz.p, d_ratio.p);
+    k_tl_ratio<kRThreads><<<1, kRThreads, 0, w.stream>>>(1, d_ratio.p, d_s.p, d_z.p, d_ds.p, d_dz.p, ne, kEta, d_scal.p + 8);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    return R3D_OK;
+  }
+
+  // phase 4: the step
+  int update() {
+    k_tl_update<<<ug, 128, 0, w.stream>>>(d_scal.p + 8, d_x.p, 1, d_dlam.p, d_ds.p, d_dz.p, ne, N, d_y.p, d_lam.p, d_s.p, d_z.p);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    return R3D_OK;
+  }
+};
+
 int translation_averaging_l1(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use, const double* rot,
                              const uint8_t* rot_kept, uint32_t n_views, const r3d_transavg_l1_options& opt, double* centers,
                              double* translations, uint8_t* view_kept, uint8_t* edge_kept, double* edge_scale,
@@ -441,169 +632,44 @@ int translation_averaging_l1(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_
   for (uint32_t v : K.kview) view_kept[v] = 1;
   if (edge_kept)
     for (uint64_t src : K.src) edge_kept[src] = 1;
-  std::vector<uint32_t> inc_ofs, inc_nbr, inc_edge;
-  ra::incidence_lists(m, K.kab, inc_ofs, inc_nbr, inc_edge);
   // ---- 2. the interior-point method ----
-  const uint32_t N = 3 * (m - 1) + 1;  // free view translations, then gamma
-  const int nblk = ((int)N + kCholNB - 1) / kCholNB;
-  const size_t nr = (size_t)kRows * ne;
-  std::vector<double> y(N, 0.0), lam(ne, 2.0), sz0(nr, 1.0);
-  y[N - 1] = 3.0;
-  std::vector<double> s0(nr);
-  for (uint32_t e = 0; e < ne; ++e) {  // s = h - G y at T = 0, lambda = 2, gamma = 3
-    for (int k = 0; k < 3; ++k) {
-      const double r = -2.0 * K.u[3 * (size_t)e + k];
-      s0[kRows * (size_t)e + k] = -(r - 3.0);
-      s0[kRows * (size_t)e + 3 + k] = -(-r - 3.0);
-    }
-    s0[kRows * (size_t)e + 6] = 1.0;
-  }
-  DevArr<uint32_t> d_iofs(w), d_inbr(w), d_iedge(w);
-  DevArr<uint2> d_ab(w);
-  DevArr<double> d_R(w), d_u(w), d_y(w), d_lam(w), d_s(w), d_z(w), d_ds(w), d_dz(w), d_dlam(w), d_ew(w), d_gg(w), d_gr(w), d_nrm(w),
-      d_ratio(w), d_rdT(w), d_A(w), d_M(w), d_b(w), d_sc(w), d_L(w), d_Linv(w), d_x(w), d_Y(w), d_Z(w), d_scal(w);
-  if (!d_iofs.alloc(m + 1) || !d_inbr.alloc(2 * (size_t)ne) || !d_iedge.alloc(2 * (size_t)ne) || !d_ab.alloc(ne) || !d_R.alloc(9 * (size_t)ne) ||
-      !d_u.alloc(3 * (size_t)ne) || !d_y.alloc(N) || !d_lam.alloc(ne) || !d_s.alloc(nr) || !d_z.alloc(nr) || !d_ds.alloc(nr) ||
-      !d_dz.alloc(nr) || !d_dlam.alloc(ne) || !d_ew.alloc((size_t)kEW * ne) || !d_gg.alloc(ne) || !d_gr.alloc(ne) ||
-      !d_nrm.alloc((size_t)kNrm * ne) || !d_ratio.alloc(2 * (size_t)ne) || !d_rdT.alloc(m - 1) || !d_A.alloc((size_t)(N + 1) * N) ||
-      !d_L.alloc((size_t)(N + 1) * N + 64) || !d_Linv.alloc((size_t)nblk * kCholNB * kCholNB) || !d_x.alloc(N) || !d_Y.alloc(3 * (size_t)N) ||
-      !d_Z.alloc(3 * (size_t)N) || !d_M.alloc((size_t)N * N) || !d_b.alloc(N) || !d_sc.alloc(N) || !d_scal.alloc(16))
-    return fail(ctx, R3D_ERR_NOMEM, std::string(fn) + "device scratch");
-  auto h2d = [&](void* dst, const void* src, size_t bytes) { return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, w.stream); };
-  R3D_CUDA_TRY(ctx, h2d(d_iofs.p, inc_ofs.data(), (m + 1) * sizeof(uint32_t)));
-  R3D_CUDA_TRY(ctx, h2d(d_inbr.p, inc_nbr.data(), inc_nbr.size() * sizeof(uint32_t)));
-  R3D_CUDA_TRY(ctx, h2d(d_iedge.p, inc_edge.data(), inc_edge.size() * sizeof(uint32_t)));
-  R3D_CUDA_TRY(ctx, h2d(d_ab.p, K.ab.data(), ne * sizeof(uint2)));
-  R3D_CUDA_TRY(ctx, h2d(d_R.p, K.Rij.data(), K.Rij.size() * sizeof(double)));
-  R3D_CUDA_TRY(ctx, h2d(d_u.p, K.u.data(), K.u.size() * sizeof(double)));
-  R3D_CUDA_TRY(ctx, h2d(d_y.p, y.data(), N * sizeof(double)));
-  R3D_CUDA_TRY(ctx, h2d(d_lam.p, lam.data(), ne * sizeof(double)));
-  R3D_CUDA_TRY(ctx, h2d(d_s.p, s0.data(), nr * sizeof(double)));
-  R3D_CUDA_TRY(ctx, h2d(d_z.p, sz0.data(), nr * sizeof(double)));
-  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_scal.p, 0, 16 * sizeof(double), w.stream));
-  int trsm_grid = 0;
-  if ((rc = ra::trsm3_grid(ctx, w, &trsm_grid))) return rc;
+  Ipm P(ctx, w, K);
+  const uint32_t N = P.N;  // free view translations, then gamma
+  if ((rc = P.init(fn, K, start_point(K, N)))) return rc;
   Events<2> evt;
   R3D_CUDA_TRY(ctx, evt.create());
   R3D_CUDA_TRY(ctx, cudaEventRecord(evt.e[0], w.stream));
-  const uint32_t eg = (ne + 127) / 128, ug = (std::max(ne, N) + 127) / 128;
-  double* scal = d_scal.p;  // 0..4 k_tl_norms, 5 not-positive-definite flag, 8..10 k_tl_ratio
-  double h_scal[16];
-  auto read_scal = [&]() -> int {
-    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(h_scal, scal, sizeof(h_scal), cudaMemcpyDeviceToHost, w.stream));
-    R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-    return R3D_OK;
-  };
-  // the reduced system of the current point: the matrix and the predictor's right-hand side into the zeroed d_A
-  auto assemble = [&]() -> int {
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_A.p, 0, (size_t)(N + 1) * N * sizeof(double), w.stream));
-    k_tl_system<<<m - 1, 128, 0, w.stream>>>(0, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_R.p, d_ew.p, d_z.p, N, d_A.p,
-                                             d_A.p + (size_t)N * N, 1, d_rdT.p);
-    ra::k_avg_sum<ra::kAvgThreads><<<1, ra::kAvgThreads, 0, w.stream>>>(d_gg.p, ne, d_A.p + (size_t)(N - 1) * N + (N - 1));
-    ra::k_avg_sum<ra::kAvgThreads><<<1, ra::kAvgThreads, 0, w.stream>>>(d_gr.p, ne, d_A.p + (size_t)N * N + (N - 1));
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    return R3D_OK;
-  };
-  // one step of iterative refinement of the scaled solution in d_x against the unregularised M, b, then unscaled:
-  // x <- sc (x + (L L^T)^-1 (b - M x))
-  const uint32_t vg = (N + 127) / 128;
-  auto refine = [&]() -> int {
-    k_tl_resid<<<(N + 3) / 4, 128, 0, w.stream>>>(d_M.p, d_b.p, d_x.p, N, d_Y.p);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    int r2;
-    if ((r2 = ra::trsm3(ctx, w, d_L.p, d_Linv.p, (int)N, d_Y.p, d_Z.p, trsm_grid))) return r2;
-    k_tl_vec<<<vg, 128, 0, w.stream>>>(2, N, d_sc.p, d_Y.p, d_x.p, d_b.p);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    return R3D_OK;
-  };
-  const double tol = opt.tolerance;
-  const double nrows = (double)nr;
   int term = 1;
   uint32_t it = 0, nreg = 0;
-  double gam = 0.0, dobj = 0.0, pviol = 0.0, dres = 0.0;
   for (;; ++it) {
-    // residuals and the predictor's system at the current point
-    k_tl_rows<<<eg, 128, 0, w.stream>>>(0, d_ab.p, d_R.p, d_u.p, d_y.p, d_lam.p, d_s.p, d_z.p, d_ds.p, d_dz.p, 0.0, ne, N, d_ew.p,
-                                        d_gg.p, d_gr.p, d_nrm.p);
-    if ((rc = assemble())) return rc;
-    k_tl_norms<ra::kAvgThreads><<<1, ra::kAvgThreads, 0, w.stream>>>(d_nrm.p, d_rdT.p, ne, m - 1, scal);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(scal + 15, d_y.p + (N - 1), sizeof(double), cudaMemcpyDeviceToDevice, w.stream));
-    if ((rc = read_scal())) return rc;
-    const double pres = h_scal[0], sz = h_scal[3];
-    pviol = h_scal[1];
-    dres = h_scal[2];
-    dobj = h_scal[4];
-    gam = h_scal[15];
-    if (pres <= tol * 2.0 && dres <= tol && std::fabs(gam - dobj) <= tol * (1.0 + std::fabs(gam))) {  // |h|_inf = 1
+    if ((rc = P.assemble())) return rc;
+    if (P.converged(opt.tolerance)) {
       term = 0;
       break;
     }
     if (it == (uint32_t)opt.max_iterations) break;
-    // the system scaled to a unit diagonal (M, b: the unregularised copy)
-    k_tl_jacobi_sc<<<(N + 127) / 128, 128, 0, w.stream>>>(d_A.p, N, d_sc.p);
-    k_tl_jacobi<<<N, 128, 0, w.stream>>>(d_A.p, N, d_sc.p, d_M.p, d_b.p);
-    // predictor: factor (reg > 0: of M + reg max(diag) I, from the copy), solve, refine against M, step lengths and the
-    // complementarity they reach
-    auto predictor = [&](double reg) -> int {
-      if (reg > 0.0) {
-        R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_A.p, d_M.p, (size_t)N * N * sizeof(double), cudaMemcpyDeviceToDevice, w.stream));
-        R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_A.p + (size_t)N * N, d_b.p, N * sizeof(double), cudaMemcpyDeviceToDevice, w.stream));
-        k_tl_regularize<kRThreads><<<1, kRThreads, 0, w.stream>>>(d_A.p, N, reg);
-      }
-      R3D_CUDA_TRY(ctx, cudaMemsetAsync(scal + 5, 0, sizeof(double), w.stream));
-      int r2;
-      if ((r2 = dense_cholesky(ctx, w, d_A.p, d_L.p, d_Linv.p, (int)N, scal + 5, d_x.p))) return r2;
-      if ((r2 = refine())) return r2;
-      k_tl_back<<<eg, 128, 0, w.stream>>>(d_ab.p, d_R.p, d_u.p, d_ew.p, d_s.p, d_z.p, d_x.p, 1, ne, N, d_dlam.p, d_ds.p, d_dz.p,
-                                          d_ratio.p);
-      k_tl_ratio<kRThreads><<<1, kRThreads, 0, w.stream>>>(0, d_ratio.p, d_s.p, d_z.p, d_ds.p, d_dz.p, ne, 1.0, scal + 8);
-      R3D_CUDA_TRY(ctx, cudaGetLastError());
-      return read_scal();
-    };
-    if ((rc = predictor(0.0))) return rc;
-    // not positive definite: again with the diagonal raised
-    double reg = kRegRel;
-    for (int k = 0; k < kRegTries && h_scal[5] != 0.0; ++k, reg *= kRegGrowth) {
-      ++nreg;
-      if ((rc = predictor(reg))) return rc;
-    }
-    if (h_scal[5] != 0.0) {
+    bool failed = false;
+    if ((rc = P.predictor(&failed))) return rc;
+    nreg += P.retries;
+    if (failed) {
       term = 2;
       break;
     }
-    const double mu = sz / nrows, ratio_mu = (h_scal[10] / nrows) / mu;
-    const double sigma = (ratio_mu * ratio_mu) * ratio_mu;
-    // corrector: the same factor, the right-hand side with the predictor's second-order term and sigma mu
-    k_tl_rows<<<eg, 128, 0, w.stream>>>(1, d_ab.p, d_R.p, d_u.p, d_y.p, d_lam.p, d_s.p, d_z.p, d_ds.p, d_dz.p, sigma * mu, ne, N,
-                                        d_ew.p, d_gg.p, d_gr.p, d_nrm.p);
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_Y.p, 0, 3 * (size_t)N * sizeof(double), w.stream));
-    k_tl_system<<<m - 1, 128, 0, w.stream>>>(1, d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, d_R.p, d_ew.p, d_z.p, N, d_A.p, d_Y.p, 3,
-                                             d_rdT.p);
-    ra::k_avg_sum<ra::kAvgThreads><<<1, ra::kAvgThreads, 0, w.stream>>>(d_gr.p, ne, d_Y.p + 3 * (size_t)(N - 1));
-    k_tl_vec<<<vg, 128, 0, w.stream>>>(0, N, d_sc.p, d_Y.p, d_x.p, d_b.p);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    if ((rc = ra::trsm3(ctx, w, d_L.p, d_Linv.p, (int)N, d_Y.p, d_Z.p, trsm_grid))) return rc;
-    k_tl_vec<<<vg, 128, 0, w.stream>>>(1, N, d_sc.p, d_Y.p, d_x.p, d_b.p);
-    if ((rc = refine())) return rc;
-    k_tl_back<<<eg, 128, 0, w.stream>>>(d_ab.p, d_R.p, d_u.p, d_ew.p, d_s.p, d_z.p, d_x.p, 1, ne, N, d_dlam.p, d_ds.p, d_dz.p,
-                                        d_ratio.p);
-    k_tl_ratio<kRThreads><<<1, kRThreads, 0, w.stream>>>(1, d_ratio.p, d_s.p, d_z.p, d_ds.p, d_dz.p, ne, kEta, scal + 8);
-    k_tl_update<<<ug, 128, 0, w.stream>>>(scal + 8, d_x.p, 1, d_dlam.p, d_ds.p, d_dz.p, ne, N, d_y.p, d_lam.p, d_s.p, d_z.p);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    if ((rc = P.corrector()) || (rc = P.update())) return rc;
   }
+  std::vector<double> y(N), lam(ne);
   R3D_CUDA_TRY(ctx, cudaEventRecord(evt.e[1], w.stream));
-  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(y.data(), d_y.p, N * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
-  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(lam.data(), d_lam.p, ne * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(y.data(), P.d_y.p, N * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(lam.data(), P.d_lam.p, ne * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
   S.ms_solve = evt.ms(0, 1);
   S.iterations = it;
   S.regularized_factorizations = nreg;
   S.termination = term;
-  S.gamma = gam;
-  S.dual_objective = dobj;
-  S.max_primal_violation = pviol;
-  S.max_dual_violation = dres;
+  S.gamma = P.h_scal[15];
+  S.dual_objective = P.h_scal[4];
+  S.max_primal_violation = P.h_scal[1];
+  S.max_dual_violation = P.h_scal[2];
   // translations T (the lowest kept view: 0), centres C = -R^T T, the scales of the kept edges
   for (uint32_t a = 0; a < m; ++a) {
     const uint32_t v = K.kview[a];
@@ -620,6 +686,95 @@ int translation_averaging_l1(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_
   S.ms_device_total = S.ms_solve;
   S.ms_host = now_ms() - t0 - S.ms_device_total;
   return R3D_OK;
+}
+
+// r3d_debug_transavg_l1_step: one iteration of the phases above from the state x (or the start point)
+int debug_step(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use, const double* rot,
+               const uint8_t* rot_kept, uint32_t n_views, const double* state, uint64_t n_state, double tolerance,
+               r3d_transavg_l1_step_out& O) {
+  const char* fn = "r3d_debug_transavg_l1_step: ";
+  DeviceWorker& w = ctx->workers[0];
+  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
+  ta::KeptEdges K;
+  int rc = ta::select_edges(ctx, fn, rel, n_rel, edge_use, rot, rot_kept, n_views, K);
+  if (rc) return rc;
+  if (K.kview.empty()) return R3D_OK;
+  const uint32_t m = (uint32_t)K.kview.size(), ne = (uint32_t)K.kab.size(), N = 3 * (m - 1) + 1;
+  const size_t nr = (size_t)kRows * ne, nx = N + ne + 2 * nr;
+  std::vector<double> x;
+  if (!state) {
+    x = start_point(K, N);
+  } else {
+    if (n_state != nx) return fail(ctx, R3D_ERR_INVALID, std::string(fn) + "the state must hold N + 15 x kept edges values");
+    x.assign(state, state + nx);
+    for (size_t i = 0; i < nx; ++i)
+      if (!std::isfinite(x[i])) return fail(ctx, R3D_ERR_INVALID, std::string(fn) + "a non-finite state");
+    for (size_t i = 0; i < nr; ++i)
+      if (!(x[N + ne + i] > 0.0) || !(x[N + ne + nr + i] >= 0.0)) return fail(ctx, R3D_ERR_INVALID, std::string(fn) + "s <= 0 or z < 0");
+  }
+  O.n_kept_views = m;
+  O.n_kept_edges = ne;
+  O.n = N;
+  for (uint32_t a = 0; a < m; ++a)
+    if (O.view_ids) O.view_ids[a] = K.kview[a];
+  for (uint32_t e = 0; e < ne; ++e) {
+    if (O.edge_record) O.edge_record[e] = K.src[e];
+    if (O.edge_ij) {
+      O.edge_ij[2 * (size_t)e] = K.ab[e].x;
+      O.edge_ij[2 * (size_t)e + 1] = K.ab[e].y;
+    }
+  }
+  if (O.Rij) std::memcpy(O.Rij, K.Rij.data(), K.Rij.size() * sizeof(double));
+  if (O.u) std::memcpy(O.u, K.u.data(), K.u.size() * sizeof(double));
+  if (O.state0) std::memcpy(O.state0, x.data(), nx * sizeof(double));
+  Ipm P(ctx, w, K);
+  if ((rc = P.init(fn, K, x))) return rc;
+  auto d2h = [&](double* dst, const double* src, size_t n) -> int {
+    if (dst) R3D_CUDA_TRY(ctx, cudaMemcpyAsync(dst, src, n * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
+    return R3D_OK;
+  };
+  auto d2h_sync = [&]() -> int {
+    R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+    return R3D_OK;
+  };
+  // the step of one phase: the direction of the reduced solve and its back-substitution
+  auto direction = [&](double* dy, double* dlam, double* ds, double* dz) -> int {
+    if ((rc = d2h(dy, P.d_x.p, N)) || (rc = d2h(dlam, P.d_dlam.p, ne)) || (rc = d2h(ds, P.d_ds.p, nr)) || (rc = d2h(dz, P.d_dz.p, nr)))
+      return rc;
+    return d2h_sync();
+  };
+  if ((rc = P.assemble())) return rc;
+  std::memcpy(O.norms, P.h_scal, sizeof(O.norms));
+  if ((rc = d2h(O.A, P.d_A.p, (size_t)(N + 1) * N)) || (rc = d2h_sync())) return rc;
+  if (P.converged(tolerance)) {
+    O.converged = 1;
+    return R3D_OK;
+  }
+  bool failed = false;
+  if ((rc = P.predictor(&failed))) return rc;
+  std::copy(P.not_pd, P.not_pd + kRegTries + 1, O.not_pd);
+  O.retries = P.retries;
+  if ((rc = d2h(O.sc, P.d_sc.p, N)) || (rc = direction(O.pred_dy, O.pred_dlam, O.pred_ds, O.pred_dz))) return rc;
+  O.pred_alpha_p = P.h_scal[8];
+  O.pred_alpha_d = P.h_scal[9];
+  O.pred_complementarity = P.h_scal[10];
+  if (failed) {
+    O.failed = 1;
+    return R3D_OK;
+  }
+  if ((rc = P.corrector())) return rc;
+  O.sigma = P.sigma;
+  if ((rc = d2h(O.corr_rhs, P.d_b.p, N)) || (rc = direction(O.corr_dy, O.corr_dlam, O.corr_ds, O.corr_dz)) || (rc = P.read_scal()))
+    return rc;
+  O.alpha_p = P.h_scal[8];
+  O.alpha_d = P.h_scal[9];
+  if ((rc = P.update())) return rc;
+  if (O.state) {
+    if ((rc = d2h(O.state, P.d_y.p, N)) || (rc = d2h(O.state + N, P.d_lam.p, ne)) || (rc = d2h(O.state + N + ne, P.d_s.p, nr)) ||
+        (rc = d2h(O.state + N + ne + nr, P.d_z.p, nr)))
+      return rc;
+  }
+  return d2h_sync();
 }
 
 }  // namespace tl
@@ -646,4 +801,19 @@ extern "C" int r3d_translation_averaging_l1(r3d_ctx* ctx, const r3d_relative_pos
     return fail(ctx, R3D_ERR_INVALID, "r3d_translation_averaging_l1: max_iterations < 1 or tolerance <= 0");
   return tl::translation_averaging_l1(ctx, rel, n_rel, edge_use, rotations, rot_kept, n_views, *opt, centers, translations, view_kept,
                                       edge_kept, edge_scale, *summary);
+}
+
+extern "C" int r3d_debug_transavg_l1_step(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, const uint8_t* edge_use,
+                                          const double* rotations, const uint8_t* rot_kept, uint32_t n_views, const double* state,
+                                          uint64_t n_state, double tolerance, r3d_transavg_l1_step_out* out) {
+  if (!ctx || (!rel && n_rel) || (n_views && (!rotations || !rot_kept)) || (!state && n_state) || !(tolerance > 0.0) || !out)
+    return fail(ctx, R3D_ERR_INVALID, "r3d_debug_transavg_l1_step: bad arguments");
+  r3d_transavg_l1_step_out& O = *out;
+  O.n_kept_views = O.n_kept_edges = O.n = 0;
+  std::memset(O.norms, 0, sizeof(O.norms));
+  std::memset(O.not_pd, 0, sizeof(O.not_pd));
+  O.retries = 0;
+  O.pred_alpha_p = O.pred_alpha_d = O.pred_complementarity = O.sigma = O.alpha_p = O.alpha_d = 0.0;
+  O.converged = O.failed = 0;
+  return tl::debug_step(ctx, rel, n_rel, edge_use, rotations, rot_kept, n_views, state, n_state, tolerance, O);
 }

@@ -68,9 +68,10 @@ def build_lp(rel, rotations, view_kept, edge_kept):
     return G, h, c, views, recs
 
 
-def solve(G, h, c, n_free, max_iterations=100, tolerance=1e-9):
+def solve(G, h, c, n_free, max_iterations=100, tolerance=1e-9, trace=None):
     """Mehrotra predictor-corrector on min c^T y s.t. G y + s = h, s >= 0; the first n_free coordinates of y are the
-    views' translations, then one lambda per edge (7 rows each), then gamma.  Returns (y, summary dict)."""
+    views' translations, then one lambda per edge (7 rows each), then gamma.  Returns (y, summary dict).  trace: called
+    as trace(iteration, y, s, z) with the state each iteration starts from (the tests take late states from it)."""
     nr, nv = G.shape
     ne = nr // 7
     x_idx = np.r_[np.arange(n_free), nv - 1]          # the dense system: T and gamma
@@ -84,6 +85,8 @@ def solve(G, h, c, n_free, max_iterations=100, tolerance=1e-9):
     hn = np.abs(h).max()
     term, nreg, it = 1, 0, 0
     while True:
+        if trace is not None:
+            trace(it, y.copy(), s.copy(), z.copy())
         rp = G @ y + s - h
         rd = c + Gt @ z
         gam, dobj = y[-1], -h @ z
