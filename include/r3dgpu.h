@@ -374,7 +374,8 @@ int r3d_get_resection_timing(const r3d_ctx* ctx, r3d_resection_timing* out);
 
 /* ---- global rotations from the relative motions (global SfM, second step) ------------------------------------- */
 #define R3D_ROTAVG_L2 0              /* ROTATION_AVERAGING_L2 (src/threads/R3DTriangulationThread.cpp:201) */
-#define R3D_ROTAVG_L1 1              /* ROTATION_AVERAGING_L1: not implemented, R3D_ERR_UNSUPPORTED */
+#define R3D_ROTAVG_L1 1              /* ROTATION_AVERAGING_L1: R3D_ERR_UNSUPPORTED here, solved by
+                                      * r3d_rotation_averaging_l1 */
 #define R3D_ROTAVG_MAX_VIEWS 4096    /* kept views above this (a dense 3n x 3n system): R3D_ERR_UNSUPPORTED */
 typedef struct {
   int method;                        /* R3D_ROTAVG_L2 */
@@ -410,6 +411,40 @@ typedef struct {
 int r3d_rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views,
                            const r3d_rotavg_options* opt, double* rotations, uint8_t* view_kept, uint8_t* edge_kept,
                            uint32_t* edge_support, r3d_rotavg_summary* summary);
+/* ---- global rotations by Regard3D's "L1 rotation averaging (Chatterjee)", ROTATION_AVERAGING_L1 ------------------- */
+typedef struct {
+  double max_angular_error_deg;      /* 5.0: the same TripletRotationRejection as the L2 method */
+  double irls_sigma_deg;             /* 5.0: Geman-McClure scale of the IRLS step (> 0) */
+  int l1_max_iterations;             /* 32: L1RA outer iterations (>= 1) */
+  int irls_max_iterations;           /* 32: IRLS iterations (>= 0; 0 skips IRLS) */
+  double tolerance;                  /* 1e-5: a loop stops when max_v |x_v| (radians) of its last update <= tolerance (> 0) */
+} r3d_rotavg_l1_options;
+void r3d_rotavg_l1_default_options(r3d_rotavg_l1_options* o);  /* 5.0, 5.0, 32, 32, 1e-5 */
+typedef struct {
+  int success;                       /* as r3d_rotavg_summary */
+  uint64_t n_edges, n_triplets, n_valid_triplets, n_kept_edges;
+  uint32_t n_kept_views;
+  uint32_t l1_iterations;            /* L1RA outer iterations run */
+  uint32_t pd_iterations;            /* primal-dual Newton steps, over all L1RA iterations */
+  uint32_t pd_backtracks;            /* rejected trial steps of the primal-dual line search, over all of them */
+  uint32_t irls_iterations;
+  int termination;                   /* of the last loop that ran (IRLS unless skipped): 0 it met the tolerance, 1 its
+                                      * iteration cap, 2 a factorisation was not positive definite (the call returns the
+                                      * rotations reached before it); -1 not run */
+  double initial_l1_cost, final_l1_cost;  /* sum over kept edges of |log(R_j^T R_ij R_i)|_1 at the start and the end */
+  double ms_triplets, ms_init, ms_l1, ms_irls, ms_device_total, ms_host;  /* ms_init: the host spanning tree */
+} r3d_rotavg_l1_summary;
+/* Replaces GlobalSfM_Rotation_AveragingSolver::Run with ROTATION_AVERAGING_L1 (OpenMVG 1.4, reached from
+ * src/threads/R3DTriangulationThread.cpp:201-203 when Regard3D's rotation averaging method is "L1"): Chatterjee &
+ * Govindu's robust rotation averaging.  Inputs, edge rules, triplet rejection, the kept component, error codes, the
+ * R3D_ROTAVG_MAX_VIEWS limit, the gauge (the lowest kept view id gets R = I exactly) and the four outputs are those of
+ * r3d_rotation_averaging; the solver on the kept component differs: a breadth-first spanning tree from the gauge view
+ * (neighbours in ascending order) as the start, then L1RA (per iteration x = argmin |A x - b|_1, b_e = log(R_j^T R_ij
+ * R_i), by l1-magic's primal-dual method, R_v <- R_v exp([x_v]x)), then IRLS with Geman-McClure weights.  Invalid
+ * options: R3D_ERR_INVALID.  One global problem: it runs on the context's first device. */
+int r3d_rotation_averaging_l1(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views,
+                              const r3d_rotavg_l1_options* opt, double* rotations, uint8_t* view_kept, uint8_t* edge_kept,
+                              uint32_t* edge_support, r3d_rotavg_l1_summary* summary);
 /* graph::CleanGraph_KeepLargestBiEdge_Nodes + KeepOnlyReferencedElement on a PairWiseMatches (how upstream's
  * GlobalSfMReconstructionEngine_RelativeMotions::Process() starts): the pairs whose views both lie in the largest
  * 2-edge-connected component of the pair graph (most views; a tie keeps the component holding the smallest view id).

@@ -25,7 +25,7 @@ NVCC_FLAGS = ARCH + [
 # translation units whose floating-point decisions must match the CPU restatement bit for bit are
 # compiled without FMA contraction
 NO_FMAD = {"acransac_kernels.cu", "acransac_fused.cu", "akaze.cu", "liop.cu", "relpose.cu", "resection.cu", "rotavg.cu",
-           "transavg.cu", "transavg_l1.cu"}
+           "rotavg_l1.cu", "transavg.cu", "transavg_l1.cu"}
 
 
 def sources():

@@ -36,7 +36,8 @@ EXPORTS = [
     "r3d_sfm_structure_from_tracks", "r3d_sfm_remove_outliers", "r3d_cascade_prepare", "r3d_debug_cascade_view",
     "r3d_relpose_default_options", "r3d_relative_poses", "r3d_get_relpose_timing",
     "r3d_resection_default_options", "r3d_resect_views", "r3d_sfm_resect_views", "r3d_get_resection_timing",
-    "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_matches_keep_largest_biedge_component",
+    "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_rotavg_l1_default_options", "r3d_rotation_averaging_l1",
+    "r3d_matches_keep_largest_biedge_component",
     "r3d_transavg_default_options", "r3d_translation_averaging", "r3d_transavg_l1_default_options",
     "r3d_translation_averaging_l1", "r3d_debug_transavg_l1_step", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
     "r3d_debug_acransac_score", "r3d_debug_detmath", "r3d_debug_ba_step",
@@ -221,6 +222,20 @@ class RotavgSummary(C.Structure):
                 ("lm_iterations", C.c_uint32), ("lm_successful_steps", C.c_uint32), ("lm_termination", C.c_int),
                 ("lm_initial_cost", C.c_double), ("lm_final_cost", C.c_double), ("ms_triplets", C.c_double),
                 ("ms_init", C.c_double), ("ms_refine", C.c_double), ("ms_device_total", C.c_double), ("ms_host", C.c_double)]
+
+
+class RotavgL1Options(C.Structure):
+    _fields_ = [("max_angular_error_deg", C.c_double), ("irls_sigma_deg", C.c_double), ("l1_max_iterations", C.c_int),
+                ("irls_max_iterations", C.c_int), ("tolerance", C.c_double)]
+
+
+class RotavgL1Summary(C.Structure):
+    _fields_ = [("success", C.c_int), ("n_edges", C.c_uint64), ("n_triplets", C.c_uint64), ("n_valid_triplets", C.c_uint64),
+                ("n_kept_edges", C.c_uint64), ("n_kept_views", C.c_uint32), ("l1_iterations", C.c_uint32),
+                ("pd_iterations", C.c_uint32), ("pd_backtracks", C.c_uint32), ("irls_iterations", C.c_uint32),
+                ("termination", C.c_int), ("initial_l1_cost", C.c_double), ("final_l1_cost", C.c_double),
+                ("ms_triplets", C.c_double), ("ms_init", C.c_double), ("ms_l1", C.c_double), ("ms_irls", C.c_double),
+                ("ms_device_total", C.c_double), ("ms_host", C.c_double)]
 
 
 TRANSAVG_L1, TRANSAVG_L2_CHORDAL, TRANSAVG_SOFTL1 = 1, 2, 3
@@ -1135,6 +1150,28 @@ class Context:
         self._check(lib().r3d_rotation_averaging(self._h, _p(rel), C.c_uint64(len(rel)), C.c_uint32(n_views), C.byref(o), _p(rot),
                                                  _p(vk), _p(ek), _p(sup), C.byref(s)))
         summ = {k: getattr(s, k) for k, _ in RotavgSummary._fields_}
+        return rot[:n_views], vk[:n_views].astype(bool), ek[:len(rel)].astype(bool), sup[:len(rel)].copy(), summ
+
+    def rotation_averaging_l1(self, rel, n_views, **options):
+        """r3d_rotation_averaging_l1 (Regard3D's L1 rotation averaging) on the OK entries of `rel` (relpose_dtype).
+        options: r3d_rotavg_l1_options fields (max_angular_error_deg, irls_sigma_deg, l1_max_iterations,
+        irls_max_iterations, tolerance); the others keep their defaults.  Returns the 5-tuple of rotation_averaging with
+        this method's summary dict."""
+        rel = np.ascontiguousarray(rel, relpose_dtype)
+        o = RotavgL1Options()
+        lib().r3d_rotavg_l1_default_options(C.byref(o))
+        for k, v in options.items():
+            if k not in dict(RotavgL1Options._fields_):
+                raise TypeError("unknown option %r" % k)
+            setattr(o, k, v)
+        rot = np.zeros((max(n_views, 1), 3, 3))
+        vk = np.zeros(max(n_views, 1), np.uint8)
+        ek = np.zeros(max(len(rel), 1), np.uint8)
+        sup = np.zeros(max(len(rel), 1), np.uint32)
+        s = RotavgL1Summary()
+        self._check(lib().r3d_rotation_averaging_l1(self._h, _p(rel), C.c_uint64(len(rel)), C.c_uint32(n_views), C.byref(o),
+                                                    _p(rot), _p(vk), _p(ek), _p(sup), C.byref(s)))
+        summ = {k: getattr(s, k) for k, _ in RotavgL1Summary._fields_}
         return rot[:n_views], vk[:n_views].astype(bool), ek[:len(rel)].astype(bool), sup[:len(rel)].copy(), summ
 
     def translation_averaging(self, rel, rotations, rot_kept, n_views, method=TRANSAVG_L2_CHORDAL, edge_use=None,

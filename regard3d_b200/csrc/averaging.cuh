@@ -54,6 +54,58 @@ __device__ __forceinline__ double val(double x) { return x; }
 template <class T> __device__ __forceinline__ T mk(double x) { return dconst<T::kN>(x); }
 template <> __device__ __forceinline__ double mk<double>(double x) { return x; }
 
+// ---- Ceres' angle-axis conversions, for T = double and T = Dual (rotavg.cu, rotavg_l1.cu) ------------------------
+// ceres::AngleAxisToRotationMatrix (row-major)
+template <class T>
+__device__ void aa_to_R(const T* aa, T* R) {
+  const T th2 = aa[0] * aa[0] + aa[1] * aa[1] + aa[2] * aa[2];
+  if (val(th2) > 2.220446049250313e-16) {
+    const T th = sqrt(th2);
+    const T wx = aa[0] / th, wy = aa[1] / th, wz = aa[2] / th;
+    const T c = cos(th), s = sin(th), oc = 1.0 - c;
+    R[0] = c + wx * wx * oc;      R[1] = wx * wy * oc - wz * s; R[2] = wy * s + wx * wz * oc;
+    R[3] = wz * s + wx * wy * oc; R[4] = c + wy * wy * oc;      R[5] = wy * wz * oc - wx * s;
+    R[6] = wx * wz * oc - wy * s; R[7] = wx * s + wy * wz * oc; R[8] = c + wz * wz * oc;
+  } else {
+    R[0] = mk<T>(1.0); R[1] = -aa[2];     R[2] = aa[1];
+    R[3] = aa[2];      R[4] = mk<T>(1.0); R[5] = -aa[0];
+    R[6] = -aa[1];     R[7] = aa[0];      R[8] = mk<T>(1.0);
+  }
+}
+// ceres::RotationMatrixToAngleAxis: RotationMatrixToQuaternion + QuaternionToAngleAxis (row-major)
+template <class T>
+__device__ void R_to_aa(const T* R, T* aa) {
+  T q[4];
+  const T tr = R[0] + R[4] + R[8];
+  if (val(tr) >= 0.0) {
+    T t = sqrt(tr + 1.0);
+    q[0] = 0.5 * t;
+    t = mk<T>(0.5) / t;
+    q[1] = (R[7] - R[5]) * t;
+    q[2] = (R[2] - R[6]) * t;
+    q[3] = (R[3] - R[1]) * t;
+  } else {
+    int i = 0;
+    if (val(R[4]) > val(R[0])) i = 1;
+    if (val(R[8]) > val(R[4 * i])) i = 2;
+    const int j = (i + 1) % 3, k = (j + 1) % 3;
+    T t = sqrt(R[4 * i] - R[4 * j] - R[4 * k] + 1.0);
+    q[i + 1] = 0.5 * t;
+    t = mk<T>(0.5) / t;
+    q[0] = (R[3 * k + j] - R[3 * j + k]) * t;
+    q[j + 1] = (R[3 * j + i] + R[3 * i + j]) * t;
+    q[k + 1] = (R[3 * k + i] + R[3 * i + k]) * t;
+  }
+  const T s2 = q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
+  if (val(s2) > 0.0) {
+    const T st = sqrt(s2);
+    const T two_theta = 2.0 * (val(q[0]) < 0.0 ? atan2(-st, -q[0]) : atan2(st, q[0]));
+    const T kk = two_theta / st;
+    for (int c = 0; c < 3; ++c) aa[c] = q[c + 1] * kk;
+  } else {
+    for (int c = 0; c < 3; ++c) aa[c] = 2.0 * q[c + 1];
+  }
+}
 // ---- kernels ----------------------------------------------------------------------------------------------------
 // All are templates, so that each translation unit that launches one has its own instance.
 constexpr int kAvgThreads = 256;  // the one-CTA kernels: k_avg_step, k_avg_sum
@@ -158,6 +210,24 @@ __global__ void __launch_bounds__(128, 9) k_avg_grad(int mode, const uint32_t* _
 // remaining edges.  Returns the component with the most nodes (>= 2; a tie keeps the one holding the smallest node), or
 // -1; comp[v] = component of v, -1 for nodes without edges.
 int largest_biedge_component(uint32_t n, const std::vector<uint32_t>& eu, const std::vector<uint32_t>& ev, std::vector<int>& comp);
+
+// rotavg.cu: steps 1 and 2 of both rotation-averaging methods (r3d_rotation_averaging, r3d_rotation_averaging_l1): the
+// OK records checked (I != J, ids < n_views, no unordered pair twice) as canonical edges (min, max), triplet rotation
+// rejection on the device (k_rotavg_triplets), the largest bi-edge-connected component of the supported edges, local
+// ids in view id order (local 0 = the lowest kept view id, the gauge) and the incidence lists.  Zeroes and fills
+// view_kept, edge_kept and edge_support (both may be NULL).  R3D_OK with K.kview empty when no component survives;
+// R3D_ERR_INVALID for a bad record, R3D_ERR_UNSUPPORTED above kMaxTripletNodes nodes or R3D_ROTAVG_MAX_VIEWS kept views;
+// fn prefixes the error messages.
+struct KeptComponent {
+  uint64_t n_edges = 0, n_triplets = 0, n_valid_triplets = 0;
+  double ms_triplets = 0.0;
+  std::vector<uint32_t> kview;                      // kept view ids by local id
+  std::vector<uint2> kab;                           // kept edges (a < b), in (a, b) order
+  std::vector<double> kR;                           // per kept edge R_ab (9, row-major): R_b = R_ab R_a
+  std::vector<uint32_t> inc_ofs, inc_nbr, inc_edge;  // incidence_lists of kab
+};
+int select_component(r3d_ctx* ctx, const char* fn, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views,
+                     double max_angular_error_deg, uint8_t* view_kept, uint8_t* edge_kept, uint32_t* edge_support, KeptComponent& K);
 
 // rotavg.cu: L Lt X = Y in place of Y (n x 3 row-major), Z: n x 3 scratch, with the factor L, Linv of dense_cholesky
 // (one cooperative launch); trsm3_grid resolves grid 0 and checks that the grid can be co-resident.

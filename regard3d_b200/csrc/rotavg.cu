@@ -11,6 +11,7 @@
 //      the cycle trace of R_ik^T R_jk R_ij, a two-tier decision (cos bounds away from the threshold, the exact
 //      float(acos) test inside the band) and integer atomics on the support of its three edges.
 //   2. host: bridges (Tarjan) and the largest 2-edge-connected component of the supported edges, reindexing.
+//      Steps 1 and 2 are select_component, which the L1 method (rotavg_l1.cu) shares.
 //   3. L2 initialisation: M = A^T A assembled by one owner per block row, M + sigma I factored once by k_chol_fused
 //      (ba.cu), block inverse iteration with 3 right-hand sides (k_rotavg_trsm3: blocked forward / backward
 //      substitution, one cooperative launch) and a 3 x 3 Cholesky-QR (k_rotavg_orth), then the sign, the SO(3)
@@ -327,57 +328,6 @@ __global__ void __launch_bounds__(kOThreads) k_rotavg_project(const double* __re
 }
 
 // ---- 4. refinement ----------------------------------------------------------------------------------------------
-// ceres::AngleAxisToRotationMatrix (row-major)
-template <class T>
-__device__ void aa_to_R(const T* aa, T* R) {
-  const T th2 = aa[0] * aa[0] + aa[1] * aa[1] + aa[2] * aa[2];
-  if (val(th2) > 2.220446049250313e-16) {
-    const T th = sqrt(th2);
-    const T wx = aa[0] / th, wy = aa[1] / th, wz = aa[2] / th;
-    const T c = cos(th), s = sin(th), oc = 1.0 - c;
-    R[0] = c + wx * wx * oc;      R[1] = wx * wy * oc - wz * s; R[2] = wy * s + wx * wz * oc;
-    R[3] = wz * s + wx * wy * oc; R[4] = c + wy * wy * oc;      R[5] = wy * wz * oc - wx * s;
-    R[6] = wx * wz * oc - wy * s; R[7] = wx * s + wy * wz * oc; R[8] = c + wz * wz * oc;
-  } else {
-    R[0] = mk<T>(1.0); R[1] = -aa[2];     R[2] = aa[1];
-    R[3] = aa[2];      R[4] = mk<T>(1.0); R[5] = -aa[0];
-    R[6] = -aa[1];     R[7] = aa[0];      R[8] = mk<T>(1.0);
-  }
-}
-// ceres::RotationMatrixToAngleAxis: RotationMatrixToQuaternion + QuaternionToAngleAxis (row-major)
-template <class T>
-__device__ void R_to_aa(const T* R, T* aa) {
-  T q[4];
-  const T tr = R[0] + R[4] + R[8];
-  if (val(tr) >= 0.0) {
-    T t = sqrt(tr + 1.0);
-    q[0] = 0.5 * t;
-    t = mk<T>(0.5) / t;
-    q[1] = (R[7] - R[5]) * t;
-    q[2] = (R[2] - R[6]) * t;
-    q[3] = (R[3] - R[1]) * t;
-  } else {
-    int i = 0;
-    if (val(R[4]) > val(R[0])) i = 1;
-    if (val(R[8]) > val(R[4 * i])) i = 2;
-    const int j = (i + 1) % 3, k = (j + 1) % 3;
-    T t = sqrt(R[4 * i] - R[4 * j] - R[4 * k] + 1.0);
-    q[i + 1] = 0.5 * t;
-    t = mk<T>(0.5) / t;
-    q[0] = (R[3 * k + j] - R[3 * j + k]) * t;
-    q[j + 1] = (R[3 * j + i] + R[3 * i + j]) * t;
-    q[k + 1] = (R[3 * k + i] + R[3 * i + k]) * t;
-  }
-  const T s2 = q[1] * q[1] + q[2] * q[2] + q[3] * q[3];
-  if (val(s2) > 0.0) {
-    const T st = sqrt(s2);
-    const T two_theta = 2.0 * (val(q[0]) < 0.0 ? atan2(-st, -q[0]) : atan2(st, q[0]));
-    const T kk = two_theta / st;
-    for (int c = 0; c < 3; ++c) aa[c] = q[c + 1] * kk;
-  } else {
-    for (int c = 0; c < 3; ++c) aa[c] = 2.0 * q[c + 1];
-  }
-}
 // r = log(R_ab^T R_b R_a^T)^v
 template <class T>
 __device__ void edge_residual(const T* aa_a, const T* aa_b, const double* Rab, T* r) {
@@ -578,32 +528,29 @@ double init_value(uint64_t k) {
   return (double)(z >> 11) * (1.0 / 9007199254740992.0) - 0.5;
 }
 
-int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views, const r3d_rotavg_options& opt,
-                       double* rotations, uint8_t* view_kept, uint8_t* edge_kept, uint32_t* edge_support, r3d_rotavg_summary& S) {
-  const double t0 = now_ms();
+int select_component(r3d_ctx* ctx, const char* fn, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views,
+                     double max_angular_error_deg, uint8_t* view_kept, uint8_t* edge_kept, uint32_t* edge_support, KeptComponent& K) {
   DeviceWorker& w = ctx->workers[0];
-  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
-  std::memset(rotations, 0, (size_t)n_views * 9 * sizeof(double));
   std::memset(view_kept, 0, n_views);
   if (edge_kept) std::memset(edge_kept, 0, n_rel);
   if (edge_support) std::memset(edge_support, 0, n_rel * sizeof(uint32_t));
-  S.lm_termination = -1;
+  const std::string f(fn);
   // ---- 1. edges: canonical (i < j) with R_ij, checked ----
   struct Edge { uint32_t i, j; uint64_t src; };
   std::vector<Edge> edges;
   for (uint64_t k = 0; k < n_rel; ++k) {
     const r3d_relative_pose& r = rel[k];
     if (r.status != R3D_RELPOSE_OK) continue;
-    if (r.I == r.J) return fail(ctx, R3D_ERR_INVALID, "r3d_rotation_averaging: an edge joins a view to itself");
-    if (r.I >= n_views || r.J >= n_views) return fail(ctx, R3D_ERR_INVALID, "r3d_rotation_averaging: view id >= n_views");
+    if (r.I == r.J) return fail(ctx, R3D_ERR_INVALID, f + "an edge joins a view to itself");
+    if (r.I >= n_views || r.J >= n_views) return fail(ctx, R3D_ERR_INVALID, f + "view id >= n_views");
     edges.push_back({std::min(r.I, r.J), std::max(r.I, r.J), k});
   }
-  S.n_edges = edges.size();
+  K.n_edges = edges.size();
   std::sort(edges.begin(), edges.end(), [](const Edge& a, const Edge& b) { return a.i != b.i ? a.i < b.i : a.j < b.j; });
   for (size_t k = 1; k < edges.size(); ++k)
     if (edges[k].i == edges[k - 1].i && edges[k].j == edges[k - 1].j)
-      return fail(ctx, R3D_ERR_INVALID, "r3d_rotation_averaging: the same pair of views is given twice");
-  if (edges.size() > 0xfffffff0ull) return fail(ctx, R3D_ERR_UNSUPPORTED, "r3d_rotation_averaging: too many edges");
+      return fail(ctx, R3D_ERR_INVALID, f + "the same pair of views is given twice");
+  if (edges.size() > 0xfffffff0ull) return fail(ctx, R3D_ERR_UNSUPPORTED, f + "too many edges");
   // nodes: the views with an edge, in id order
   std::vector<uint32_t> node_of(n_views, UINT32_MAX), view_of;
   for (const Edge& e : edges) { node_of[e.i] = 0; node_of[e.j] = 0; }
@@ -611,7 +558,7 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
     if (node_of[v] == 0) { node_of[v] = (uint32_t)view_of.size(); view_of.push_back(v); }
   const uint32_t nn = (uint32_t)view_of.size();
   const uint32_t E = (uint32_t)edges.size();
-  if (nn > kMaxTripletNodes) return fail(ctx, R3D_ERR_UNSUPPORTED, "r3d_rotation_averaging: more than 57344 views with edges");
+  if (nn > kMaxTripletNodes) return fail(ctx, R3D_ERR_UNSUPPORTED, f + "more than 57344 views with edges");
   // upper CSR over the nodes; edge id = position (edges are sorted by (i, j), so the positions are the sorted order)
   std::vector<uint32_t> up_ofs(nn + 1, 0), up_nbr(E);
   std::vector<double> rot_soa((size_t)9 * E);
@@ -625,23 +572,23 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
         rot_soa[(size_t)(3 * a + b) * E + p] = r.I < r.J ? r.rotation[3 * a + b] : r.rotation[3 * b + a];
   }
   for (uint32_t v = 0; v < nn; ++v) up_ofs[v + 1] += up_ofs[v];
-  Events<6> ev;
-  R3D_CUDA_TRY(ctx, ev.create());
   std::vector<uint32_t> support(E, 0);
   if (E) {
+    Events<2> ev;
+    R3D_CUDA_TRY(ctx, ev.create());
     DevArr<uint32_t> d_ofs(w), d_nbr(w), d_sup(w), d_work(w);
     DevArr<double> d_rot(w);
     DevArr<unsigned long long> d_cnt(w);
     if (!d_ofs.alloc(nn + 1) || !d_nbr.alloc(E) || !d_sup.alloc(E) || !d_work.alloc(1) || !d_rot.alloc((size_t)9 * E) || !d_cnt.alloc(2))
-      return fail(ctx, R3D_ERR_NOMEM, "r3d_rotation_averaging: device scratch");
+      return fail(ctx, R3D_ERR_NOMEM, f + "device scratch");
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_ofs.p, up_ofs.data(), (nn + 1) * sizeof(uint32_t), cudaMemcpyHostToDevice, w.stream));
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_nbr.p, up_nbr.data(), E * sizeof(uint32_t), cudaMemcpyHostToDevice, w.stream));
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_rot.p, rot_soa.data(), rot_soa.size() * sizeof(double), cudaMemcpyHostToDevice, w.stream));
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_sup.p, 0, E * sizeof(uint32_t), w.stream));
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_work.p, 0, sizeof(uint32_t), w.stream));
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_cnt.p, 0, 2 * sizeof(unsigned long long), w.stream));
-    const float thr = (float)opt.max_angular_error_deg;
-    const double c_thr = std::cos(opt.max_angular_error_deg * (R3D_PI / 180.0));
+    const float thr = (float)max_angular_error_deg;
+    const double c_thr = std::cos(max_angular_error_deg * (R3D_PI / 180.0));
     const size_t smem = (size_t)nn * sizeof(int32_t);
     R3D_CUDA_TRY(ctx, cudaFuncSetAttribute(k_rotavg_triplets, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)std::max<size_t>(smem, 1)));
     int per_sm = 0;
@@ -656,9 +603,9 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(support.data(), d_sup.p, E * sizeof(uint32_t), cudaMemcpyDeviceToHost, w.stream));
     R3D_CUDA_TRY(ctx, cudaMemcpyAsync(cnt, d_cnt.p, sizeof(cnt), cudaMemcpyDeviceToHost, w.stream));
     R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
-    S.ms_triplets = ev.ms(0, 1);
-    S.n_triplets = cnt[0];
-    S.n_valid_triplets = cnt[1];
+    K.ms_triplets = ev.ms(0, 1);
+    K.n_triplets = cnt[0];
+    K.n_valid_triplets = cnt[1];
   }
   if (edge_support)
     for (uint32_t p = 0; p < E; ++p) edge_support[edges[p].src] = support[p];
@@ -668,35 +615,61 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
     if (support[p]) { eu.push_back(node_of[edges[p].i]); evv.push_back(up_nbr[p]); eid.push_back(p); }
   std::vector<int> comp;
   const int best = largest_biedge_component(nn, eu, evv, comp);
-  if (best < 0) {
+  if (best < 0) return R3D_OK;
+  std::vector<uint32_t> local(nn, UINT32_MAX);  // local index = rank of the view id among the kept views
+  for (uint32_t v = 0; v < nn; ++v)
+    if (comp[v] == best) { local[v] = (uint32_t)K.kview.size(); K.kview.push_back(view_of[v]); }
+  const uint32_t m = (uint32_t)K.kview.size();
+  if (m > R3D_ROTAVG_MAX_VIEWS) {
+    K.kview.clear();
+    return fail(ctx, R3D_ERR_UNSUPPORTED, f + "more than R3D_ROTAVG_MAX_VIEWS views in the component");
+  }
+  for (size_t q = 0; q < eid.size(); ++q) {
+    const uint32_t p = eid[q];
+    const uint32_t a = local[eu[q]], b = local[evv[q]];
+    if (a == UINT32_MAX || b == UINT32_MAX) continue;
+    K.kab.push_back(make_uint2(a, b));
+    for (int c = 0; c < 9; ++c) K.kR.push_back(rot_soa[(size_t)c * E + p]);
+    if (edge_kept) edge_kept[edges[p].src] = 1;
+  }
+  for (uint32_t v : K.kview) view_kept[v] = 1;
+  incidence_lists(m, K.kab, K.inc_ofs, K.inc_nbr, K.inc_edge);
+  return R3D_OK;
+}
+
+int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views, const r3d_rotavg_options& opt,
+                       double* rotations, uint8_t* view_kept, uint8_t* edge_kept, uint32_t* edge_support, r3d_rotavg_summary& S) {
+  const double t0 = now_ms();
+  DeviceWorker& w = ctx->workers[0];
+  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
+  std::memset(rotations, 0, (size_t)n_views * 9 * sizeof(double));
+  S.lm_termination = -1;
+  // ---- 1, 2. the kept component ----
+  KeptComponent K;
+  int rc = select_component(ctx, "r3d_rotation_averaging: ", rel, n_rel, n_views, opt.max_angular_error_deg, view_kept, edge_kept,
+                            edge_support, K);
+  S.n_edges = K.n_edges;
+  S.n_triplets = K.n_triplets;
+  S.n_valid_triplets = K.n_valid_triplets;
+  S.ms_triplets = K.ms_triplets;
+  if (rc) return rc;
+  if (K.kview.empty()) {
     S.success = 0;
     S.ms_device_total = S.ms_triplets;
     S.ms_host = now_ms() - t0 - S.ms_device_total;
     return R3D_OK;
   }
-  std::vector<uint32_t> local(nn, UINT32_MAX), kview;  // local index = rank of the view id among the kept views
-  for (uint32_t v = 0; v < nn; ++v)
-    if (comp[v] == best) { local[v] = (uint32_t)kview.size(); kview.push_back(view_of[v]); }
+  const std::vector<uint32_t>& kview = K.kview;
+  const std::vector<uint2>& kab = K.kab;
+  const std::vector<double>& kR = K.kR;
+  const std::vector<uint32_t>&inc_ofs = K.inc_ofs, &inc_nbr = K.inc_nbr, &inc_edge = K.inc_edge;
   const uint32_t m = (uint32_t)kview.size();
-  if (m > R3D_ROTAVG_MAX_VIEWS)
-    return fail(ctx, R3D_ERR_UNSUPPORTED, "r3d_rotation_averaging: more than R3D_ROTAVG_MAX_VIEWS views in the component");
-  std::vector<uint2> kab;  // kept edges (a < b), in (a, b) order
-  std::vector<double> kR;
-  for (size_t q = 0; q < eid.size(); ++q) {
-    const uint32_t p = eid[q];
-    const uint32_t a = local[eu[q]], b = local[evv[q]];
-    if (a == UINT32_MAX || b == UINT32_MAX) continue;
-    kab.push_back(make_uint2(a, b));
-    for (int c = 0; c < 9; ++c) kR.push_back(rot_soa[(size_t)c * E + p]);
-    if (edge_kept) edge_kept[edges[p].src] = 1;
-  }
   const uint32_t ne = (uint32_t)kab.size();
   S.success = 1;
   S.n_kept_views = m;
   S.n_kept_edges = ne;
-  for (uint32_t v : kview) view_kept[v] = 1;
-  std::vector<uint32_t> inc_ofs, inc_nbr, inc_edge;
-  incidence_lists(m, kab, inc_ofs, inc_nbr, inc_edge);
+  Events<6> ev;
+  R3D_CUDA_TRY(ctx, ev.create());
   uint32_t max_deg = 0;
   for (uint32_t a = 0; a < m; ++a) max_deg = std::max(max_deg, inc_ofs[a + 1] - inc_ofs[a]);
   // ---- 3. L2 initialisation ----
@@ -724,7 +697,6 @@ int rotation_averaging(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_re
     R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
     return R3D_OK;
   };
-  int rc;
   R3D_CUDA_TRY(ctx, cudaEventRecord(ev.e[2], w.stream));
   R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_A.p, 0, (size_t)(N + 1) * N * sizeof(double), w.stream));
   R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_scal.p, 0, 8 * sizeof(double), w.stream));
