@@ -45,7 +45,7 @@ EXPORTS = [
     "r3d_features_get", "r3d_free_features", "r3d_get_akaze_timing", "r3d_debug_akaze_levels",
     "r3d_debug_akaze_refine", "r3d_debug_view_operands",
     "r3d_extract_default_options", "r3d_extract_features", "r3d_features_descriptors", "r3d_save_features",
-    "r3d_get_extract_timing",
+    "r3d_get_extract_timing", "r3d_detect_keypoints", "r3d_extract_features_detector", "r3d_debug_akaze_masks",
 ]
 
 CHOL_DENSE, CHOL_ENVELOPE = 0, 1
@@ -58,6 +58,8 @@ DETMATH_LOG10, DETMATH_CBRT, DETMATH_COS, DETMATH_ACOS = 0, 1, 2, 3
 
 
 AKAZE_DIFF_PM_G2 = 1
+# r3d_detect_keypoints / r3d_extract_features_detector: Regard3D's "Fast-AKAZE" and "AKAZE" detectors
+DETECTOR_FAST_AKAZE, DETECTOR_AKAZE = 0, 1
 # r3d_akaze_keypoint: angle in degrees after Regard3D's conversion; class_id = evolution level
 akaze_keypoint_dtype = np.dtype([("x", np.float32), ("y", np.float32), ("size", np.float32), ("angle", np.float32),
                                  ("response", np.float32), ("octave", np.int32), ("class_id", np.int32)])
@@ -825,17 +827,17 @@ class Context:
                                             _p(kps), C.c_uint32(len(kps)), C.c_float(kp_size_factor), _p(desc)))
         return desc
 
-    def akaze_detect(self, images, **opts):
-        """Fast-AKAZE keypoints of a list of (h, w) float32 gray images in [0, 1]: one akaze_keypoint_dtype array per
-        image, in upstream order."""
+    def akaze_detect(self, images, detector=DETECTOR_FAST_AKAZE, **opts):
+        """Keypoints of a list of (h, w) float32 gray images in [0, 1] by Fast-AKAZE (the default) or, with
+        detector=DETECTOR_AKAZE, by OpenCV's AKAZE: one akaze_keypoint_dtype array per image, in upstream order."""
         imgs = [np.ascontiguousarray(im, np.float32) for im in images]
         n = len(imgs)
         ptrs = (C.c_void_p * max(n, 1))(*[im.ctypes.data for im in imgs])
         ws = np.array([im.shape[1] if im.ndim == 2 else 0 for im in imgs] or [0], np.uint32)
         hs = np.array([im.shape[0] if im.ndim == 2 else 0 for im in imgs] or [0], np.uint32)
         f = C.c_void_p()
-        self._check(lib().r3d_akaze_detect(self._h, ptrs, _p(ws), _p(hs), C.c_uint32(n), C.byref(akaze_options(**opts)),
-                                           C.byref(f)))
+        self._check(lib().r3d_detect_keypoints(self._h, C.c_int(detector), ptrs, _p(ws), _p(hs), C.c_uint32(n),
+                                               C.byref(akaze_options(**opts)), C.byref(f)))
         try:
             out = []
             for i in range(n):
@@ -848,8 +850,10 @@ class Context:
         finally:
             lib().r3d_free_features(f)
 
-    def extract_features(self, images, out_dir=None, basenames=None, threshold=1e-3, kp_size_factor=8.0, progress=None):
-        """Fast-AKAZE keypoints described with LIOP-144, each image uploaded once: one (akaze_keypoint_dtype array,
+    def extract_features(self, images, out_dir=None, basenames=None, threshold=1e-3, kp_size_factor=8.0, progress=None,
+                         detector=DETECTOR_FAST_AKAZE):
+        """Keypoints (Fast-AKAZE by default, or detector=DETECTOR_AKAZE) described with LIOP-144, each image uploaded
+        once: one (akaze_keypoint_dtype array,
         (n, 144) float32) pair per image.  out_dir: also write <out_dir>/<basenames[i]>.feat / .desc; progress(fraction,
         message, user), as compute_matches takes it, runs after each finished image (0.2 + 0.4 done / n)."""
         imgs = [np.ascontiguousarray(im, np.float32) for im in images]
@@ -869,8 +873,8 @@ class Context:
             o.basenames = C.cast(names, C.POINTER(C.c_char_p))
         cb = PROGRESS_CB(progress) if progress else C.cast(None, PROGRESS_CB)
         f = C.c_void_p()
-        self._check(lib().r3d_extract_features(self._h, ptrs, _p(ws), _p(hs), C.c_uint32(n), C.byref(o), cb, None,
-                                               C.byref(f)))
+        self._check(lib().r3d_extract_features_detector(self._h, C.c_int(detector), ptrs, _p(ws), _p(hs), C.c_uint32(n),
+                                                        C.byref(o), cb, None, C.byref(f)))
         try:
             out = []
             for i in range(n):
@@ -933,6 +937,32 @@ class Context:
             d["deleted_lower"] = (flags[c:c + n] & 1).astype(bool)
             d["deleted_upper"] = (flags[c:c + n] & 2).astype(bool)
             c += n
+            out.append(d)
+        return out
+
+    def debug_akaze_masks(self, image, **opts):
+        """One image through the AKAZE detector's kernels: per level a dict with the level record, kcontrast, the five
+        arrays (AKAZE_ARRAYS) and the kept-point masks (bool, level shape) after the same-level, the lower-level and
+        the upper-level passes ("same", "lower", "upper")."""
+        image = np.ascontiguousarray(image, np.float32)
+        h, w = image.shape
+        lv = akaze_levels(w, h, **{k: v for k, v in opts.items() if k != "threshold"})
+        npx = sum(int(l["width"]) * int(l["height"]) for l in lv)
+        arrays = np.zeros(max(5 * npx, 1), np.float32)
+        kc = np.zeros(max(len(lv), 1), np.float32)
+        masks = np.zeros(max(3 * npx, 1), np.uint8)
+        self._check(lib().r3d_debug_akaze_masks(self._h, _p(image), C.c_uint32(w), C.c_uint32(h),
+                                                C.byref(akaze_options(**opts)), _p(arrays), _p(kc), _p(masks)))
+        out, a, m = [], 0, 0
+        for i, l in enumerate(lv):
+            lw, lh = int(l["width"]), int(l["height"])
+            d = {"level": l, "kcontrast": float(kc[i])}
+            for name in AKAZE_ARRAYS:
+                d[name] = arrays[a:a + lw * lh].reshape(lh, lw)
+                a += lw * lh
+            for name in ("same", "lower", "upper"):
+                d[name] = masks[m:m + lw * lh].reshape(lh, lw).astype(bool)
+                m += lw * lh
             out.append(d)
         return out
 

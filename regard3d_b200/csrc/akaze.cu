@@ -1,4 +1,5 @@
-// akaze.cu -- Fast-AKAZE keypoints on the device: Regard3D's default detector (SURVEY.md 3, the feature stage).
+// akaze.cu -- Fast-AKAZE and OpenCV's AKAZE keypoints on the device (SURVEY.md 3, the feature stage): R3DFParams'
+// default detector and the compute-matches dialog's default, on one scale space (the AKAZE passes: DESIGN.md 2.3a).
 // COMPILED WITH --fmad=false (regard3d_b200/build.py): every float operation below rounds like the CPU restatement
 // (oracle/oracle_akaze.cpp), one operation at a time, in the same order, so levels and keypoints agree bit for bit.
 //
@@ -557,6 +558,158 @@ __global__ void k_refine(const LevelRef* refs, int nl, int n_img, KpDev* out, co
   *o = kp;
 }
 
+// ---- AKAZE (cv::AKAZE of OpenCV 4): the same candidates, kept points as per-level masks --------------------------
+// Each (image, level) has three uint8 masks of its pixels: m[0] after the same-level pass, m[1] after the lower-level
+// passes, m[2] after the upper-level passes.  Pass i of either cross-level sweep reads its source level as the
+// previous sweep left it (the next pass that changes that level runs later) and is the only pass that changes its
+// target level, so every pass of a sweep runs at once, one warp per (image, level).
+struct CvRef {
+  const float* det;
+  const int2* cand;  // raster order (k_cand_rows)
+  int n_cand, w, h, r;  // r: sigma_size
+  float ratio, size;
+  int octave, level;
+  uint8_t* m[3];
+};
+
+// find_neighbor_point: the first set pixel in row-major order of the window [y - R, y + R) x [x - R, x + R) with
+// dx^2 + dy^2 <= R^2; lanes test 32 window cells at a time, the lowest set ballot bit is the first hit.  -1: none.
+__device__ __forceinline__ int cv_find(const uint8_t* m, int w, int x, int y, int R, int lane) {
+  const int side = 2 * R, n = side * side;
+  for (int base = 0; base < n; base += 32) {
+    const int k = base + lane, dy = k / side - R, dx = k % side - R;
+    const bool hit = k < n && dx * dx + dy * dy <= R * R && m[(size_t)(y + dy) * w + x + dx] != 0;
+    const unsigned b = __ballot_sync(0xffffffffu, hit);
+    if (b) {
+      const int f = base + __ffs(b) - 1;
+      return (y + f / side - R) * w + x + f % side - R;
+    }
+  }
+  return -1;
+}
+
+// the same-level pass: candidates in raster order; a candidate with a kept point in its window replaces that point
+// when stronger and is dropped otherwise; without one it is kept
+__global__ void k_cv_same(const CvRef* refs, int n_refs) {
+  const int r = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32, lane = threadIdx.x & 31;
+  if (r >= n_refs) return;
+  const CvRef L = refs[r];
+  for (int c = 0; c < L.n_cand; ++c) {
+    const int2 q = L.cand[c];
+    const int p = q.y * L.w + q.x;
+    const int hit = cv_find(L.m[0], L.w, q.x, q.y, L.r, lane);
+    if (lane == 0) {
+      if (hit < 0) {
+        L.m[0][p] = 1;
+      } else if (L.det[p] > L.det[hit]) {
+        L.m[0][hit] = 0;
+        L.m[0][p] = 1;
+      }
+    }
+    __syncwarp();
+  }
+}
+
+// the lower-level pass i (i >= 1): each point of level i, in raster order, looks at (x, y) * diff_ratio in level
+// i - 1 within sigma_size_i * diff_ratio and clears the point found there when that one is weaker
+__global__ void k_cv_lower(const CvRef* refs, int nl, int n_img, const int* n_levels) {
+  const int t = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32, lane = threadIdx.x & 31;
+  const int b = t / nl, i = t % nl;
+  if (b >= n_img || i < 1 || i >= n_levels[b]) return;
+  const CvRef S = refs[b * nl + i], T = refs[b * nl + i - 1];
+  const int dr = (int)(S.ratio / T.ratio), R = S.r * dr;
+  for (int c = 0; c < S.n_cand; ++c) {
+    const int2 q = S.cand[c];
+    const int p = q.y * S.w + q.x;
+    if (!S.m[0][p]) continue;
+    const int hit = cv_find(T.m[1], T.w, q.x * dr, q.y * dr, R, lane);
+    if (lane == 0 && hit >= 0 && S.det[p] > T.det[hit]) T.m[1][hit] = 0;
+    __syncwarp();
+  }
+}
+
+// the upper-level pass i (i <= levels - 2): each point of level i looks at (x, y) / diff_ratio in level i + 1 within
+// sigma_size_(i+1) and clears the point found there when that one is weaker
+__global__ void k_cv_upper(const CvRef* refs, int nl, int n_img, const int* n_levels) {
+  const int t = blockIdx.x * (blockDim.x / 32) + threadIdx.x / 32, lane = threadIdx.x & 31;
+  const int b = t / nl, i = t % nl;
+  if (b >= n_img || i + 1 >= n_levels[b]) return;
+  const CvRef S = refs[b * nl + i], T = refs[b * nl + i + 1];
+  const int dr = (int)(T.ratio / S.ratio);
+  for (int c = 0; c < S.n_cand; ++c) {
+    const int2 q = S.cand[c];
+    const int p = q.y * S.w + q.x;
+    if (!S.m[1][p]) continue;
+    const int hit = cv_find(T.m[2], T.w, q.x / dr, q.y / dr, T.r, lane);
+    if (lane == 0 && hit >= 0 && S.det[p] > T.det[hit]) T.m[2][hit] = 0;
+    __syncwarp();
+  }
+}
+
+// Do_Subpixel_Refinement of cv::AKAZE on every candidate still set in m[2]: the 2x2 solve of k_refine, then
+// x = (x + dx) ratio + 0.5 (ratio - 1); out.class_id = -1 marks a cleared or rejected candidate
+__global__ void k_cv_refine(const CvRef* refs, int nl, int n_img, KpDev* out, const int* out_ofs) {
+  const int b = blockIdx.z, i = blockIdx.y;
+  if (b >= n_img) return;
+  const CvRef L = refs[b * nl + i];
+  const int j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= L.n_cand) return;
+  KpDev* o = out + out_ofs[b * nl + i] + j;
+  const int x = L.cand[j].x, y = L.cand[j].y, cols = L.w;
+  const float* l = L.det;
+  if (!L.m[2][y * cols + x]) {
+    o->class_id = -1;
+    return;
+  }
+  const float Dx = 0.5f * (l[y * cols + x + 1] - l[y * cols + x - 1]);
+  const float Dy = 0.5f * (l[(y + 1) * cols + x] - l[(y - 1) * cols + x]);
+  const float Dxx = l[y * cols + x + 1] + l[y * cols + x - 1] - 2.0f * l[y * cols + x];
+  const float Dyy = l[(y + 1) * cols + x] + l[(y - 1) * cols + x] - 2.0f * l[y * cols + x];
+  const float Dxy = 0.25f * (l[(y + 1) * cols + x + 1] + l[(y - 1) * cols + x - 1] - l[(y - 1) * cols + x + 1] -
+                             l[(y + 1) * cols + x - 1]);
+  const float b0 = -Dx, b1 = -Dy;
+  float dx = 0.0f, dy = 0.0f;
+  double d = (double)Dxx * Dyy - (double)Dxy * Dxy;
+  if (d != 0.0) {
+    d = 1.0 / d;
+    dx = (float)(((double)b0 * Dyy - (double)b1 * Dxy) * d);
+    dy = (float)(((double)b1 * Dxx - (double)b0 * Dxy) * d);
+  }
+  if (fabsf(dx) > 1.0f || fabsf(dy) > 1.0f) {
+    o->class_id = -1;
+    return;
+  }
+  KpDev kp;
+  kp.x = ((float)x + dx) * L.ratio + 0.5f * (L.ratio - 1.0f);
+  kp.y = ((float)y + dy) * L.ratio + 0.5f * (L.ratio - 1.0f);
+  kp.size = L.size * 2.0f;
+  kp.angle = 0.0f;
+  kp.response = l[y * cols + x];
+  kp.octave = L.octave;
+  kp.class_id = L.level;
+  *o = kp;
+}
+
+__host__ __device__ __forceinline__ float fast_atan2_deg(float y, float x) {  // hal::fastAtan2 (fastAtan32f), degrees
+  const float r2d = (float)(180 / kPi);
+  const float p1 = 0.9997878412794807f * r2d, p3 = -0.3258083974640975f * r2d, p5 = 0.1555786518463281f * r2d,
+              p7 = -0.04432655554792128f * r2d;
+  const float ax = fabsf(x), ay = fabsf(y);
+  float a, c, c2;
+  if (ax >= ay) {
+    c = ay / (ax + (float)DBL_EPSILON);
+    c2 = c * c;
+    a = (((p7 * c2 + p5) * c2 + p3) * c2 + p1) * c;
+  } else {
+    c = ax / (ay + (float)DBL_EPSILON);
+    c2 = c * c;
+    a = 90.f - (((p7 * c2 + p5) * c2 + p3) * c2 + p1) * c;
+  }
+  if (x < 0) a = 180.f - a;
+  if (y < 0) a = 360.f - a;
+  return a;
+}
+
 __device__ __forceinline__ float fast_atan2(float y, float x) {  // hal::fastAtan2 (OpenCV 4.x fastAtan32f), radians
   const float r2d = (float)(180 / kPi);
   const float p1 = 0.9997878412794807f * r2d, p3 = -0.3258083974640975f * r2d, p5 = 0.1555786518463281f * r2d,
@@ -694,11 +847,12 @@ size_t image_bytes(const Image& im) {
   return (5 * px + 10 * (size_t)im.W * im.H) * 4 + 4096;
 }
 
-struct Debug {  // r3d_debug_akaze_levels' outputs (batch of one image)
+struct Debug {  // r3d_debug_akaze_levels' / r3d_debug_akaze_masks' outputs (batch of one image)
   float *arrays, *kcontrast;
-  r3d_akaze_keypoint* cands;
+  r3d_akaze_keypoint* cands;  // Fast-AKAZE
   uint8_t* flags;
   uint32_t cap, *counts;
+  uint8_t* masks;  // AKAZE: per level, the three masks
 };
 
 constexpr int kStages = 6;  // upload, scale space, candidates, same-level pass, cross-level passes, refine + orient
@@ -726,7 +880,7 @@ struct Pending {
 
 // One batch of images on one device.  kps[b]: the image's keypoints on return.  keep: hand the original images to
 // keep->held / keep->S instead of releasing them.
-int run_batch(r3d_ctx* ctx, DeviceWorker& w, std::vector<Image*>& imgs, float threshold,
+int run_batch(r3d_ctx* ctx, DeviceWorker& w, std::vector<Image*>& imgs, float threshold, int detector,
               std::vector<std::vector<r3d_akaze_keypoint>*>& kps_out, const Debug* dbg, double* stage_ms,
               uint32_t* launches, Pending* keep = nullptr) {
   const int B = (int)imgs.size();
@@ -1072,30 +1226,85 @@ int run_batch(r3d_ctx* ctx, DeviceWorker& w, std::vector<Image*>& imgs, float th
       R.cell = R.size * 1.0625f;
     }
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_refs, refs.data(), refs.size() * sizeof(LevelRef), cudaMemcpyHostToDevice, st));
-  R3D_CUDA_TRY(ctx, cudaEventRecord(T.e[3], st));
-  k_same_level<<<(B * nl + 3) / 4, 128, 0, st>>>(d_refs, B * nl);
-  ++nlaunch;
-  R3D_CUDA_TRY(ctx, cudaGetLastError());
-  R3D_CUDA_TRY(ctx, cudaEventRecord(T.e[4], st));
   std::vector<int> nkp_h(B * nl);
-  R3D_CUDA_TRY(ctx, cudaMemcpyAsync(nkp_h.data(), d_nkp, nkp_h.size() * 4, cudaMemcpyDeviceToHost, st));
-  R3D_CUDA_TRY(ctx, cudaStreamSynchronize(st));
-  int max_kp = 1;
-  for (int v : nkp_h) max_kp = std::max(max_kp, v);
-  R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_flags, 0, (size_t)std::max(n_cand, 1), st));
-  if (nl > 1) {
-    k_lower<<<dim3((max_kp + 127) / 128, nl - 1, B), 128, 0, st>>>(d_refs, nl, B);
+  uint8_t* d_mask = nullptr;
+  std::vector<size_t> mask_ofs(B * nl + 1, 0);  // AKAZE: each (image, level)'s pixels in one mask
+  if (detector == R3D_DETECTOR_AKAZE) {
+    for (int b = 0; b < B; ++b)
+      for (int l = 0; l < nl; ++l) {
+        const int r = b * nl + l;
+        const bool has = l < (int)imgs[b]->lv.size();
+        mask_ofs[r + 1] = mask_ofs[r] + (has ? (size_t)imgs[b]->lv[l].width * imgs[b]->lv[l].height : 0);
+      }
+    const size_t mp = std::max<size_t>(mask_ofs.back(), 1);
+    d_mask = (uint8_t*)alloc(3 * mp);
+    CvRef* d_cv = (CvRef*)alloc((size_t)B * nl * sizeof(CvRef));
+    int* d_nlev = (int*)alloc((size_t)B * 4);
+    if (!d_mask || !d_cv || !d_nlev) return fail(ctx, R3D_ERR_NOMEM, "r3d_detect_keypoints: device allocation failed");
+    std::vector<CvRef> cv(B * nl);
+    std::vector<int> nlev(B);
+    for (int b = 0; b < B; ++b) {
+      nlev[b] = (int)imgs[b]->lv.size();
+      for (int l = 0; l < nl; ++l) {
+        const int r = b * nl + l;
+        CvRef& R = cv[r];
+        R = CvRef{};
+        for (int k = 0; k < 3; ++k) R.m[k] = d_mask + k * mp + mask_ofs[r];
+        R.cand = d_cand + cand_ofs[r];
+        R.n_cand = cand_ofs[r + 1] - cand_ofs[r];
+        nkp_h[r] = R.n_cand;
+        if (l >= nlev[b]) continue;
+        const r3d_akaze_level& L = imgs[b]->lv[l];
+        R.det = M[b].Ldet[l], R.w = L.width, R.h = L.height, R.r = L.sigma_size;
+        R.ratio = L.ratio, R.size = L.esigma * kDerivFactor, R.octave = L.octave, R.level = l;
+      }
+    }
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_cv, cv.data(), cv.size() * sizeof(CvRef), cudaMemcpyHostToDevice, st));
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_nlev, nlev.data(), (size_t)B * 4, cudaMemcpyHostToDevice, st));
+    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_mask, 0, mp, st));
+    R3D_CUDA_TRY(ctx, cudaEventRecord(T.e[3], st));
+    const unsigned warps = (unsigned)(B * nl + 3) / 4;
+    k_cv_same<<<warps, 128, 0, st>>>(d_cv, B * nl);
     ++nlaunch;
-  }
-  k_upper<<<dim3((max_kp + 127) / 128, nl, B), 128, 0, st>>>(d_refs, nl, B);
-  ++nlaunch;
-  R3D_CUDA_TRY(ctx, cudaGetLastError());
-  R3D_CUDA_TRY(ctx, cudaEventRecord(T.e[5], st));
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    R3D_CUDA_TRY(ctx, cudaEventRecord(T.e[4], st));
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_mask + mp, d_mask, mp, cudaMemcpyDeviceToDevice, st));
+    k_cv_lower<<<warps, 128, 0, st>>>(d_cv, nl, B, d_nlev);
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(d_mask + 2 * mp, d_mask + mp, mp, cudaMemcpyDeviceToDevice, st));
+    k_cv_upper<<<warps, 128, 0, st>>>(d_cv, nl, B, d_nlev);
+    nlaunch += 2;
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    R3D_CUDA_TRY(ctx, cudaEventRecord(T.e[5], st));
+    int max_c = 1;
+    for (int v : nkp_h) max_c = std::max(max_c, v);
+    k_cv_refine<<<dim3((max_c + 127) / 128, nl, B), 128, 0, st>>>(d_cv, nl, B, d_ref, d_cofs);
+    ++nlaunch;
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+  } else {
+    R3D_CUDA_TRY(ctx, cudaEventRecord(T.e[3], st));
+    k_same_level<<<(B * nl + 3) / 4, 128, 0, st>>>(d_refs, B * nl);
+    ++nlaunch;
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    R3D_CUDA_TRY(ctx, cudaEventRecord(T.e[4], st));
+    R3D_CUDA_TRY(ctx, cudaMemcpyAsync(nkp_h.data(), d_nkp, nkp_h.size() * 4, cudaMemcpyDeviceToHost, st));
+    R3D_CUDA_TRY(ctx, cudaStreamSynchronize(st));
+    int max_kp = 1;
+    for (int v : nkp_h) max_kp = std::max(max_kp, v);
+    R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_flags, 0, (size_t)std::max(n_cand, 1), st));
+    if (nl > 1) {
+      k_lower<<<dim3((max_kp + 127) / 128, nl - 1, B), 128, 0, st>>>(d_refs, nl, B);
+      ++nlaunch;
+    }
+    k_upper<<<dim3((max_kp + 127) / 128, nl, B), 128, 0, st>>>(d_refs, nl, B);
+    ++nlaunch;
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    R3D_CUDA_TRY(ctx, cudaEventRecord(T.e[5], st));
 
-  // ---- refinement, orientation ----
-  k_refine<<<dim3((max_kp + 127) / 128, nl, B), 128, 0, st>>>(d_refs, nl, B, d_ref, d_cofs);
-  ++nlaunch;
-  R3D_CUDA_TRY(ctx, cudaGetLastError());
+    // ---- refinement, orientation ----
+    k_refine<<<dim3((max_kp + 127) / 128, nl, B), 128, 0, st>>>(d_refs, nl, B, d_ref, d_cofs);
+    ++nlaunch;
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+  }
   std::vector<KpDev> ref_h(n_cand);
   R3D_CUDA_TRY(ctx, cudaMemcpyAsync(ref_h.data(), d_ref, (size_t)n_cand * sizeof(KpDev), cudaMemcpyDeviceToHost, st));
   R3D_CUDA_TRY(ctx, cudaStreamSynchronize(st));
@@ -1129,7 +1338,8 @@ int run_batch(r3d_ctx* ctx, DeviceWorker& w, std::vector<Image*>& imgs, float th
   for (int k = 0; k < nf; ++k) {
     r3d_akaze_keypoint o;
     std::memcpy(&o, &fin[k], sizeof(o));
-    o.angle = regard3d_angle(ori[k].x, ori[k].y);
+    // cv::AKAZE keeps fastAtan2's degrees; Regard3D converts only Fast-AKAZE's getAngleV2 radians
+    o.angle = detector == R3D_DETECTOR_AKAZE ? fast_atan2_deg(ori[k].y, ori[k].x) : regard3d_angle(ori[k].x, ori[k].y);
     kps_out[fin_img[k]]->push_back(o);
   }
   for (int s = 0; s < kStages; ++s) {
@@ -1152,6 +1362,17 @@ int run_batch(r3d_ctx* ctx, DeviceWorker& w, std::vector<Image*>& imgs, float th
     std::vector<float> kc((size_t)kMaxBatch * nl);
     R3D_CUDA_TRY(ctx, cudaMemcpy(kc.data(), d_kc, kc.size() * 4, cudaMemcpyDeviceToHost));
     for (int l = 0; l < nl; ++l) dbg->kcontrast[l] = nl > 1 ? kc[l * kMaxBatch] : 0.0f;
+    if (dbg->masks) {
+      const size_t mp = std::max<size_t>(mask_ofs.back(), 1);
+      uint8_t* m = dbg->masks;
+      for (int l = 0; l < nl; ++l)
+        for (int k = 0; k < 3; ++k) {
+          const size_t lp = mask_ofs[l + 1] - mask_ofs[l];
+          R3D_CUDA_TRY(ctx, cudaMemcpy(m, d_mask + k * mp + mask_ofs[l], lp, cudaMemcpyDeviceToHost));
+          m += lp;
+        }
+      return R3D_OK;
+    }
     size_t total = 0;
     for (int l = 0; l < nl; ++l) total += nkp_h[l];
     if (total > dbg->cap) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_akaze_levels: more candidates than cand_cap");
@@ -1166,6 +1387,8 @@ int run_batch(r3d_ctx* ctx, DeviceWorker& w, std::vector<Image*>& imgs, float th
   }
   return R3D_OK;
 }
+
+bool known_detector(int detector) { return detector == R3D_DETECTOR_FAST_AKAZE || detector == R3D_DETECTOR_AKAZE; }
 
 int check_options(const r3d_akaze_options* opt) {
   return opt && std::isfinite(opt->threshold) && opt->octaves >= 1 && opt->octaves <= 8 && opt->sublevels >= 1 &&
@@ -1322,7 +1545,7 @@ struct Acc {  // one device's share of a call
 // contiguous slices; each device runs its slice in batches of at most kMaxBatch images and half its free memory, on a
 // host thread of its own.  With X, batch b's descriptors are computed on the second stream while batch b + 1 builds its
 // scale space, and W[d] writes the files.
-int run_devices(r3d_ctx* ctx, std::vector<Image>& ims, float threshold, r3d_features& F, const Extract* X,
+int run_devices(r3d_ctx* ctx, std::vector<Image>& ims, float threshold, int detector, r3d_features& F, const Extract* X,
                 std::vector<std::unique_ptr<Writer>>* W, std::vector<Acc>& acc) {
   const uint32_t n_images = (uint32_t)ims.size();
   const int nd = (int)acc.size();
@@ -1385,7 +1608,7 @@ int run_devices(r3d_ctx* ctx, std::vector<Image>& ims, float threshold, r3d_feat
       }
       cur.i1 = i;
       if (!work.empty() &&
-          (A.rc = run_batch(ctx, w, work, threshold, wout, nullptr, A.ms, &A.launches, X ? &cur : nullptr)))
+          (A.rc = run_batch(ctx, w, work, threshold, detector, wout, nullptr, A.ms, &A.launches, X ? &cur : nullptr)))
         return;
       ++A.batches;
       if (!X) continue;
@@ -1428,11 +1651,12 @@ extern "C" int r3d_akaze_levels(uint32_t width, uint32_t height, const r3d_akaze
   return (int)lv.size();
 }
 
-extern "C" int r3d_akaze_detect(r3d_ctx* ctx, const float* const* images, const uint32_t* widths,
-                                const uint32_t* heights, uint32_t n_images, const r3d_akaze_options* opt,
-                                r3d_features** out) {
+extern "C" int r3d_detect_keypoints(r3d_ctx* ctx, int detector, const float* const* images, const uint32_t* widths,
+                                    const uint32_t* heights, uint32_t n_images, const r3d_akaze_options* opt,
+                                    r3d_features** out) {
   if (!out) return fail(ctx, R3D_ERR_INVALID, "r3d_akaze_detect: out is NULL");
   *out = nullptr;
+  if (!akaze::known_detector(detector)) return fail(ctx, R3D_ERR_INVALID, "r3d_detect_keypoints: unknown detector");
   std::vector<akaze::Image> ims;
   int rc = akaze::prepare(ctx, images, widths, heights, n_images, opt, ims);
   if (rc) return rc;
@@ -1441,7 +1665,7 @@ extern "C" int r3d_akaze_detect(r3d_ctx* ctx, const float* const* images, const 
   F->kps.resize(n_images);
   const int nd = (int)std::min<size_t>(ctx->workers.size(), std::max<uint32_t>(n_images, 1));
   std::vector<akaze::Acc> acc(nd);
-  if ((rc = akaze::run_devices(ctx, ims, opt->threshold, *F, nullptr, nullptr, acc))) return rc;
+  if ((rc = akaze::run_devices(ctx, ims, opt->threshold, detector, *F, nullptr, nullptr, acc))) return rc;
   r3d_akaze_timing T{};
   for (const akaze::Acc& A : acc) {
     T.upload_ms += A.ms[0], T.scale_space_ms += A.ms[1], T.candidates_ms += A.ms[2], T.same_level_ms += A.ms[3];
@@ -1455,6 +1679,12 @@ extern "C" int r3d_akaze_detect(r3d_ctx* ctx, const float* const* images, const 
   ctx->akaze_timing = T;
   *out = F.release();
   return R3D_OK;
+}
+
+extern "C" int r3d_akaze_detect(r3d_ctx* ctx, const float* const* images, const uint32_t* widths,
+                                const uint32_t* heights, uint32_t n_images, const r3d_akaze_options* opt,
+                                r3d_features** out) {
+  return r3d_detect_keypoints(ctx, R3D_DETECTOR_FAST_AKAZE, images, widths, heights, n_images, opt, out);
 }
 
 extern "C" uint32_t r3d_features_num_images(const r3d_features* f) { return f ? (uint32_t)f->kps.size() : 0; }
@@ -1480,10 +1710,13 @@ extern "C" void r3d_extract_default_options(r3d_extract_options* out) {
   out->basenames = nullptr;
 }
 
-extern "C" int r3d_extract_features(r3d_ctx* ctx, const float* const* images, const uint32_t* widths,
-                                    const uint32_t* heights, uint32_t n_images, const r3d_extract_options* opt,
-                                    r3d_progress_cb cb, void* user, r3d_features** out) {
+extern "C" int r3d_extract_features_detector(r3d_ctx* ctx, int detector, const float* const* images,
+                                             const uint32_t* widths, const uint32_t* heights, uint32_t n_images,
+                                             const r3d_extract_options* opt, r3d_progress_cb cb, void* user,
+                                             r3d_features** out) {
   if (out) *out = nullptr;
+  if (!akaze::known_detector(detector))
+    return fail(ctx, R3D_ERR_INVALID, "r3d_extract_features_detector: unknown detector");
   if (!opt || !std::isfinite(opt->kp_size_factor) || opt->kp_size_factor <= 0.0f)
     return fail(ctx, R3D_ERR_INVALID, "r3d_extract_features: bad options");
   const bool files = opt->out_dir != nullptr;
@@ -1521,7 +1754,7 @@ extern "C" int r3d_extract_features(r3d_ctx* ctx, const float* const* images, co
       wr->th = std::thread([wr, &F, &X] { wr->run(*F, X); });
     }
   std::vector<akaze::Acc> acc(nd);
-  rc = akaze::run_devices(ctx, ims, opt->akaze.threshold, *F, &X, files ? &W : nullptr, acc);
+  rc = akaze::run_devices(ctx, ims, opt->akaze.threshold, detector, *F, &X, files ? &W : nullptr, acc);
   r3d_extract_timing T{};
   for (std::unique_ptr<akaze::Writer>& wr : W) {
     wr->close();
@@ -1541,6 +1774,13 @@ extern "C" int r3d_extract_features(r3d_ctx* ctx, const float* const* images, co
   ctx->extract_timing = T;
   if (out) *out = F.release();
   return R3D_OK;
+}
+
+extern "C" int r3d_extract_features(r3d_ctx* ctx, const float* const* images, const uint32_t* widths,
+                                    const uint32_t* heights, uint32_t n_images, const r3d_extract_options* opt,
+                                    r3d_progress_cb cb, void* user, r3d_features** out) {
+  return r3d_extract_features_detector(ctx, R3D_DETECTOR_FAST_AKAZE, images, widths, heights, n_images, opt, cb, user,
+                                       out);
 }
 
 extern "C" const float* r3d_features_descriptors(const r3d_features* f, uint32_t image) {
@@ -1568,10 +1808,29 @@ extern "C" int r3d_debug_akaze_levels(r3d_ctx* ctx, const float* image, uint32_t
   std::vector<akaze::Image*> batch{&ims[0]};
   std::vector<r3d_akaze_keypoint> kps;
   std::vector<std::vector<r3d_akaze_keypoint>*> outs{&kps};
-  const akaze::Debug dbg{arrays, kcontrast, cands, flags, cand_cap, cand_counts};
+  const akaze::Debug dbg{arrays, kcontrast, cands, flags, cand_cap, cand_counts, nullptr};
   double ms[akaze::kStages] = {};
   uint32_t launches = 0;
-  return akaze::run_batch(ctx, w, batch, opt->threshold, outs, &dbg, ms, &launches);
+  return akaze::run_batch(ctx, w, batch, opt->threshold, R3D_DETECTOR_FAST_AKAZE, outs, &dbg, ms, &launches);
+}
+
+extern "C" int r3d_debug_akaze_masks(r3d_ctx* ctx, const float* image, uint32_t width, uint32_t height,
+                                     const r3d_akaze_options* opt, float* arrays, float* kcontrast, uint8_t* masks) {
+  std::vector<akaze::Image> ims;
+  int rc = akaze::prepare(ctx, &image, &width, &height, 1, opt, ims);
+  if (rc) return rc;
+  if (!arrays || !kcontrast || !masks) return fail(ctx, R3D_ERR_INVALID, "r3d_debug_akaze_masks: bad arguments");
+  if (ims[0].lv.empty()) return R3D_OK;
+  DeviceWorker& w = ctx->workers[0];
+  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
+  std::vector<akaze::Image*> batch{&ims[0]};
+  std::vector<r3d_akaze_keypoint> kps;
+  std::vector<std::vector<r3d_akaze_keypoint>*> outs{&kps};
+  uint32_t count = 0;
+  const akaze::Debug dbg{arrays, kcontrast, nullptr, nullptr, 0, &count, masks};
+  double ms[akaze::kStages] = {};
+  uint32_t launches = 0;
+  return akaze::run_batch(ctx, w, batch, opt->threshold, R3D_DETECTOR_AKAZE, outs, &dbg, ms, &launches);
 }
 
 extern "C" int r3d_debug_akaze_refine(r3d_ctx* ctx, const float* ldet, uint32_t width, uint32_t height, float ratio,
