@@ -68,9 +68,10 @@ __device__ __forceinline__ float chunk_key(int32_t m, int32_t qn, uint32_t cid, 
 // Rounding to nearest is monotone and F is a float, so every integer distance >= F converts to a float >= F:
 // m + qn <= ceil(F) - 1 keeps every chunk that can enter the set (and a few that cannot: the network drops those).
 // F is +inf while the set holds the FLT_MAX sentinel; the conversion saturates to INT_MAX there.
-__device__ __forceinline__ int32_t bracket_bound(float kmax, uint32_t keep_mask, int32_t qn) {
+// Returned as ~bound = qn - ceil(F), so that m passes exactly when m + ~bound is negative.
+__device__ __forceinline__ int32_t bracket_bound_not(float kmax, uint32_t keep_mask, int32_t qn) {
   const float f = __uint_as_float((__float_as_uint(kmax) & keep_mask) - keep_mask);  // - keep_mask = + 2^chunk_bits
-  return __float2int_ru(f) - 1 - qn;
+  return qn - __float2int_ru(f);
 }
 
 // the kNumKeys smallest keys of this lane's set and the set of lane ^ d (the keys of different chunks differ)
@@ -215,6 +216,16 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       const int32_t qn1 = __ldg(pd.normJ + wi.sb * kBlockRows + row0 + 8u);
       int32_t acc[64];
       constexpr uint32_t kNkb = (kKSteps + 3) / 4;
+      // The low descriptor words of the consumer's query rows (K-block 0) and of the ring (stage 0, half 0), taken
+      // once per item from a warp-uniform consumer index, so they and everything derived from them stay in uniform
+      // registers.  Shared-memory addresses are below 2^18 bytes, so the 14-bit start-address field of a descriptor
+      // never carries: K-block kb, stage s, half h and k-step k only add (kb * kBoxBytes + s * kStageBytes +
+      // h * kBoxBytes) / 16 + 2 k.
+      const uint32_t cw_u = __shfl_sync(0xffffffffu, cw, 0);
+      const uint32_t a_lo = desc_lo(q_base + qb * q_bytes +
+                                    (kQBoxes == 1 ? cw_u * (kBoxBytes / 2)
+                                                  : (cw_u >> 1) * nkb * kBoxBytes + (cw_u & 1u) * (kBoxBytes / 2)));
+      const uint32_t d_lo = desc_lo(d_base);
       // MMAs of half h (database rows h * 128 .. + 127) of the tile whose K-blocks start at stage s0: kKSteps
       // back-to-back m64n128k32 behind one fence, no branch
       auto issue = [&](uint32_t h, uint32_t s0) {
@@ -222,11 +233,11 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
         uint32_t s = s0;
 #pragma unroll
         for (uint32_t kb = 0; kb < kNkb; ++kb) {
-          const uint32_t a_lo = desc_lo(a_base + kb * kBoxBytes);
-          const uint32_t b_lo = desc_lo(d_base + s * kStageBytes + h * kBoxBytes);
+          const uint32_t b_lo = d_lo + (s * kStageBytes + h * kBoxBytes) / 16u;
 #pragma unroll
           for (uint32_t k = 0; k < 4 && 4 * kb + k < kKSteps; ++k)
-            wgmma_m64n128k32_u8(acc, make_desc(a_lo + 2 * k), make_desc(b_lo + 2 * k), (kb | k) != 0u ? 1u : 0u);
+            wgmma_m64n128k32_u8(acc, make_desc(a_lo + kb * (kBoxBytes / 16u) + 2 * k), make_desc(b_lo + 2 * k),
+                                (kb | k) != 0u ? 1u : 0u);
           if (kb + 1 < kNkb && ++s == n_stages) s = 0;
         }
         wgmma_commit();
@@ -237,21 +248,22 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       // are the 8 rows of chunk t * 32 + h * 16 + 4 g + q, and their norms are 8 consecutive words of shared memory.
       // ||q - a||^2 = ||q||^2 + (||a||^2 - 2 q.a): each lane takes the minima of its chunks over the bracket, exactly
       // in s32 and without leaving its registers.
-      // A chunk can only enter its set if its key is below the set's largest, which never grows: bracket_bound turns
-      // that largest key, once per half, into an integer bound on the bracket minimum, so a chunk costs one compare
-      // and its key is only formed if it passes.  The chunks that pass are inserted in warp-uniform rounds, one per set
-      // and lane per round (FLT_MAX, a no-op of the network, where a lane has none left); a key that passed the bound
-      // but is not below the set's largest is a no-op too.  The keys of a set differ in their chunk bits, so the order
-      // of the insertions does not change the set.
+      // A chunk can only enter its set if its key is below the set's largest, which never grows: bracket_bound_not
+      // turns that largest key, once per half, into an integer bound on the bracket minimum, so a chunk costs one add
+      // (the sign of m + ~bound says whether it passes) and its key is only formed in an insertion round.  A chunk that
+      // fails has a key above the set's largest key, so inserting it is a no-op of the network; so is a chunk that
+      // passed but is not below the largest key.  The keys of a set differ in their chunk bits, so the order of the
+      // insertions does not change the set.
       // take_minima reads the accumulator and the half's norms; insert reads neither, so it runs while the MMAs of the
       // next half write the accumulator.
       int32_t m0[4], m1[4];
-      uint32_t p0, p1;  // bit g: m0[g] / m1[g] is still to be inserted
+      // The insertion order of each set's four chunks, highest bit first: bit 16 + 4 g + 3 for a chunk g that passed
+      // the bound, bit 4 g + 3 for one that failed.  Bits 2 and 3 of a bit's index are g.
+      uint32_t u0, u1;
       auto take_minima = [&](uint32_t h, uint32_t s0) {
         const int32_t* nrm = (const int32_t*)(smem_raw + (n_base + s0 * kNormBytes - smem_u32(smem_raw))) + h * 128u + 8u * q;
-        const int32_t b0 = bracket_bound(key0[kNumKeys - 1], keep_mask, qn0);
-        const int32_t b1 = bracket_bound(key1[kNumKeys - 1], keep_mask, qn1);
-        p0 = p1 = 0;
+        const int32_t nb0 = bracket_bound_not(key0[kNumKeys - 1], keep_mask, qn0);
+        const int32_t nb1 = bracket_bound_not(key1[kNumKeys - 1], keep_mask, qn1);
 #pragma unroll
         for (uint32_t g = 0; g < 4; ++g) {
           const int4 na = *(const int4*)(nrm + kGroupRows * g);
@@ -263,26 +275,35 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
                                  nb.x - 2 * a[10], nb.y - 2 * a[11], nb.z - 2 * a[14], nb.w - 2 * a[15]};
           m0[g] = min8(d0);
           m1[g] = min8(d1);
-          p0 |= (m0[g] <= b0 ? 1u : 0u) << g;
-          p1 |= (m1[g] <= b1 ? 1u : 0u) << g;
         }
+        // the top nibble of m[g] + ~bound to nibble g (its sign to bit 4 g + 3), one funnel shift per chunk; no
+        // overflow: m + ~bound = (m + qn) - ceil(F) with 0 <= m + qn <= 2^28 + 2^23 and 16 <= ceil(F) <= INT_MAX
+        uint32_t w0 = 0, w1 = 0;
+#pragma unroll
+        for (int g = 3; g >= 0; --g) {
+          w0 = __funnelshift_l((uint32_t)(m0[g] + nb0), w0, 4);
+          w1 = __funnelshift_l((uint32_t)(m1[g] + nb1), w1, 4);
+        }
+        w0 &= 0x8888u;
+        w1 &= 0x8888u;
+        u0 = w0 << 16 | (w0 ^ 0x8888u);
+        u1 = w1 << 16 | (w1 ^ 0x8888u);
+      };
+      // Per round every lane inserts the next chunk of each of its sets, until no lane of the warp has a chunk that
+      // passed left.  A lane with fewer such chunks inserts chunks that failed, which leaves its sets as they are.  No
+      // chunk is inserted twice, and a set has four chunks and at most four rounds run, so no sentinel is needed.
+      auto next_key = [&](uint32_t& u, const int32_t (&m)[4], int32_t qn, uint32_t chunk0) {
+        const uint32_t i = 31 - __clz(u);
+        u ^= 1u << i;
+        const bool g1 = (i & 4u) != 0u;
+        const int32_t y = (i & 8u) ? (g1 ? m[3] : m[2]) : (g1 ? m[1] : m[0]);
+        return chunk_key(y, qn, chunk0 | (i & 12u), keep_mask);
       };
       auto insert = [&](uint32_t t, uint32_t h) {
-        const uint32_t chunk0 = t * (kTileN / kChunk) + h * (kTileN / 2 / kChunk) + q;
-        while (__any_sync(0xffffffffu, (p0 | p1) != 0u)) {
-          int32_t y0 = 0, y1 = 0;
-          uint32_t g0 = 0, g1 = 0;
-#pragma unroll
-          for (int g = 3; g >= 0; --g) {  // the lowest pending chunk of each set
-            if (p0 & (1u << g)) { y0 = m0[g]; g0 = g; }
-            if (p1 & (1u << g)) { y1 = m1[g]; g1 = g; }
-          }
-          const float x0 = p0 != 0u ? chunk_key(y0, qn0, chunk0 + 4 * g0, keep_mask) : __uint_as_float(kKeySentinel);
-          const float x1 = p1 != 0u ? chunk_key(y1, qn1, chunk0 + 4 * g1, keep_mask) : __uint_as_float(kKeySentinel);
-          p0 &= p0 - 1u;
-          p1 &= p1 - 1u;
-          key_insert_packed(x0, key0);
-          key_insert_packed(x1, key1);
+        const uint32_t chunk0 = t * (kTileN / kChunk) + h * (kTileN / 2 / kChunk) + q;  // bits 2 and 3 clear
+        while (__any_sync(0xffffffffu, (u0 | u1) >> 16 != 0u)) {
+          key_insert_packed(next_key(u0, m0, qn0, chunk0), key0);
+          key_insert_packed(next_key(u1, m1, qn1, chunk0), key1);
         }
       };
       // the first stage of the next tile, once all of its K-blocks have landed
