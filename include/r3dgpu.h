@@ -554,6 +554,50 @@ int r3d_sfm_structure_from_tracks(r3d_ctx* ctx, r3d_sfm_data* sd, const r3d_trac
 int r3d_sfm_remove_outliers(r3d_ctx* ctx, r3d_sfm_data* sd, double max_pixel_residual, uint32_t min_track_length,
                             double min_angle_deg, uint32_t* removed_observations, uint32_t* removed_landmarks);
 
+/* ---- after the engine: the coloured model and the undistorted views (DESIGN.md 4.5i) -------------------------------
+ * The plan of OpenMVGHelper::ColorizeTracks (src/utils/OpenMVGHelper.cpp:2453-2560), the greedy loop the triangulation
+ * step runs after Process() (src/threads/R3DTriangulationThread.cpp:461-476, :267-278): each round counts, per view, the
+ * observations of the landmarks not coloured yet, picks the first view in id order with the largest count
+ * (sort_index_helper with nbuplet = 1: std::partial_sort under val >, a first-max), and every remaining landmark that
+ * view observes takes its colour from that view's image at (int)y, (int)x (truncated toward zero).  The whole loop runs
+ * on the device; the images stay with the caller, who reads them in round_view order and gathers rgb[y][x].
+ * round_view: num_views entries, the view id chosen in each of the *n_rounds rounds; lm_round: per landmark in id order,
+ * the round that colours it; lm_pixel: per landmark, (x, y) in that round's image.  R3D_ERR_INVALID before any device
+ * work for: a landmark without observations, an observation whose truncated position lies outside its view's
+ * width x height, an observation of a view without a pose or intrinsic (never in a reconstructed scene).  A pose shared by
+ * views with different intrinsics: R3D_ERR_UNSUPPORTED (the scene as r3d_sfm_bundle_adjust reads it).  Runs on the
+ * context's first device. */
+int r3d_sfm_colorize_plan(r3d_ctx* ctx, const r3d_sfm_data* sd, uint32_t* round_view, uint32_t* n_rounds,
+                          uint32_t* lm_round, int32_t* lm_pixel);
+/* Host only: FinalColorized.ply as plyHelper::exportToPly writes it with colours (SfMPlyHelper.hpp:62-116): an ASCII
+ * header, every landmark in id order as "x y z r g b" (std::fixed, precision 16; colors: num_landmarks x 3 in landmark
+ * id order, NULL = 255 255 255), then the centre of every pose in pose-id order with 0 255 0.  R3D_ERR_IO naming the
+ * path. */
+int r3d_sfm_write_colorized_ply(const r3d_sfm_data* sd, const uint8_t* colors, const char* path);
+
+/* OpenMVG 1.4's UndistortImage(image, cam, image_ud, BLACK), which every densification export runs on every
+ * reconstructed view (OpenMVGHelper.cpp:750, :1223, :1377, :1819, :2093, :2281, :2860, :3026,
+ * OpenMVGExportToMVS.cpp:157).  Per view: a pinhole intrinsic copies the image; every other model (zero coefficients
+ * too) fills black, then each output pixel (i, j) whose distorted position d = cam2ima(add_disto(ima2cam(i, j)))
+ * (double) satisfies Contains((int)d.y, (int)d.x) takes Sampler2d<SamplerLinear>(in, (float)d.y, (float)d.x): float
+ * weights over the 2 x 2 taps from floor, taps outside the image dropped, the sum accumulated in double and divided by
+ * the total weight when that is not 1, total weight <= 0.2: black; the value clamped to [0, 255] and truncated
+ * (DESIGN.md 2.4).  rgb[k] / out[k]: heights[k] x widths[k] x 3 uint8, row-major; intr[k]: the view's intrinsic (its
+ * model, focal, principal point and disto; its width / height are not read).  R3D_ERR_INVALID before any work for a
+ * NULL pointer, a zero width or height, an unknown model.  Images are dealt to the context's devices in contiguous
+ * runs; on each, pinned staging buffers double-buffer the uploads (copy stream) against the kernel and downloads
+ * (compute stream).  timing (may be NULL): the call's stage times. */
+typedef struct {
+  double upload_ms;    /* host -> device copies (CUDA events, summed over images and devices) */
+  double kernel_ms;    /* the undistortion kernels */
+  double download_ms;  /* device -> host copies */
+  double stage_ms;     /* host copies into and out of the pinned staging buffers (wall time, summed over devices) */
+  double total_ms;     /* the call's wall time */
+  uint32_t images, copied, kernel_launches, devices;  /* copied: pinhole views */
+} r3d_undistort_timing;
+int r3d_undistort_images(r3d_ctx* ctx, uint32_t n, const r3d_sfm_intrinsic* intr, const uint8_t* const* rgb,
+                         const uint32_t* widths, const uint32_t* heights, uint8_t* const* out, r3d_undistort_timing* timing);
+
 /* ---- multi-GPU bundle adjustment (SURVEY.md 8e: the one path with a real exchange step) -------
  * One process per GPU.  The 3-D points (with all their observations) are partitioned over the
  * ranks, cameras and intrinsics are replicated: every rank passes r3d_bundle_adjust ALL cameras /

@@ -24,7 +24,7 @@ NVCC_FLAGS = ARCH + [
 ]
 # translation units whose floating-point decisions must match the CPU restatement bit for bit are
 # compiled without FMA contraction
-NO_FMAD = {"acransac_kernels.cu", "acransac_fused.cu", "akaze.cu", "liop.cu", "relpose.cu", "resection.cu", "rotavg.cu",
+NO_FMAD = {"acransac_kernels.cu", "acransac_fused.cu", "akaze.cu", "export.cu", "liop.cu", "relpose.cu", "resection.cu", "rotavg.cu",
            "rotavg_l1.cu", "transavg.cu", "transavg_l1.cu"}
 
 

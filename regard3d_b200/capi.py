@@ -46,6 +46,7 @@ EXPORTS = [
     "r3d_debug_akaze_refine", "r3d_debug_view_operands",
     "r3d_extract_default_options", "r3d_extract_features", "r3d_features_descriptors", "r3d_save_features",
     "r3d_get_extract_timing", "r3d_detect_keypoints", "r3d_extract_features_detector", "r3d_debug_akaze_masks",
+    "r3d_sfm_colorize_plan", "r3d_sfm_write_colorized_ply", "r3d_undistort_images",
 ]
 
 CHOL_DENSE, CHOL_ENVELOPE = 0, 1
@@ -366,6 +367,10 @@ def lib():
         L.r3d_sfm_structure_from_tracks.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.r3d_sfm_remove_outliers.argtypes = [C.c_void_p, C.c_void_p, C.c_double, C.c_uint32, C.c_double, C.c_void_p, C.c_void_p]
         L.r3d_sfm_bundle_adjust.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.r3d_sfm_colorize_plan.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.r3d_sfm_write_colorized_ply.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p]
+        L.r3d_undistort_images.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p]
         L.r3d_save_matches.argtypes = [C.c_void_p, C.c_char_p]
         L.r3d_save_matches_bin.argtypes = [C.c_void_p, C.c_char_p]
         L.r3d_comm_world.argtypes = [C.c_void_p]
@@ -526,6 +531,12 @@ SFM_VIEWS, SFM_EXTRINSICS, SFM_INTRINSICS, SFM_STRUCTURE, SFM_CONTROL_POINTS, SF
 CAM_PINHOLE, CAM_RADIAL1, CAM_RADIAL3, CAM_BROWN, CAM_FISHEYE = 1, 2, 3, 4, 5
 
 
+class UndistortTiming(C.Structure):
+    _fields_ = [("upload_ms", C.c_double), ("kernel_ms", C.c_double), ("download_ms", C.c_double), ("stage_ms", C.c_double),
+                ("total_ms", C.c_double), ("images", C.c_uint32), ("copied", C.c_uint32), ("kernel_launches", C.c_uint32),
+                ("devices", C.c_uint32)]
+
+
 class ResectionOptions(C.Structure):
     _fields_ = [("precision_px", C.c_double), ("max_iter", C.c_uint32), ("refine", C.c_int), ("ba", BAOptions)]
 
@@ -682,6 +693,33 @@ class SfmData:
             out.append(dict(id=lid.value, X=list(X), obs=[(arr[q].id_view, arr[q].id_feat, arr[q].x[0], arr[q].x[1])
                                                           for q in range(n.value)]))
         return out
+
+    def colorize(self, ctx, read_rgb):
+        """OpenMVGHelper::ColorizeTracks: the colour of every landmark, (num_landmarks, 3) uint8 in landmark id order.
+        The plan comes from the device (Context.colorize_plan); read_rgb(view_id) -> H x W x 3 uint8 is called once per
+        round, in the order upstream reads the images, and only the planned pixels are gathered from each."""
+        round_view, lm_round, lm_pixel = ctx.colorize_plan(self)
+        sizes = {v["id_view"]: (v["height"], v["width"]) for v in self.views()}
+        colors = np.zeros((len(lm_round), 3), np.uint8)
+        for r, v in enumerate(round_view.tolist()):
+            img = np.asarray(read_rgb(v))
+            if img.dtype != np.uint8 or img.shape != sizes[v] + (3,):
+                raise ValueError("read_rgb(%d): expected a %d x %d x 3 uint8 image, got %s %s"
+                                 % ((v,) + sizes[v] + (img.dtype, img.shape)))
+            sel = np.nonzero(lm_round == r)[0]
+            colors[sel] = img[lm_pixel[sel, 1], lm_pixel[sel, 0]]
+        return colors
+
+    def write_colorized_ply(self, path, colors=None):
+        """FinalColorized.ply: landmarks with colors ((num_landmarks, 3) uint8, None = white), then the pose centres."""
+        col = None
+        if colors is not None:
+            col = np.ascontiguousarray(colors, np.uint8)
+            if col.shape != (lib().r3d_sfm_num_landmarks(self.h, 0), 3):
+                raise ValueError("colors: expected (num_landmarks, 3), got %s" % (col.shape,))
+        rc = lib().r3d_sfm_write_colorized_ply(self.h, None if col is None else _p(col), path.encode())
+        if rc:
+            raise R3DError(rc, lib().r3d_last_error(None).decode())
 
 
 class Tracks:
@@ -1431,6 +1469,46 @@ class Context:
         self._check(lib().r3d_sfm_remove_outliers(self._h, sd.h, C.c_double(max_pixel_residual), C.c_uint32(min_track_length),
                                                   C.c_double(min_angle_deg), C.byref(a), C.byref(b)))
         return a.value, b.value
+
+    def colorize_plan(self, sd):
+        """r3d_sfm_colorize_plan: (round_view[:n_rounds] view ids, lm_round (num_landmarks,) uint32,
+        lm_pixel (num_landmarks, 2) int32 as (x, y)), landmarks in id order."""
+        nv, nl = lib().r3d_sfm_num_views(sd.h), lib().r3d_sfm_num_landmarks(sd.h, 0)
+        rv = np.zeros(max(nv, 1), np.uint32)
+        nr = C.c_uint32()
+        lr = np.zeros(max(nl, 1), np.uint32)
+        lp = np.zeros((max(nl, 1), 2), np.int32)
+        self._check(lib().r3d_sfm_colorize_plan(self._h, sd.h, _p(rv), C.byref(nr), _p(lr), _p(lp)))
+        return rv[:nr.value].copy(), lr[:nl].copy(), lp[:nl].copy()
+
+    def undistort_images(self, intrinsics, images):
+        """UndistortImage with black fill of each H x W x 3 uint8 image through its intrinsic (a dict with model, focal,
+        ppx, ppy, disto as SfmData.intrinsics() returns, or an SfmIntrinsic); returns the undistorted images.  The call's
+        stage times are left in self.last_undistort_timing."""
+        n = len(images)
+        if len(intrinsics) != n:
+            raise ValueError("one intrinsic per image")
+        imgs = [np.ascontiguousarray(a, np.uint8) for a in images]
+        for a in imgs:
+            if a.ndim != 3 or a.shape[2] != 3:
+                raise ValueError("images must be H x W x 3 uint8, got %s" % (a.shape,))
+        intr = (SfmIntrinsic * max(n, 1))()
+        for k, d in enumerate(intrinsics):
+            if isinstance(d, SfmIntrinsic):
+                intr[k] = d
+                continue
+            dist = list(d.get("disto", ())) + [0.0] * (5 - len(d.get("disto", ())))
+            intr[k] = SfmIntrinsic(int(d.get("id", k)), int(d["model"]), int(d.get("width", 0)), int(d.get("height", 0)),
+                                   float(d["focal"]), float(d["ppx"]), float(d["ppy"]), (C.c_double * 5)(*dist))
+        outs = [np.empty_like(a) for a in imgs]
+        src = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in imgs])
+        dst = (C.c_void_p * max(n, 1))(*[a.ctypes.data for a in outs])
+        ws = np.array([a.shape[1] for a in imgs] or [0], np.uint32)
+        hs = np.array([a.shape[0] for a in imgs] or [0], np.uint32)
+        t = UndistortTiming()
+        self._check(lib().r3d_undistort_images(self._h, C.c_uint32(n), intr, src, _p(ws), _p(hs), dst, C.byref(t)))
+        self.last_undistort_timing = {k: getattr(t, k) for k, _ in UndistortTiming._fields_}
+        return outs
 
     def sfm_bundle_adjust(self, sd, max_iterations=500, refine_intrinsics=1, use_motion_priors=0, huber_a=16.0):
         class SfmBAOptions(C.Structure):
