@@ -22,8 +22,8 @@
 //           next half's MMAs are issued, and the half's key insertion runs behind them.  The other three consumers
 //           keep MMAs in the tensor pipe too.  The database map loads every 32-row group with its row pairs
 //           transposed (context.cu), so each lane of a quad holds whole chunks: the chunk minima take no shuffle.  An
-//           integer bound taken once per half from each set's largest key rejects nearly every chunk before its key
-//           is formed; the rest are inserted in warp-uniform rounds.
+//           integer bound taken once per tile from the quad's four sets of a row rejects nearly every chunk before its
+//           key is formed; the rest are inserted in warp-uniform rounds, one round loop per set.
 // Barriers: full[s] (TMA bytes landed), empty[s] (every consumer warp is done with the stage), qfull / qempty the same
 // for the query buffers.
 #include "r3d_internal.cuh"
@@ -72,6 +72,19 @@ __device__ __forceinline__ float chunk_key(int32_t m, int32_t qn, uint32_t cid, 
 __device__ __forceinline__ int32_t bracket_bound_not(float kmax, uint32_t keep_mask, int32_t qn) {
   const float f = __uint_as_float((__float_as_uint(kmax) & keep_mask) - keep_mask);  // - keep_mask = + 2^chunk_bits
   return qn - __float2int_ru(f);
+}
+
+// u8: an upper bound on the kNumKeys-th smallest key of the union of the quad's four sets of one row: the smallest of
+// their largest keys, or the largest of their second keys (eight keys are at or below it).  The FLT_MAX sentinels are
+// equal, but a bound below FLT_MAX is the largest key of a full set or the largest of eight real keys, which differ.
+__device__ __forceinline__ float quad_bound(const float (&key)[kNumKeys]) {
+  float k5 = key[kNumKeys - 1], k1 = key[1];
+#pragma unroll
+  for (int d = 1; d <= 2; d *= 2) {
+    k5 = fminf(k5, __shfl_xor_sync(0xffffffffu, k5, d));
+    k1 = fmaxf(k1, __shfl_xor_sync(0xffffffffu, k1, d));
+  }
+  return fminf(k5, k1);
 }
 
 // the kNumKeys smallest keys of this lane's set and the set of lane ^ d (the keys of different chunks differ)
@@ -248,22 +261,29 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
       // are the 8 rows of chunk t * 32 + h * 16 + 4 g + q, and their norms are 8 consecutive words of shared memory.
       // ||q - a||^2 = ||q||^2 + (||a||^2 - 2 q.a): each lane takes the minima of its chunks over the bracket, exactly
       // in s32 and without leaving its registers.
-      // A chunk can only enter its set if its key is below the set's largest, which never grows: bracket_bound_not
-      // turns that largest key, once per half, into an integer bound on the bracket minimum, so a chunk costs one add
-      // (the sign of m + ~bound says whether it passes) and its key is only formed in an insertion round.  A chunk that
-      // fails has a key above the set's largest key, so inserting it is a no-op of the network; so is a chunk that
-      // passed but is not below the largest key.  The keys of a set differ in their chunk bits, so the order of the
-      // insertions does not change the set.
+      // The item writes the kNumKeys smallest keys of the union of the quad's four sets (merge_keys), so a chunk whose
+      // key is not below U, any upper bound on the union's kNumKeys-th smallest key, can be dropped: it is not in the
+      // row's final keys, and every chunk that is passes U and stays among its own set's kNumKeys smallest.  Keys
+      // only fall, so a U taken earlier stays valid.  Once per tile, in the first half, after the previous half's
+      // insertion, quad_bound takes U from the four sets and bracket_bound_not turns it into an integer bound on the
+      // bracket minimum; the second half reuses it.  A chunk costs one add (the sign of m + ~bound says whether it
+      // passes) and its key is only formed in an insertion round.  Inserting a chunk whose key is above U, passed or
+      // failed, is harmless: it can only push out keys above its own, which are not among the row's final keys.  So
+      // the rounds below may insert chunks that failed, and the merged keys do not depend on the order of insertion
+      // (the keys of a row differ in their chunk bits).
       // take_minima reads the accumulator and the half's norms; insert reads neither, so it runs while the MMAs of the
       // next half write the accumulator.
       int32_t m0[4], m1[4];
+      int32_t nb0, nb1;  // ~bound of each set for the current tile
       // The insertion order of each set's four chunks, highest bit first: bit 16 + 4 g + 3 for a chunk g that passed
       // the bound, bit 4 g + 3 for one that failed.  Bits 2 and 3 of a bit's index are g.
       uint32_t u0, u1;
       auto take_minima = [&](uint32_t h, uint32_t s0) {
         const int32_t* nrm = (const int32_t*)(smem_raw + (n_base + s0 * kNormBytes - smem_u32(smem_raw))) + h * 128u + 8u * q;
-        const int32_t nb0 = bracket_bound_not(key0[kNumKeys - 1], keep_mask, qn0);
-        const int32_t nb1 = bracket_bound_not(key1[kNumKeys - 1], keep_mask, qn1);
+        if (h == 0) {
+          nb0 = bracket_bound_not(quad_bound(key0), keep_mask, qn0);
+          nb1 = bracket_bound_not(quad_bound(key1), keep_mask, qn1);
+        }
 #pragma unroll
         for (uint32_t g = 0; g < 4; ++g) {
           const int4 na = *(const int4*)(nrm + kGroupRows * g);
@@ -289,22 +309,23 @@ k_l2_candidates(const CUtensorMap* __restrict__ tmapQ, const CUtensorMap* __rest
         u0 = w0 << 16 | (w0 ^ 0x8888u);
         u1 = w1 << 16 | (w1 ^ 0x8888u);
       };
-      // Per round every lane inserts the next chunk of each of its sets, until no lane of the warp has a chunk that
-      // passed left.  A lane with fewer such chunks inserts chunks that failed, which leaves its sets as they are.  No
-      // chunk is inserted twice, and a set has four chunks and at most four rounds run, so no sentinel is needed.
+      // One warp-uniform round loop per set: per round every lane inserts the set's next chunk, until no lane of the
+      // warp has a chunk that passed left, so a set in which no lane's chunk passed costs one vote.  A lane with fewer
+      // such chunks inserts chunks that failed, which is harmless (above).  No chunk is inserted twice, and a set has
+      // four chunks and at most four rounds run, so no sentinel is needed.
       auto next_key = [&](uint32_t& u, const int32_t (&m)[4], int32_t qn, uint32_t chunk0) {
         const uint32_t i = 31 - __clz(u);
-        u ^= 1u << i;
-        const bool g1 = (i & 4u) != 0u;
-        const int32_t y = (i & 8u) ? (g1 ? m[3] : m[2]) : (g1 ? m[1] : m[0]);
-        return chunk_key(y, qn, chunk0 | (i & 12u), keep_mask);
+        uint32_t below;  // (1 << i) - 1 in one BMSK: clears u's highest bit
+        asm("bmsk.clamp.b32 %0, 0, %1;" : "=r"(below) : "r"(i));
+        u &= below;
+        const int32_t lo = (i & 4u) ? m[1] : m[0];
+        const int32_t hi = (i & 4u) ? m[3] : m[2];
+        return chunk_key((i & 8u) ? hi : lo, qn, chunk0 | (i & 12u), keep_mask);
       };
       auto insert = [&](uint32_t t, uint32_t h) {
         const uint32_t chunk0 = t * (kTileN / kChunk) + h * (kTileN / 2 / kChunk) + q;  // bits 2 and 3 clear
-        while (__any_sync(0xffffffffu, (u0 | u1) >> 16 != 0u)) {
-          key_insert_packed(next_key(u0, m0, qn0, chunk0), key0);
-          key_insert_packed(next_key(u1, m1, qn1, chunk0), key1);
-        }
+        while (__any_sync(0xffffffffu, u0 >> 16 != 0u)) key_insert_packed(next_key(u0, m0, qn0, chunk0), key0);
+        while (__any_sync(0xffffffffu, u1 >> 16 != 0u)) key_insert_packed(next_key(u1, m1, qn1, chunk0), key1);
       };
       // the first stage of the next tile, once all of its K-blocks have landed
       auto wait_tile = [&]() {
