@@ -445,6 +445,57 @@ typedef struct {
 int r3d_rotation_averaging_l1(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views,
                               const r3d_rotavg_l1_options* opt, double* rotations, uint8_t* view_kept, uint8_t* edge_kept,
                               uint32_t* edge_support, r3d_rotavg_l1_summary* summary);
+/* Diagnostics (device): one step of r3d_rotation_averaging_l1 through the members that function runs, on the same kept
+ * component (m views, E edges, n = m - 1 free views).  kind 0: one Newton iteration of l1decode_pd (primal-dual), from
+ * `state` at `tau` or, with state NULL, from the start point k_l1_pd_start forms at the residuals; then the rotations
+ * updated by the resulting x, as after the last iteration of an L1RA step.  kind 1: one IRLS iteration.  kind 2: the
+ * weighted normal equations (A^T diag(weights) A) dx = A^T rhs for n_systems (weights, rhs) pairs of 3E rows each, one
+ * after the other on the same scratch.  A state is x (3n), A x, u, lambda_1, lambda_2 (3E each), A^T (lambda_1 -
+ * lambda_2) (3n): 12 (E + n / 2) values.  Per-row arrays are E x 3 (row 3e + k), per-variable arrays component-major
+ * (k n + a - 1).  Array outputs are caller-allocated for at most m = n_views and E = n_rel, NULL ones are skipped; the
+ * scalars are always filled. */
+typedef struct {
+  uint32_t n_kept_views, n_kept_edges;  /* m, E; 0: no component, nothing else written */
+  uint32_t* view_ids;       /* m: the kept view ids by local id (local 0: the gauge) */
+  uint32_t* ab;             /* E x 2: each kept edge's local (a, b), a < b, in the kernels' order */
+  double* Rk;               /* E x 9: its R_ab (R_b = R_ab R_a), row-major */
+  double* rotations0;       /* m x 9: the rotations the step started from, by local id */
+  double *b, *cost;         /* 3E, E: the residuals log(R_b^T R_ab R_a) there and |b_e|_1 */
+  double bmax;              /* max |b| */
+  int b_zero;               /* kind 0 from the start point: b = 0, so x = 0 and no iteration ran */
+  /* kind 0 */
+  double* state0;           /* the state the iteration started from */
+  double sdg0, tau0, resnorm0;  /* its surrogate duality gap, tau and residual norm |(r_dual, r_cent)| */
+  double *sigx, *rrow, *w2; /* 3E: the Newton system's row weights, right-hand-side rows and w2 */
+  double* laplacians;       /* kinds 0, 1: 3 x (n + 1) x n, kind 2: n_systems of them: per component the Laplacian
+                             * (rows 0..n-1) and the right-hand side A^T v (row n) as assembled, before factoring */
+  int not_pd;               /* kinds 0, 1: the system was not positive definite (nothing after the solve ran) */
+  double* dx;               /* kinds 0, 1: 3n; kind 2: n_systems x 3n, not written for a system that is not PD */
+  double *Adx, *du, *dl1, *dl2;  /* 3E: the direction's other parts */
+  double* Atdv;             /* 3n: A^T (dl1 - dl2) */
+  double* rmin;             /* E: per edge min(1, its largest feasible step) */
+  double step_max;          /* min over rmin: the ratio test's step before the 0.99 */
+  uint32_t n_trials;        /* trial steps of the line search (<= 33) */
+  double trial_step[33], trial_resnorm[33];  /* each trial's step and residual norm */
+  int accepted;             /* the last trial was accepted (else the solver stops with the state it started from) */
+  double* state;            /* the state after the iteration */
+  double sdg, tau, resnorm; /* its values */
+  /* kind 1 */
+  double *w, *wb;           /* 3E: the Geman-McClure weights and w b */
+  /* kinds 0, 1 */
+  double* rotations;        /* m x 9: R_v exp([x_v]x) by local id (kind 0: x of the state after the iteration) */
+  double xmax;              /* max |x| */
+  /* kind 2 */
+  int* sys_not_pd;          /* n_systems: each system was not positive definite */
+} r3d_rotavg_l1_step_out;
+/* rotations: NULL for the spanning-tree start, else n_views x 9 by view id (rotation_averaging_l1's layout; the kept
+ * views' are read), finite.  kind 0: state NULL (n_state 0) or n_state = 12 E + 6 n finite values with u > |A x - b|
+ * and lambda > 0 at the residuals, and tau > 0 finite; else R3D_ERR_INVALID.  kind 2: weights and rhs hold n_systems x
+ * 3E values (n_systems >= 1).  opt: r3d_rotation_averaging_l1's (the kept component, irls_sigma_deg). */
+int r3d_debug_rotavg_l1_step(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views,
+                             const r3d_rotavg_l1_options* opt, const double* rotations, int kind, const double* state,
+                             uint64_t n_state, double tau, const double* weights, const double* rhs, uint32_t n_systems,
+                             r3d_rotavg_l1_step_out* out);
 /* graph::CleanGraph_KeepLargestBiEdge_Nodes + KeepOnlyReferencedElement on a PairWiseMatches (how upstream's
  * GlobalSfMReconstructionEngine_RelativeMotions::Process() starts): the pairs whose views both lie in the largest
  * 2-edge-connected component of the pair graph (most views; a tie keeps the component holding the smallest view id).

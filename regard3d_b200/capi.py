@@ -37,7 +37,7 @@ EXPORTS = [
     "r3d_relpose_default_options", "r3d_relative_poses", "r3d_get_relpose_timing",
     "r3d_resection_default_options", "r3d_resect_views", "r3d_sfm_resect_views", "r3d_get_resection_timing",
     "r3d_rotavg_default_options", "r3d_rotation_averaging", "r3d_rotavg_l1_default_options", "r3d_rotation_averaging_l1",
-    "r3d_matches_keep_largest_biedge_component",
+    "r3d_debug_rotavg_l1_step", "r3d_matches_keep_largest_biedge_component",
     "r3d_transavg_default_options", "r3d_translation_averaging", "r3d_transavg_l1_default_options",
     "r3d_translation_averaging_l1", "r3d_debug_transavg_l1_step", "r3d_debug_cholesky", "r3d_debug_chol_solve3",
     "r3d_debug_acransac_score", "r3d_debug_detmath", "r3d_debug_ba_step",
@@ -239,6 +239,19 @@ class RotavgL1Summary(C.Structure):
                 ("termination", C.c_int), ("initial_l1_cost", C.c_double), ("final_l1_cost", C.c_double),
                 ("ms_triplets", C.c_double), ("ms_init", C.c_double), ("ms_l1", C.c_double), ("ms_irls", C.c_double),
                 ("ms_device_total", C.c_double), ("ms_host", C.c_double)]
+
+
+class RotavgL1StepOut(C.Structure):
+    _fields_ = [("n_kept_views", C.c_uint32), ("n_kept_edges", C.c_uint32), ("view_ids", C.c_void_p), ("ab", C.c_void_p),
+                ("Rk", C.c_void_p), ("rotations0", C.c_void_p), ("b", C.c_void_p), ("cost", C.c_void_p), ("bmax", C.c_double),
+                ("b_zero", C.c_int), ("state0", C.c_void_p), ("sdg0", C.c_double), ("tau0", C.c_double),
+                ("resnorm0", C.c_double), ("sigx", C.c_void_p), ("rrow", C.c_void_p), ("w2", C.c_void_p),
+                ("laplacians", C.c_void_p), ("not_pd", C.c_int), ("dx", C.c_void_p), ("Adx", C.c_void_p), ("du", C.c_void_p),
+                ("dl1", C.c_void_p), ("dl2", C.c_void_p), ("Atdv", C.c_void_p), ("rmin", C.c_void_p), ("step_max", C.c_double),
+                ("n_trials", C.c_uint32), ("trial_step", C.c_double * 33), ("trial_resnorm", C.c_double * 33),
+                ("accepted", C.c_int), ("state", C.c_void_p), ("sdg", C.c_double), ("tau", C.c_double),
+                ("resnorm", C.c_double), ("w", C.c_void_p), ("wb", C.c_void_p), ("rotations", C.c_void_p),
+                ("xmax", C.c_double), ("sys_not_pd", C.c_void_p)]
 
 
 TRANSAVG_L1, TRANSAVG_L2_CHORDAL, TRANSAVG_SOFTL1 = 1, 2, 3
@@ -1241,6 +1254,84 @@ class Context:
                                                     _p(rot), _p(vk), _p(ek), _p(sup), C.byref(s)))
         summ = {k: getattr(s, k) for k, _ in RotavgL1Summary._fields_}
         return rot[:n_views], vk[:n_views].astype(bool), ek[:len(rel)].astype(bool), sup[:len(rel)].copy(), summ
+
+    def debug_rotavg_l1_step(self, rel, n_views, kind=0, rotations=None, state=None, tau=0.0, weights=None, rhs=None,
+                             **options):
+        """r3d_debug_rotavg_l1_step: one step of rotation_averaging_l1 on the same kept component (m views, E edges,
+        n = m - 1).  kind 0: one primal-dual Newton iteration from state = (x, Ax, u, l1, l2, Atv) at tau, or with None
+        from the start point; kind 1: one IRLS iteration; kind 2: the weighted normal equations for each row of weights /
+        rhs ((K, 3E) each).  rotations: (n_views, 3, 3) by view id, None for the spanning-tree start.  options:
+        r3d_rotavg_l1_options fields.  Returns a dict: m, E, n, view_ids, ab (E, 2), Rk (E, 3, 3), rotations0 (m, 3, 3),
+        b (3E), cost (E), bmax, b_zero; kind 0: state0 / state (tuples as state; x and Atv (3n) component-major, the others
+        3E), sdg0, tau0, resnorm0, sigx, rrow, w2, not_pd, laplacians (3, n + 1, n), dx, Adx, du, dl1, dl2, Atdv, rmin,
+        step_max, trials ((step, residual norm) per trial), accepted, sdg, tau, resnorm; kind 1: w, wb, laplacians,
+        not_pd, dx; kinds 0 and 1: rotations (m, 3, 3) after the update, xmax; kind 2: laplacians (K, 3, n + 1, n), dx
+        (K, 3n; NaN for a system that is not positive definite), sys_not_pd (K)."""
+        rel = np.ascontiguousarray(rel, relpose_dtype)
+        o = RotavgL1Options()
+        lib().r3d_rotavg_l1_default_options(C.byref(o))
+        for k, v in options.items():
+            if k not in dict(RotavgL1Options._fields_):
+                raise TypeError("unknown option %r" % k)
+            setattr(o, k, v)
+        rot = None
+        if rotations is not None:
+            rot = np.ascontiguousarray(np.asarray(rotations, np.float64).reshape(-1, 9))
+            if len(rot) < n_views:
+                raise ValueError("rotations hold fewer than n_views views")
+        x = None if state is None else np.ascontiguousarray(np.concatenate([np.asarray(a, np.float64).ravel() for a in state]))
+        K = 1
+        wt = rh = None
+        if kind == 2:
+            wt = np.ascontiguousarray(np.atleast_2d(np.asarray(weights, np.float64)))
+            rh = np.ascontiguousarray(np.atleast_2d(np.asarray(rhs, np.float64)))
+            if wt.shape != rh.shape:
+                raise ValueError("weights and rhs must have the same shape")
+            K = len(wt)
+        mc, ec = max(n_views, 1), max(len(rel), 1)
+        nr, nv, nst = 3 * ec, 3 * mc, 12 * ec + 6 * mc
+        r = {"view_ids": np.zeros(mc, np.uint32), "ab": np.zeros(2 * ec, np.uint32), "Rk": np.zeros(9 * ec),
+             "rotations0": np.zeros(9 * mc), "b": np.zeros(nr), "cost": np.zeros(ec), "state0": np.zeros(nst),
+             "laplacians": np.zeros(K * 3 * mc * mc), "dx": np.full(K * nv, np.nan), "Atdv": np.zeros(nv), "rmin": np.zeros(ec),
+             "state": np.zeros(nst), "rotations": np.zeros(9 * mc), "sys_not_pd": np.zeros(K, np.int32)}
+        for k in ("sigx", "rrow", "w2", "Adx", "du", "dl1", "dl2", "w", "wb"):
+            r[k] = np.zeros(nr)
+        out = RotavgL1StepOut(**{k: v.ctypes.data for k, v in r.items()})
+        self._check(lib().r3d_debug_rotavg_l1_step(self._h, _p(rel), C.c_uint64(len(rel)), C.c_uint32(n_views), C.byref(o),
+                                                   None if rot is None else _p(rot), C.c_int(kind),
+                                                   None if x is None else _p(x), C.c_uint64(0 if x is None else len(x)),
+                                                   C.c_double(tau), None if wt is None else _p(wt), None if rh is None else _p(rh),
+                                                   C.c_uint32(K), C.byref(out)))
+        m, E = out.n_kept_views, out.n_kept_edges
+        n = max(m, 1) - 1
+        nr, nv = 3 * E, 3 * n
+
+        def unpack(v):
+            o1 = [0, nv, nv + nr, nv + 2 * nr, nv + 3 * nr, nv + 4 * nr, 2 * nv + 4 * nr]
+            return tuple(v[o1[i]:o1[i + 1]].copy() for i in range(6))
+
+        d = {"m": m, "E": E, "n": n, "view_ids": r["view_ids"][:m].copy(), "ab": r["ab"][:2 * E].reshape(E, 2).astype(np.int64),
+             "Rk": r["Rk"][:9 * E].reshape(E, 3, 3).copy(), "rotations0": r["rotations0"][:9 * m].reshape(m, 3, 3).copy(),
+             "b": r["b"][:nr].copy(), "cost": r["cost"][:E].copy(), "bmax": out.bmax, "b_zero": bool(out.b_zero),
+             "not_pd": bool(out.not_pd), "rotations": r["rotations"][:9 * m].reshape(m, 3, 3).copy(), "xmax": out.xmax}
+        lap = 3 * (n + 1) * n
+        if kind == 2:
+            d["laplacians"] = r["laplacians"][:K * lap].reshape(K, 3, n + 1, n).copy()
+            d["dx"] = r["dx"][:K * nv].reshape(K, nv).copy()
+            d["sys_not_pd"] = r["sys_not_pd"].astype(bool)
+            return d
+        d["laplacians"] = r["laplacians"][:lap].reshape(3, n + 1, n).copy()
+        d["dx"] = r["dx"][:nv].copy()
+        if kind == 1:
+            d.update(w=r["w"][:nr].copy(), wb=r["wb"][:nr].copy())
+            return d
+        d.update(state0=unpack(r["state0"]), state=unpack(r["state"]), sdg0=out.sdg0, tau0=out.tau0, resnorm0=out.resnorm0,
+                 step_max=out.step_max, trials=[(out.trial_step[t], out.trial_resnorm[t]) for t in range(out.n_trials)],
+                 accepted=bool(out.accepted), sdg=out.sdg, tau=out.tau, resnorm=out.resnorm)
+        for k in ("sigx", "rrow", "w2", "Adx", "du", "dl1", "dl2"):
+            d[k] = r[k][:nr].copy()
+        d.update(Atdv=r["Atdv"][:nv].copy(), rmin=r["rmin"][:E].copy())
+        return d
 
     def translation_averaging(self, rel, rotations, rot_kept, n_views, method=TRANSAVG_L2_CHORDAL, edge_use=None,
                               softl1_loss=0.01, **lm):

@@ -297,6 +297,12 @@ std::vector<double> spanning_tree_start(const ra::KeptComponent& K) {
   return R;
 }
 
+// what r3d_debug_rotavg_l1_step reads back from inside the solver's members (none in rotation_averaging_l1)
+struct Trace {
+  double* A3 = nullptr;                // 3 (n + 1) n: the systems of each solve as assembled, before they are factored
+  std::vector<double> step, resnorm;   // per trial step of the line search: the step and the trial's residual norm
+};
+
 // the device side of one call on the kept component
 struct Solver {
   r3d_ctx* ctx;
@@ -312,6 +318,7 @@ struct Solver {
   int cur = 0;
   // 0 not-positive-definite flag, 1 max|b|, 2 min step ratio, 3 residual norm^2, 4 sum fu^T lambda, 5 max|x|, 6 cost
   double h[8] = {};
+  Trace* tr = nullptr;
 
   Solver(r3d_ctx* c, DeviceWorker& wk, const ra::KeptComponent& K)
       : ctx(c), w(wk), m((uint32_t)K.kview.size()), ne((uint32_t)K.kab.size()), n(m - 1), nr(3 * ne), nv(3 * (m - 1)),
@@ -371,6 +378,8 @@ struct Solver {
     R3D_CUDA_TRY(ctx, cudaMemsetAsync(d_scal.p, 0, sizeof(double), w.stream));
     k_l1_system<<<n, 128, 0, w.stream>>>(d_iofs.p, d_inbr.p, d_iedge.p, d_ab.p, wt, v, n, mstride, d_A3.p);
     R3D_CUDA_TRY(ctx, cudaGetLastError());
+    if (tr && tr->A3)
+      R3D_CUDA_TRY(ctx, cudaMemcpyAsync(tr->A3, d_A3.p, 3 * mstride * sizeof(double), cudaMemcpyDeviceToHost, w.stream));
     int rc;
     for (int k = 0; k < 3; ++k)
       if ((rc = dense_cholesky(ctx, w, d_A3.p + k * mstride, d_L.p, d_Linv.p, (int)n, d_scal.p, d_dx.p + (size_t)k * n))) return rc;
@@ -388,58 +397,105 @@ struct Solver {
     return read();
   }
 
+  // l1decode_pd's start on the residuals in d_b (max |b| in h[1]): S[cur].x = 0, then, unless b = 0 (*zero: x = 0 is
+  // the solution), k_l1_pd_start's point in S[cur] with its surrogate duality gap sdg, tau and residual norm
+  int pd_start(bool* zero, double& sdg, double& tau, double& resnorm) {
+    PdState& s0 = S[cur];
+    R3D_CUDA_TRY(ctx, cudaMemsetAsync(s0.x, 0, nv * sizeof(double), w.stream));
+    *zero = h[1] == 0.0;
+    if (*zero) return R3D_OK;
+    k_l1_pd_start<<<blocks(nr), 128, 0, w.stream>>>(d_b.p, d_scal.p + 1, nr, s0, d_dv.p);
+    k_l1_at<<<blocks(nv), 128, 0, w.stream>>>(d_iofs.p, d_iedge.p, d_ab.p, d_dv.p, n, s0.Atv);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    int rc;
+    if ((rc = norms(cur, 0.0))) return rc;
+    sdg = -h[4];
+    tau = kPdMu * (2.0 * (double)nr) / sdg;
+    if ((rc = norms(cur, 1.0 / tau))) return rc;
+    resnorm = std::sqrt(h[3]);
+    return R3D_OK;
+  }
+
+  // One Newton iteration of l1decode_pd from S[cur] at tau, whose residual norm there is resnorm: the Newton system,
+  // the direction, the ratio test (min step ratio in h[2]) and the backtracking line search.  Accepted: S[cur] becomes
+  // the trial point and sdg, tau, resnorm its values; else *stuck and S[cur] is unchanged.  *not_pd: the Newton system
+  // was not positive definite (nothing after the solve ran).
+  int pd_iteration(double& sdg, double& tau, double& resnorm, uint32_t* backtracks, bool* not_pd, bool* stuck) {
+    *stuck = false;
+    const double tinv = 1.0 / tau;
+    const PdState& s = S[cur];
+    k_l1_newton<<<blocks(nr), 128, 0, w.stream>>>(d_b.p, s, nr, tinv, d_sigx.p, d_rrow.p, d_w2.p);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    int rc;
+    if ((rc = solve(d_sigx.p, d_rrow.p, not_pd))) return rc;
+    if (*not_pd) return R3D_OK;
+    k_l1_direction<<<blocks(ne), 128, 0, w.stream>>>(d_ab.p, d_b.p, s, d_w2.p, d_dx.p, ne, n, tinv, D, d_dv.p, d_rmin.p);
+    k_l1_at<<<blocks(nv), 128, 0, w.stream>>>(d_iofs.p, d_iedge.p, d_ab.p, d_dv.p, n, d_Atdv.p);
+    reduce(2, d_rmin.p, ne, 2);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    if ((rc = read())) return rc;
+    double step = 0.99 * h[2];
+    bool ok = false;
+    for (int bt = 0; bt <= kPdMaxBacktracks; ++bt) {
+      k_l1_trial<<<blocks(std::max(nr, nv)), 128, 0, w.stream>>>(s, D, d_dx.p, d_Atdv.p, nr, nv, step, S[1 - cur]);
+      R3D_CUDA_TRY(ctx, cudaGetLastError());
+      if ((rc = norms(1 - cur, tinv))) return rc;
+      if (tr) {
+        tr->step.push_back(step);
+        tr->resnorm.push_back(std::sqrt(h[3]));
+      }
+      if (std::sqrt(h[3]) <= (1.0 - kPdAlpha * step) * resnorm) {
+        ok = true;
+        break;
+      }
+      ++*backtracks;
+      step = kPdBeta * step;
+    }
+    if (!ok) {
+      *stuck = true;
+      return R3D_OK;
+    }
+    cur = 1 - cur;
+    sdg = -h[4];
+    tau = kPdMu * (2.0 * (double)nr) / sdg;
+    if ((rc = norms(cur, 1.0 / tau))) return rc;
+    resnorm = std::sqrt(h[3]);
+    return R3D_OK;
+  }
+
   // l1decode_pd on the residuals in d_b (max |b| in h[1]); the solution is S[cur].x.  *not_pd: a Newton system was not
   // positive definite.
   int l1_regression(uint32_t* iters, uint32_t* backtracks, bool* not_pd) {
     *not_pd = false;
-    PdState& s0 = S[cur];
-    R3D_CUDA_TRY(ctx, cudaMemsetAsync(s0.x, 0, nv * sizeof(double), w.stream));
-    if (h[1] == 0.0) return R3D_OK;  // b = 0: x = 0
-    k_l1_pd_start<<<blocks(nr), 128, 0, w.stream>>>(d_b.p, d_scal.p + 1, nr, s0, d_dv.p);
-    k_l1_at<<<blocks(nv), 128, 0, w.stream>>>(d_iofs.p, d_iedge.p, d_ab.p, d_dv.p, n, s0.Atv);
-    R3D_CUDA_TRY(ctx, cudaGetLastError());
-    const double M2 = 2.0 * (double)nr;
+    bool zero = false, stuck = false;
+    double sdg = 0.0, tau = 0.0, resnorm = 0.0;
     int rc;
-    if ((rc = norms(cur, 0.0))) return rc;
-    double sdg = -h[4];
-    double tau = kPdMu * M2 / sdg;
-    if ((rc = norms(cur, 1.0 / tau))) return rc;
-    double resnorm = std::sqrt(h[3]);
+    if ((rc = pd_start(&zero, sdg, tau, resnorm))) return rc;
+    if (zero) return R3D_OK;
     for (int it = 0; !(sdg < kPdTol || it >= kPdMaxIter);) {
       ++it;
       ++*iters;
-      const double tinv = 1.0 / tau;
-      const PdState& s = S[cur];
-      k_l1_newton<<<blocks(nr), 128, 0, w.stream>>>(d_b.p, s, nr, tinv, d_sigx.p, d_rrow.p, d_w2.p);
-      R3D_CUDA_TRY(ctx, cudaGetLastError());
-      if ((rc = solve(d_sigx.p, d_rrow.p, not_pd))) return rc;
-      if (*not_pd) return R3D_OK;
-      k_l1_direction<<<blocks(ne), 128, 0, w.stream>>>(d_ab.p, d_b.p, s, d_w2.p, d_dx.p, ne, n, tinv, D, d_dv.p, d_rmin.p);
-      k_l1_at<<<blocks(nv), 128, 0, w.stream>>>(d_iofs.p, d_iedge.p, d_ab.p, d_dv.p, n, d_Atdv.p);
-      reduce(2, d_rmin.p, ne, 2);
-      R3D_CUDA_TRY(ctx, cudaGetLastError());
-      if ((rc = read())) return rc;
-      double step = 0.99 * h[2];
-      bool ok = false;
-      for (int bt = 0; bt <= kPdMaxBacktracks; ++bt) {
-        k_l1_trial<<<blocks(std::max(nr, nv)), 128, 0, w.stream>>>(s, D, d_dx.p, d_Atdv.p, nr, nv, step, S[1 - cur]);
-        R3D_CUDA_TRY(ctx, cudaGetLastError());
-        if ((rc = norms(1 - cur, tinv))) return rc;
-        if (std::sqrt(h[3]) <= (1.0 - kPdAlpha * step) * resnorm) {
-          ok = true;
-          break;
-        }
-        ++*backtracks;
-        step = kPdBeta * step;
-      }
-      if (!ok) break;  // stuck: the last iterate
-      cur = 1 - cur;
-      sdg = -h[4];
-      tau = kPdMu * M2 / sdg;
-      if ((rc = norms(cur, 1.0 / tau))) return rc;
-      resnorm = std::sqrt(h[3]);
+      if ((rc = pd_iteration(sdg, tau, resnorm, backtracks, not_pd, &stuck))) return rc;
+      if (*not_pd || stuck) break;  // stuck: the last iterate
     }
     return R3D_OK;
+  }
+
+  // One IRLS iteration at the current rotations: the residuals, the Geman-McClure weights w (d_sigx) and w b (d_rrow)
+  // with s2 = sigma^2, the weighted normal equations and R <- R exp(dx) (max |dx| in h[5]).  *not_pd: the system was not
+  // positive definite (nothing after the solve ran).
+  int irls_iteration(double s2, bool* not_pd) {
+    int rc;
+    if ((rc = residuals())) return rc;
+    k_l1_irls<<<blocks(nr), 128, 0, w.stream>>>(d_b.p, nr, s2, d_sigx.p, d_rrow.p);
+    R3D_CUDA_TRY(ctx, cudaGetLastError());
+    if ((rc = solve(d_sigx.p, d_rrow.p, not_pd))) return rc;
+    if (*not_pd) return R3D_OK;
+    return rotate(d_dx.p);
+  }
+  static double irls_s2(const r3d_rotavg_l1_options& opt) {
+    const double sg = opt.irls_sigma_deg * (R3D_PI / 180.0);
+    return sg * sg;
   }
 
   // R <- R exp(x) with x = the current solution; max |x| into h[5]
@@ -506,18 +562,13 @@ int rotation_averaging_l1(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
   // ---- IRLS ----
   if (term != 2 && opt.irls_max_iterations > 0) {
     term = 1;
-    const double sg = opt.irls_sigma_deg * (R3D_PI / 180.0);
-    const double s2 = sg * sg;
+    const double s2 = Solver::irls_s2(opt);
     for (int it = 0; it < opt.irls_max_iterations; ++it) {
-      if ((rc = L.residuals())) return rc;
-      k_l1_irls<<<Solver::blocks(L.nr), 128, 0, w.stream>>>(L.d_b.p, L.nr, s2, L.d_sigx.p, L.d_rrow.p);
-      R3D_CUDA_TRY(ctx, cudaGetLastError());
-      if ((rc = L.solve(L.d_sigx.p, L.d_rrow.p, &not_pd))) return rc;
+      if ((rc = L.irls_iteration(s2, &not_pd))) return rc;
       if (not_pd) {
         term = 2;
         break;
       }
-      if ((rc = L.rotate(L.d_dx.p))) return rc;
       ++S.irls_iterations;
       if (L.h[5] <= opt.tolerance) {
         term = 0;
@@ -539,6 +590,149 @@ int rotation_averaging_l1(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n
   S.ms_device_total = S.ms_triplets + S.ms_l1 + S.ms_irls;
   S.ms_host = now_ms() - t0 - S.ms_device_total;
   return R3D_OK;
+}
+
+// r3d_debug_rotavg_l1_step: one step of the members above on the kept component
+int debug_step(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views, const r3d_rotavg_l1_options& opt,
+               const double* rotations, int kind, const double* state, uint64_t n_state, double tau_in, const double* weights,
+               const double* rhs, uint32_t n_systems, r3d_rotavg_l1_step_out& O) {
+  const char* fn = "r3d_debug_rotavg_l1_step: ";
+  DeviceWorker& w = ctx->workers[0];
+  R3D_CUDA_TRY(ctx, cudaSetDevice(w.device));
+  std::vector<uint8_t> vk(std::max(n_views, 1u));
+  ra::KeptComponent K;
+  int rc = ra::select_component(ctx, fn, rel, n_rel, n_views, opt.max_angular_error_deg, vk.data(), nullptr, nullptr, K);
+  if (rc) return rc;
+  if (K.kview.empty()) return R3D_OK;
+  const uint32_t m = (uint32_t)K.kview.size(), ne = (uint32_t)K.kab.size(), n = m - 1;
+  const size_t nr = 3 * (size_t)ne, nv = 3 * (size_t)n, nst = 4 * nr + 2 * nv;
+  if (kind == 0 && state && n_state != nst) return fail(ctx, R3D_ERR_INVALID, std::string(fn) + "the state must hold 12 E + 6 n values");
+  if (kind == 0 && state && !(std::isfinite(tau_in) && tau_in > 0.0)) return fail(ctx, R3D_ERR_INVALID, std::string(fn) + "tau <= 0");
+  std::vector<double> R0;
+  if (!rotations) {
+    R0 = spanning_tree_start(K);
+  } else {
+    R0.resize(9 * (size_t)m);
+    for (uint32_t a = 0; a < m; ++a) std::memcpy(&R0[9 * (size_t)a], rotations + 9 * (size_t)K.kview[a], 9 * sizeof(double));
+    for (double v : R0)
+      if (!std::isfinite(v)) return fail(ctx, R3D_ERR_INVALID, std::string(fn) + "non-finite rotations");
+  }
+  O.n_kept_views = m;
+  O.n_kept_edges = ne;
+  for (uint32_t a = 0; a < m; ++a)
+    if (O.view_ids) O.view_ids[a] = K.kview[a];
+  for (uint32_t e = 0; e < ne; ++e)
+    if (O.ab) {
+      O.ab[2 * (size_t)e] = K.kab[e].x;
+      O.ab[2 * (size_t)e + 1] = K.kab[e].y;
+    }
+  if (O.Rk) std::memcpy(O.Rk, K.kR.data(), K.kR.size() * sizeof(double));
+  if (O.rotations0) std::memcpy(O.rotations0, R0.data(), R0.size() * sizeof(double));
+  Solver L(ctx, w, K);
+  if ((rc = L.init(K, R0))) return rc;
+  Trace T;
+  auto d2h = [&](void* dst, const void* src, size_t bytes) -> int {
+    if (dst) R3D_CUDA_TRY(ctx, cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, w.stream));
+    return R3D_OK;
+  };
+  auto sync = [&]() -> int {
+    R3D_CUDA_TRY(ctx, cudaStreamSynchronize(w.stream));
+    return R3D_OK;
+  };
+  auto residual_out = [&]() -> int {
+    O.bmax = L.h[1];
+    if ((rc = d2h(O.b, L.d_b.p, nr * sizeof(double))) || (rc = d2h(O.cost, L.d_cost.p, ne * sizeof(double)))) return rc;
+    return sync();
+  };
+  auto rotations_out = [&]() -> int {
+    O.xmax = L.h[5];
+    if ((rc = d2h(O.rotations, L.d_R.p, 9 * (size_t)m * sizeof(double)))) return rc;
+    return sync();
+  };
+  const size_t lap = 3 * L.mstride;
+  if (kind == 1) {
+    T.A3 = O.laplacians;
+    L.tr = &T;
+    bool not_pd = false;
+    if ((rc = L.irls_iteration(Solver::irls_s2(opt), &not_pd)) || (rc = residual_out())) return rc;
+    O.not_pd = not_pd;
+    if ((rc = d2h(O.w, L.d_sigx.p, nr * sizeof(double))) || (rc = d2h(O.wb, L.d_rrow.p, nr * sizeof(double)))) return rc;
+    if (not_pd) return sync();
+    if ((rc = d2h(O.dx, L.d_dx.p, nv * sizeof(double)))) return rc;
+    return rotations_out();
+  }
+  if ((rc = L.residuals()) || (rc = residual_out())) return rc;
+  if (kind == 2) {
+    for (uint32_t q = 0; q < n_systems; ++q) {
+      T.A3 = O.laplacians ? O.laplacians + q * lap : nullptr;
+      L.tr = &T;
+      R3D_CUDA_TRY(ctx, L.h2d(L.d_sigx.p, weights + q * nr, nr * sizeof(double)));
+      R3D_CUDA_TRY(ctx, L.h2d(L.d_rrow.p, rhs + q * nr, nr * sizeof(double)));
+      bool not_pd = false;
+      if ((rc = L.solve(L.d_sigx.p, L.d_rrow.p, &not_pd))) return rc;
+      if (O.sys_not_pd) O.sys_not_pd[q] = not_pd;
+      if (!not_pd && O.dx && (rc = d2h(O.dx + q * nv, L.d_dx.p, nv * sizeof(double)))) return rc;
+    }
+    return sync();
+  }
+  // kind 0
+  double sdg = 0.0, tau = 0.0, resnorm = 0.0;
+  if (!state) {
+    bool zero = false;
+    if ((rc = L.pd_start(&zero, sdg, tau, resnorm))) return rc;
+    if (zero) {
+      O.b_zero = 1;
+      if ((rc = L.rotate(L.S[L.cur].x))) return rc;
+      return rotations_out();
+    }
+  } else {
+    std::vector<double> bh(nr);
+    if ((rc = d2h(bh.data(), L.d_b.p, nr * sizeof(double))) || (rc = sync())) return rc;
+    for (size_t i = 0; i < nst; ++i)
+      if (!std::isfinite(state[i])) return fail(ctx, R3D_ERR_INVALID, std::string(fn) + "a non-finite state");
+    const double *Ax = state + nv, *u = Ax + nr, *l1 = u + nr, *l2 = l1 + nr;
+    for (size_t i = 0; i < nr; ++i) {
+      const double f1 = (Ax[i] - bh[i]) - u[i], f2 = (-Ax[i] + bh[i]) - u[i];
+      if (!(f1 < 0.0) || !(f2 < 0.0) || !(l1[i] > 0.0) || !(l2[i] > 0.0))
+        return fail(ctx, R3D_ERR_INVALID, std::string(fn) + "u or lambda outside the interior");
+    }
+    R3D_CUDA_TRY(ctx, L.h2d(L.d_st[L.cur].p, state, nst * sizeof(double)));
+    tau = tau_in;
+    if ((rc = L.norms(L.cur, 1.0 / tau))) return rc;
+    sdg = -L.h[4];
+    resnorm = std::sqrt(L.h[3]);
+  }
+  O.sdg0 = sdg;
+  O.tau0 = tau;
+  O.resnorm0 = resnorm;
+  if ((rc = d2h(O.state0, L.d_st[L.cur].p, nst * sizeof(double)))) return rc;
+  T.A3 = O.laplacians;
+  L.tr = &T;
+  uint32_t backtracks = 0;
+  bool not_pd = false, stuck = false;
+  if ((rc = L.pd_iteration(sdg, tau, resnorm, &backtracks, &not_pd, &stuck))) return rc;
+  O.not_pd = not_pd;
+  if ((rc = d2h(O.sigx, L.d_sigx.p, nr * sizeof(double))) || (rc = d2h(O.rrow, L.d_rrow.p, nr * sizeof(double))) ||
+      (rc = d2h(O.w2, L.d_w2.p, nr * sizeof(double))))
+    return rc;
+  if (not_pd) return sync();
+  O.step_max = L.h[2];
+  O.n_trials = (uint32_t)T.step.size();
+  for (uint32_t t = 0; t < O.n_trials; ++t) {
+    O.trial_step[t] = T.step[t];
+    O.trial_resnorm[t] = T.resnorm[t];
+  }
+  O.accepted = !stuck;
+  O.sdg = sdg;
+  O.tau = tau;
+  O.resnorm = resnorm;
+  if ((rc = d2h(O.dx, L.d_dx.p, nv * sizeof(double))) || (rc = d2h(O.Adx, L.D.Adx, nr * sizeof(double))) ||
+      (rc = d2h(O.du, L.D.du, nr * sizeof(double))) || (rc = d2h(O.dl1, L.D.dl1, nr * sizeof(double))) ||
+      (rc = d2h(O.dl2, L.D.dl2, nr * sizeof(double))) || (rc = d2h(O.Atdv, L.d_Atdv.p, nv * sizeof(double))) ||
+      (rc = d2h(O.rmin, L.d_rmin.p, ne * sizeof(double))) || (rc = d2h(O.state, L.d_st[L.cur].p, nst * sizeof(double))))
+    return rc;
+  if ((rc = L.rotate(L.S[L.cur].x))) return rc;
+  return rotations_out();
 }
 
 }  // namespace rl
@@ -566,4 +760,24 @@ extern "C" int r3d_rotation_averaging_l1(r3d_ctx* ctx, const r3d_relative_pose* 
   if (opt->l1_max_iterations < 1 || opt->irls_max_iterations < 0 || !(opt->tolerance > 0.0) || !(opt->irls_sigma_deg > 0.0))
     return fail(ctx, R3D_ERR_INVALID, "r3d_rotation_averaging_l1: an iteration cap below its minimum, or tolerance / sigma <= 0");
   return rl::rotation_averaging_l1(ctx, rel, n_rel, n_views, *opt, rotations, view_kept, edge_kept, edge_support, *summary);
+}
+
+extern "C" int r3d_debug_rotavg_l1_step(r3d_ctx* ctx, const r3d_relative_pose* rel, uint64_t n_rel, uint32_t n_views,
+                                        const r3d_rotavg_l1_options* opt, const double* rotations, int kind, const double* state,
+                                        uint64_t n_state, double tau, const double* weights, const double* rhs, uint32_t n_systems,
+                                        r3d_rotavg_l1_step_out* out) {
+  static_assert(sizeof(out->trial_step) / sizeof(double) == rl::kPdMaxBacktracks + 1, "one slot per trial step");
+  if (!ctx || (!rel && n_rel) || !opt || kind < 0 || kind > 2 || (!state && n_state) || (kind != 0 && state) ||
+      (kind == 2 && (!weights || !rhs || n_systems < 1)) || !out)
+    return fail(ctx, R3D_ERR_INVALID, "r3d_debug_rotavg_l1_step: bad arguments");
+  if (!(opt->max_angular_error_deg > 0.0) || !(opt->irls_sigma_deg > 0.0))
+    return fail(ctx, R3D_ERR_INVALID, "r3d_debug_rotavg_l1_step: max_angular_error_deg or irls_sigma_deg <= 0");
+  r3d_rotavg_l1_step_out& O = *out;
+  O.n_kept_views = O.n_kept_edges = 0;
+  O.bmax = O.sdg0 = O.tau0 = O.resnorm0 = O.step_max = O.sdg = O.tau = O.resnorm = O.xmax = 0.0;
+  O.b_zero = O.not_pd = O.accepted = 0;
+  O.n_trials = 0;
+  std::memset(O.trial_step, 0, sizeof(O.trial_step));
+  std::memset(O.trial_resnorm, 0, sizeof(O.trial_resnorm));
+  return rl::debug_step(ctx, rel, n_rel, n_views, *opt, rotations, kind, state, n_state, tau, weights, rhs, n_systems, O);
 }

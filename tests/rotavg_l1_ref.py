@@ -112,11 +112,14 @@ def solve_laplacians(ab, w, rhs, m):
 
 
 # ---- l1decode_pd on the graph matrix ---------------------------------------------------------------------------------
-def l1_regression(ab, b, m, pdtol=PD_TOL, pdmaxiter=PD_MAX_ITER):
+def l1_regression(ab, b, m, pdtol=PD_TOL, pdmaxiter=PD_MAX_ITER, trace=None):
     """x = argmin |A x - b|_1 (x (m, 3), row 0 = 0) by l1-magic's primal-dual method on min sum u s.t. -u <= A x - b <= u,
     from x = 0, u = 0.95 |b| + 0.1 max |b|.  Returns (x, stats): iterations, backtracks (rejected trial steps), sdg
     (the final surrogate duality gap), stuck (a Newton step found no sufficient decrease in PD_MAX_BACKTRACKS halvings:
-    the last iterate is returned).  b all zero: x = 0 without iterations.  Raises FactorizationError."""
+    the last iterate is returned).  b all zero: x = 0 without iterations.  Raises FactorizationError.  trace: called
+    once per Newton iteration with a dict of the state it started from (x, u, Ax, Atv, lam1, lam2, tau), its direction
+    (dx, du, Adx, dlam1, dlam2, Atdv), the trial steps and whether the last was accepted (the tests take states and
+    steps from it)."""
     ab = np.asarray(ab, np.int64)
     b = np.asarray(b, np.float64).reshape(-1, 3)
     M = b.size
@@ -168,7 +171,9 @@ def l1_regression(ab, b, m, pdtol=PD_TOL, pdmaxiter=PD_MAX_ITER):
             if pos.any():
                 s = min(s, (-f[pos] / d[pos]).min())
         s = 0.99 * s
+        steps = []
         for _ in range(PD_MAX_BACKTRACKS + 1):
+            steps.append(s)
             xp = x + s * dx
             up = u + s * du
             Axp = Ax + s * Adx
@@ -183,6 +188,10 @@ def l1_regression(ab, b, m, pdtol=PD_TOL, pdmaxiter=PD_MAX_ITER):
             s = PD_BETA * s
         else:
             st["stuck"] = True
+        if trace is not None:
+            trace(dict(x=x, u=u, Ax=Ax, Atv=Atv, lam1=lam1, lam2=lam2, tau=tau, dx=dx, du=du, Adx=Adx, dlam1=dlam1,
+                       dlam2=dlam2, Atdv=Atdv, steps=steps, accepted=not st["stuck"]))
+        if st["stuck"]:
             break
         x, u, Ax, Atv, lam1, lam2, fu1, fu2 = xp, up, Axp, Atvp, lam1p, lam2p, fu1p, fu2p
         sdg = -((fu1 * lam1).sum() + (fu2 * lam2).sum())
